@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 blob-ingest / content-hash path.
+"""bench.py -- headline benchmark of the H100 blob-ingest / content-hash path.
 
 Workload (BASELINE.json configs[1]): the Function.map input pump -- 100 000 pickled inputs of
 256 KiB each (24.4 GiB), fused SHA-256 + MD5 per payload -- per GPU (weak scaling; payload sets are
@@ -11,8 +11,13 @@ independent, no data-path collective; the per-rank digest tables are all-gathere
             input -> parallel_map.InputPumper, against a null control plane / object store
   e2e_pinned  the same payloads through batch.hash_table_host on page-locked host memory (round 1's e2e figure)
   roofline  lane_hash_kernel: algorithmic bytes / measured kernel time vs the measured HBM copy peak
-  cpu_baseline  the reference's own get_upload_hashes (unmodified hash_utils.py from baseline/_ref through
-            oracle/ref_shim.py; oracle/ref_port.py only if that copy is missing) on the host cores, bounded sample
+  cpu_baseline  the reference's get_upload_hashes on the host cores, bounded sample: its unmodified hash_utils.py
+            through oracle/ref_shim.py when B200H_REFERENCE_ROOT names a checkout, else the hashlib port in
+            oracle/ref_port.py (the same hashlib calls)
+
+`--dump-outputs DIR` writes the digest table of the last timed HBM-resident step as DIR/sha256.npy (float32[n, 32])
+and DIR/md5.npy (float32[n, 16]), one byte per element (rank 0's table).  The payloads come from a fixed seed, so two
+builds run with the same arguments can be compared output for output.
 
 `--impl reference` times that same reference implementation (hashlib underneath, all host threads) on the same
 workload shape and prints the same JSON line.
@@ -44,7 +49,7 @@ def hbm_peak_gbs() -> tuple[float, str]:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback: NVIDIA H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -118,9 +123,9 @@ _REF = None
 
 
 def reference_hasher():
-    """(callable, kind): the reference's OWN ``get_upload_hashes`` (unmodified hash_utils.py from baseline/_ref or
-    /root/reference, loaded through oracle/ref_shim.py) -> kind "reference"; if no copy travelled, the hashlib
-    port in oracle/ref_port.py -> kind "port".  Both make exactly the same hashlib calls."""
+    """(callable, kind): the reference's OWN ``get_upload_hashes`` (unmodified hash_utils.py of the checkout named by
+    B200H_REFERENCE_ROOT, loaded through oracle/ref_shim.py) -> kind "reference"; without one, the hashlib port in
+    oracle/ref_port.py -> kind "port".  Both make exactly the same hashlib calls."""
     global _REF
     if _REF is None:
         from oracle import ref_port, ref_shim  # allowed here: CPU baseline / reference arm only
@@ -274,6 +279,16 @@ def run_map_pump(payloads, stub) -> float:
     return asyncio.run(main())
 
 
+def dump_outputs(out_dir: str, sha, md5) -> None:
+    """Digest table of one step as out_dir/sha256.npy (float32[n, 32]) and out_dir/md5.npy (float32[n, 16]), one byte
+    per element."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "sha256.npy"), np.asarray(sha, np.uint8).reshape(-1, 32).astype(np.float32))
+    np.save(os.path.join(out_dir, "md5.npy"), np.asarray(md5, np.uint8).reshape(-1, 16).astype(np.float32))
+
+
 def run_gpu(args) -> None:
     import numpy as np
     import torch
@@ -386,7 +401,7 @@ def run_gpu(args) -> None:
     del data
     torch.cuda.empty_cache()
     off_h = (np.arange(N_MSG, dtype=np.uint64) * np.uint64(MSG_BYTES))
-    e2e_steps = max(1, min(args.steps, 3))
+    e2e_steps = args.steps
     e2e_warm = max(1, min(args.warmup, 3))
 
     def all_gather_host_table(packed: np.ndarray):
@@ -493,16 +508,13 @@ def run_gpu(args) -> None:
                "serial_note": "one thread, as the reference's map pump really runs it (blob_utils.py:345)",
                "host": host_description()}
 
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, sha_dev, md5_dev)
+
     if rank == 0:
         peak, peak_src = hbm_peak_gbs()
         kern_avg_ms = kern_ms / max(kern_n, 1)
         achieved = total_bytes / 1e9 / (kern_avg_ms / 1e3) if kern_n else None
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                traffic = json.load(f).get("lane_hash_kernel_dram_bytes_per_launch")
-        except Exception:
-            pass
         out = {
             "metric": METRIC, "value": round(value, 3), "unit": "GiB/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": round(ms / args.steps, 4), "higher_is_better": True, "scaling": "weak",
@@ -513,12 +525,10 @@ def run_gpu(args) -> None:
                                       "double buffered (gather k overlaps hash k+1)") if world > 1 else "none",
                        "host_syncs_in_timed_region": int(plan_syncs), "process_bound_to_gpu_numa_node": bool(numa_bound)},
             "roofline": {"bound": "hbm", "achieved": round(achieved, 1) if achieved else None, "peak": peak, "unit": "GB/s",
-                         "frac": round(achieved / peak, 4) if achieved else None, "traffic": traffic,
+                         "frac": round(achieved / peak, 4) if achieved else None,
                          "peak_source": peak_src, "kernel": "lane_hash_kernel<sha256,md5>",
                          "kernel_avg_ms": round(kern_avg_ms, 4), "kernel_launches_timed": kern_n,
-                         "int_alu_peak": 1018.0, "int_alu_frac": round(achieved / 1018.0, 4) if achieved else None,
-                         "note": "hbm frac per the contract; the binding limit is INT32 issue: 1168 ALU-pipe instr per "
-                                 "64 B block at 0.5 warp-instr/clk/SMSP x 592 SMSP x 1.965 GHz = 1018 GB/s (DESIGN.md 5.1)"},
+                         "note": "share of HBM bandwidth; SHA-256 + MD5 is bound by INT32 issue, not by HBM (DESIGN.md 5.1)"},
             "cpu_baseline": cpu,
             "e2e": {"value": round(pump_value, 3), "unit": "GiB/s", "h2d_bytes_per_step": total_bytes + 16 * N_MSG,
                     "d2h_bytes_per_step": 56 * N_MSG, "steps": e2e_steps,
@@ -550,7 +560,11 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's digest table as DIR/sha256.npy and DIR/md5.npy (float32)")
     args = ap.parse_args()
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs writes the GPU path's digest table; the reference arm has none")
     if args.impl == "reference":
         run_reference(args)
     else:

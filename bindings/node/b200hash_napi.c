@@ -30,7 +30,7 @@ static napi_value throw_error(napi_env env, const char* msg) {
 
 static int ensure_context(napi_env env) {
     if (g_ctx) return 1;
-    if (b200h_create(0, 0, 0, &g_ctx) != 0) { /* no CPU fallback: without a B200 the addon throws */
+    if (b200h_create(0, 0, 0, &g_ctx) != 0) { /* no CPU fallback: without an H100 the addon throws */
         throw_error(env, b200h_last_error(NULL));
         return 0;
     }

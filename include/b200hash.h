@@ -1,5 +1,5 @@
 /*
- * b200hash.h -- C ABI of libb200hash.so: batched SHA-256 + MD5 content hashing on NVIDIA B200 (sm_100a).
+ * b200hash.h -- C ABI of libb200hash.so: batched SHA-256 + MD5 content hashing on NVIDIA H100 (sm_90a).
  *
  * The reference (modal-labs/modal-client) has no FFI for this path: its seam is a set of Python
  * module-level functions that call hashlib.  Each entry point below names the reference call site(s)
@@ -134,7 +134,7 @@ int b200h_hash_files(b200h_ctx* ctx, const char* const* paths, uint64_t n, const
 
 /* Incremental digest of ONE message fed in arbitrary pieces with bounded memory; the chaining state
  * stays on the device between updates.  A single message is a serial Merkle-Damgard chain, so this is
- * latency-bound by construction (~70 MB/s per stream) -- use the batch entry points for throughput.
+ * latency-bound by construction (one GPU thread's speed per stream) -- use the batch entry points for throughput.
  * update() gathers into a pinned buffer and enqueues one absorb per 4 MiB (B200H_STREAM_BUF) without waiting
  * for it; every stream has its own CUDA stream and scratch, so N streams fed from N threads advance concurrently.
  * One stream object must not be used from two threads at once (like a hashlib object).

@@ -1,9 +1,9 @@
-"""modal_client_b200 -- B200-native blob-ingest / content-hash path behind the Modal client's function surface.
+"""modal_client_b200 -- H100-native blob-ingest / content-hash path behind the Modal client's function surface.
 
 Drop-in modules (same names as the reference's ``modal/_utils``): ``hash_utils``, ``blob_utils``,
-``bytes_io_segment_payload``, ``function_utils``, ``parallel_map``.  B200 additions: ``batch`` (digest
+``bytes_io_segment_payload``, ``function_utils``, ``parallel_map``.  Additions: ``batch`` (digest
 tables), ``sharding`` (multi-GPU), ``_lib`` (ctypes binding of libb200hash.so, C ABI in include/b200hash.h).
-All arithmetic runs in hand-written sm_100a CUDA; there is no CPU fallback.
+All arithmetic runs in hand-written sm_90a CUDA; there is no CPU fallback.
 """
 __version__ = "0.1.0"
 

@@ -1,8 +1,8 @@
 """ctypes binding of libb200hash.so (C ABI: include/b200hash.h).
 
-There is deliberately no CPU fallback in this package: if the shared library is missing, or no B200
+There is deliberately no CPU fallback in this package: if the shared library is missing, or no H100
 is visible, every entry point raises ``B200HashError``.  ``build_library()`` (re)builds the .so in-tree
-with nvcc for sm_100a (cross-compiles without a GPU).
+with nvcc for sm_90a (cross-compiles without a GPU).
 """
 from __future__ import annotations
 
@@ -68,7 +68,7 @@ def load_library() -> ctypes.CDLL:
         if not os.path.exists(LIB_PATH):
             raise B200HashError(
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  modal_client_b200 has no CPU fallback."
+                "(nvcc, sm_90a).  modal_client_b200 has no CPU fallback."
             )
         L = ctypes.CDLL(LIB_PATH)
         vp, u64, u32, i32, sz = ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_int, ctypes.c_size_t
@@ -149,7 +149,7 @@ def _np_ptr(a: np.ndarray | None):
     return None if a is None else ctypes.c_void_p(a.ctypes.data)
 
 
-def plan_preview(lengths, flags: int = SHA256 | MD5, sm_count: int = 148) -> tuple[int, int]:
+def plan_preview(lengths, flags: int = SHA256 | MD5, sm_count: int = 132) -> tuple[int, int]:
     """(messages routed to the chain kernel, messages in the long lane queue) for a batch with these lengths on a
     device with ``sm_count`` SMs -- the library's host-side planner (no context, no GPU needed)."""
     L = load_library()

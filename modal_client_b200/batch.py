@@ -1,4 +1,4 @@
-"""Batch front door of the B200 hash path: many independent messages in, one digest table out.
+"""Batch front door of the GPU hash path: many independent messages in, one digest table out.
 
 This is the call the accelerated callers make (map input pump, Volume.batch_upload v1/v2, multipart
 parts): the reference hashes one payload / file / block at a time with hashlib

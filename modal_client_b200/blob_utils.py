@@ -1,7 +1,7 @@
 """Drop-in for the hashing / chunking half of the reference's ``modal/_utils/blob_utils.py``.
 
 Same public names, size classes, thresholds and integrity checks as the reference
-(py/modal/_utils/blob_utils.py), with every digest produced by libb200hash on the B200:
+(py/modal/_utils/blob_utils.py), with every digest produced by libb200hash on the GPU:
 
 =============================  ===========================================================================
 reference (file:line)          here

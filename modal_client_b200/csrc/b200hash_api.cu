@@ -111,16 +111,16 @@ struct b200h_ctx {
     cudaStream_t s_copy = nullptr, s_comp = nullptr, s_chain = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     // Outlier path: the warp-specialised chain kernel (TMA tile ring + mbarriers; schedule expansion, SHA-256 rounds
-    // and MD5 on three warps of one CTA) runs ONE chain about twice as fast as a lane does (62 vs 30 MB/s fused),
+    // and MD5 on three warps of one CTA) runs ONE chain about twice as fast as a lane does,
     // at up to 4 CTAs per SM.  The planner (plan_scan_kernel) hands it only true outliers and only when all of
     // them fit in chain_cap CTAs; everything else stays on the lane kernel.  B200H_CHAIN=0 disables it, =N sets the cap.
     bool chain_enabled = true;
     // One chain CTA per SM, each hosting up to chain_groups_per_cta() messages (set from the SM count at create).
-    uint32_t chain_cap = 592;
-    uint32_t sm_count = 148;
+    uint32_t chain_cap = 528;
+    uint32_t sm_count = 132;
     // B200H_YIELD_CHAIN_SMS=1: CTAs of a full-grid lane launch leave the SMs that host chain CTAs.  Off by default:
-    // measured on one rank's share of C3 (profiles/r2_c3v2_probe.md) it moved nothing (309 vs 310 ms) -- the long pole
-    // there was the lane tail, not the chains -- and it must never be applied to a small grid (see launch_lane_hash).
+    // on one rank's share of C3 the long pole was the lane tail, not the chains -- and it must never be applied to a
+    // small grid (see launch_lane_hash).
     bool yield_chain_sms = false;
     int* h_plan = nullptr;        // pinned: the planner's control block {avail, head, tail, outliers} of the last batch
     uint32_t last_outliers = 0;
@@ -384,8 +384,7 @@ int enqueue_device_batch(b200h_ctx* ctx, const uint8_t* d_base, const uint64_t* 
     int* qctl_long = qctl + kLongQctlAfterQctl;
     // How many outliers did the planner pick?  The count is read back (16 bytes, one stream synchronisation after
     // the ~12 us plan kernels) because a chain kernel launched "just in case" is not free: its CTAs ask for half an
-    // SM's shared memory and, idle or not, skew where the lane kernel's CTAs land (1 024 x 8 MiB: 260 -> 937 ms,
-    // 2 048 x 4 MiB: 159 -> 280 ms measured with a speculative launch before / after the lane kernel).
+    // SM's shared memory and, idle or not, skew where the lane kernel's CTAs land.
     // So: lengths known on the host -> the same selection is computed here (plan_outliers_host); otherwise read back.
     // The same goes for the long lane queue (its launch is sized on the host as well).  A batch too small to have
     // either (nothing reaches kChainMinBlocks) needs no answer at all -- but only the host can know that.
@@ -515,8 +514,7 @@ void pack_range(const Source& src, const uint64_t* len, const uint64_t* doff, ui
 // and, under torchrun, the other ranks' teams.  (Build machine, a shared 8-core VM, scattered 256 KiB sources into
 // 256 MiB slots, best of three runs: two teams of 8 threads at once 44.6 -> 48.1 GiB/s, two teams of 16 39.6 -> 43.6,
 // two teams of 4 53.0 -> 55.5; a lone team of 8 swung between 12 and 24 GiB/s with the static split and 17 and 41 with
-// grains while a neighbour was busy;
-// profiles/r2_stream_copy_build_machine.txt.)  The threads are the context's PackTeam; the calling thread works too.
+// grains while a neighbour was busy.)  The threads are the context's PackTeam; the calling thread works too.
 void pack_parallel(PackTeam& team, int threads, const Source& src, const uint64_t* len, const uint64_t* doff, uint64_t i0,
                    uint64_t i1, uint64_t lo, uint64_t hi, uint8_t* dst, const cpu_set_t* cpus = nullptr) {
     const uint64_t bytes = hi - lo;
@@ -897,8 +895,8 @@ int b200h_create(int device, size_t pinned_bytes, size_t device_bytes, b200h_ctx
     CU_INIT(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU_INIT(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
-        ctx->err = "device is not Blackwell-class (kernels are built for sm_100a only)";
+    if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 and nothing else
+        ctx->err = "device is not an H100-class GPU (compute capability 9.0; kernels are built for sm_90a only)";
         return bail(B200H_E_CUDA);
     }
     CU_INIT(configure_kernels());
@@ -940,7 +938,7 @@ int b200h_create(int device, size_t pinned_bytes, size_t device_bytes, b200h_ctx
     // One process per GPU shares the host with its siblings.  The packers run on the GPU's NUMA node, so what a rank
     // may use is that node's CPUs divided by the ranks whose GPUs hang off the same node (LOCAL_WORLD_SIZE ranks spread
     // over the nodes), and a caller that keeps two batches in flight (the map pump) runs two packer teams at once:
-    // 8 ranks x 2 x 16 packers were 256 threads on 128 CPUs in the first 8-GPU run of the pump (profiles/r2_scaling.md).
+    // 8 ranks x 2 x 16 packers were 256 threads on 128 CPUs in an early 8-GPU run of the pump.
     unsigned share = ctx->node_cpus_valid ? (unsigned)CPU_COUNT(&ctx->node_cpus) : hc;
     if (const char* e = getenv("LOCAL_WORLD_SIZE")) {
         const int lw = atoi(e);
@@ -957,7 +955,7 @@ int b200h_create(int device, size_t pinned_bytes, size_t device_bytes, b200h_ctx
             share = std::max(4u, share / std::max(1u, per_node));
         }
     }
-    ctx->pack_threads = (int)std::min(16u, std::max(2u, share / 2));  // 16: measured best on 2x Xeon 8562Y+ (8..64 tried)
+    ctx->pack_threads = (int)std::min(16u, std::max(2u, share / 2));  // 16: best of 8..64 on a two-socket host
     if (const char* e = getenv("B200H_PACK_THREADS")) ctx->pack_threads = std::max(1, atoi(e));
     ctx->io_threads = (int)std::min(16u, std::max(1u, share));  // measured: 16 > 32 > 64 > 128 (kernel-side contention)
     if (const char* e = getenv("B200H_IO_THREADS")) ctx->io_threads = std::max(1, atoi(e));

@@ -98,7 +98,7 @@ int launch_dedupe(const void* d_keys, uint64_t n, uint32_t key_bytes, uint32_t* 
     if (d_ndistinct) cudaMemsetAsync(d_ndistinct, 0, sizeof(unsigned long long), st);
     if (n == 0) return 0;
     const int threads = 256;
-    const int blocks = (int)std::min<uint64_t>((n + threads - 1) / threads, 148ull * 8);
+    const int blocks = (int)std::min<uint64_t>((n + threads - 1) / threads, (uint64_t)device_sm_count() * 8);
     const uint32_t* k = static_cast<const uint32_t*>(d_keys);
     if (key_bytes == 32)
         dedupe_insert_kernel<8><<<blocks, threads, 0, st>>>(k, (uint32_t)n, table, table + cap, cap - 1, d_first);

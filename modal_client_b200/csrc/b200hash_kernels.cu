@@ -1,4 +1,4 @@
-// b200hash_kernels.cu -- hand-written sm_100a kernels for the blob-ingest / content-hash path.
+// b200hash_kernels.cu -- hand-written sm_90a (H100) kernels for the blob-ingest / content-hash path.
 //
 // Replaces the hashlib calls of the reference (py/modal/_utils/hash_utils.py:14-101,
 // blob_utils.py:640-705 and :216-219, bytes_io_segment_payload.py:58,102) with batched device
@@ -130,8 +130,7 @@ __device__ __forceinline__ uint32_t addv(uint32_t a, uint32_t b) {
 //                  round sum (one SHF less, one IMAD.WIDE + one IMAD more);
 //   bit 2:         the plain shifts of sigma0/sigma1 are IMAD.HI by 2^(32-n) (multiplier in a register so that
 //                  ptxas cannot turn it back into a shift).
-// Measured on B200 (100000 x 256 KiB, SHA-256 only): see profiles/r1_sha_only_rot.md.  The fused kernel does not
-// use it (its FMA pipe is already loaded with MD5's adds: -9 % there), IMAD.WIDE issues at 0.18/clk/SMSP.
+// The fused kernel does not use it: its FMA pipe is already loaded with MD5's adds.
 #ifndef B200H_SHAONLY_ROT
 #define B200H_SHAONLY_ROT 3
 #endif
@@ -266,7 +265,7 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     uint32_t w[16];
     uint32_t m14 = x[14], m15 = x[15];
     // multiplies add instructions: dense instantiations only.  B200H_FUSED_ROT (default 0) is the same knob for the fused
-    // kernel; measured in round 2 (profiles/r2_kernel_lever.md): bit 2 (sigma shifts as IMAD.HI) does not pay there either.
+    // kernel: bit 2 (sigma shifts as IMAD.HI) does not pay there either.
     constexpr int kShaRot = SPARSE ? 0 : (DO_MD5 ? (B200H_FUSED_ROT) : (B200H_SHAONLY_ROT));
     const uint32_t m29 = one << 29, m22 = one << 22;  // 2^29, 2^22 as run-time values (bit 2 of kShaRot)
     (void)m29; (void)m22;
@@ -412,8 +411,14 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
 
 // ------------------------------------------------------------------------------ lane_hash_kernel
 
+// CTAs per SM the lane kernel is compiled for.  H100 (100 000 x 256 KiB, kernel time): fused SHA-256 + MD5 at 5 CTAs
+// (96 registers, a few bytes of spill) beats 4 CTAs (128 registers, no spill) by 2-3 %; MD5 alone is the same either
+// way; SHA-256 alone gains 5 % at 4 CTAs, so that instantiation gets its own bound.
 #ifndef B200H_LANE_MIN_CTAS
-#define B200H_LANE_MIN_CTAS 5  // 20 warps/SM (96 registers/thread); 6 was measured 8% slower per block
+#define B200H_LANE_MIN_CTAS 5
+#endif
+#ifndef B200H_LANE_MIN_CTAS_SHA
+#define B200H_LANE_MIN_CTAS_SHA 4
 #endif
 constexpr int kLaneThreads = 128;  // 4 warps; every warp runs an independent TMA/mbarrier ring
 constexpr int kLaneWarps = kLaneThreads / 32;
@@ -457,12 +462,11 @@ __device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
 // boundary a warp whose lanes still hold unfinished messages puts them back on the queue *if other messages
 // are waiting* and pops the next ones, so n messages share S < n lanes evenly (no wave quantisation) and
 // mixed sizes balance like longest-first list scheduling.  Digest chaining state travels through st[].
-// (6 CTAs/SM was also tried for the MD5-only instantiation: 3.39 TB/s at full occupancy vs 3.42 at 5 -- no gain.)
 // SPARSE: instantiation for batches that leave every warp alone on its SMSP (<= 4 warps per SM): such a warp is
 // bound by its own issue rate (one instruction per two cycles), so the adds are left to ptxas (IADD3 / LEA fusion,
 // ~15 % fewer instructions per block) instead of being spread over the FMA pipe.
 template <bool DO_SHA, bool DO_MD5, bool SPARSE>
-__global__ void __launch_bounds__(kLaneThreads, B200H_LANE_MIN_CTAS)
+__global__ void __launch_bounds__(kLaneThreads, (DO_SHA && !DO_MD5) ? B200H_LANE_MIN_CTAS_SHA : B200H_LANE_MIN_CTAS)
 lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ off, const uint64_t* __restrict__ len,
                  uint32_t* __restrict__ ring, uint32_t ring_mask, int* __restrict__ qctl, const int* __restrict__ ctl,
                  uint32_t flags, int lanes_per_warp, uint32_t quantum, uint8_t* __restrict__ sha_out,
@@ -479,7 +483,7 @@ lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ 
     if (flags & F_YIELD_CHAIN_SMS) {
         // This SM hosts a chain CTA that carries one of the batch's longest messages: the chain's round warp issues at
         // most one instruction every two cycles and every lane warp next to it on the SMSP takes slots away from the
-        // one chain that sets the makespan (C3-v2, 93 chains + 12.5 GiB of lane work per GPU: 327 ms with shared SMs).
+        // one chain that sets the makespan.
         // The queue makes leaving free: whatever this CTA would have hashed is pulled by the CTAs on the other SMs.
         // The chain kernel is launched just before this one, on a high-priority stream, with at most one CTA per SM
         // on at most 3/4 of the SMs: its CTAs are resident within microseconds.  Wait for them (bounded: if they are
@@ -780,8 +784,7 @@ lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ 
 // w % 4 the twelve warps of a full CTA put exactly one expander, one SHA-256 and one MD5 warp on every SMSP.
 
 constexpr int kChainGroups = 4;     // messages per CTA by default (one expander, one SHA-256 and one MD5 warp per SMSP)
-constexpr int kChainGroupsMax = 8;  // B200H_CHAIN_GROUPS=8: twice that per SMSP -- measured: no gain over packed lanes (same code, more
-                                    // groups) except for MD5-only sets, profiles/r1_outlier_chain.md; off by default
+constexpr int kChainGroupsMax = 8;  // B200H_CHAIN_GROUPS=8: twice that per SMSP; off by default
 constexpr int kChainGroupThreads = 96;
 constexpr int kChainThreadsMax = kChainGroupThreads * kChainGroupsMax;
 constexpr int kTileBlocks = 32;
@@ -852,8 +855,8 @@ __device__ __forceinline__ void load_block_words(const uint8_t* blk, uint32_t to
 
 // MD5 block for the chain warp.  One chain on one warp is bound by the dependent-instruction latency of a step
 // (b -> F -> sum -> rotate -> + b), not by issue slots, so the step is written for the shortest dependency chain:
-// (x + T) off the critical path, one IADD3, and rotate+add left to ptxas as a single LEA.HI:
-// 1 204 -> 816 cycles per block (104 -> 154 MB/s, tools/chainbench.cu).
+// (x + T) off the critical path, one IADD3, and rotate+add left to ptxas as a single LEA.HI (tools/chainbench.cu
+// measures the cycles per block).
 // T[i] = floor(2^32 * |sin(i + 1)|) (RFC 1321); a switch so that the unrolled steps get immediates, not
 // constant-bank loads whose latency a lone warp cannot hide.
 __device__ __forceinline__ constexpr uint32_t md5_T(int i) {
@@ -1188,7 +1191,7 @@ chain_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__
 //                      trimmed[m] and gives up as soon as a later chunk of the same message has found a byte.
 //                      Long zero runs (blank volumefs2 blocks, sparse files) are therefore read by every SM at once
 //                      -- this is the one HBM-bound kernel on the path -- instead of by one warp walking 2 KiB per
-//                      dependent step (round 1: ~1 280 warps x 2 KiB in flight for 1 280 blank 8 MiB blocks).
+//                      dependent step (~1 280 warps x 2 KiB in flight for 1 280 blank 8 MiB blocks).
 
 constexpr int kTrimProbeSteps = 8;              // 16 KiB settled by the probe warp before a message goes wide
 constexpr uint64_t kTrimWideMin = 256 * 1024;   // shorter remainders stay on the probe warp
@@ -1409,8 +1412,8 @@ __host__ __device__ __forceinline__ uint64_t plan_bucket_min_blocks(uint32_t b) 
 // Rule (3) of the chain selection, shared by the planner kernel and its host mirror.
 //   count          messages that satisfy rules (1) and (2)
 //   chain_blocks   lower bound of their 64-byte blocks (bucket lower bounds x bucket counts; buckets are 12.5 % wide)
-// Chain CTAs and lane CTAs that share an SM slow each other down badly (round 2, one rank's share of C3-v2: the blocks
-// of 1..4 MiB alone took 250 ms with 344 of them on chains spread over every SM, ~110 ms with all of them on lanes).  So:
+// Chain CTAs and lane CTAs that share an SM slow each other down badly (one rank's share of C3-v2 with
+// its 1..4 MiB blocks on chains spread over every SM took more than twice as long as with all of them on lanes).  So:
 //   * up to 3/4 of the SMs' worth of outliers get an SM each, which the lane kernel then leaves alone (F_YIELD_CHAIN_SMS);
 //   * more than that only when (almost) nothing is left for the lanes -- a batch of equally long messages, where the
 //     chain kernel runs by itself at up to max_chain chains (4 per SM);
@@ -1427,8 +1430,8 @@ __host__ __device__ __forceinline__ uint32_t plan_chain_count(uint32_t count, un
 
 // The LONG lane messages: those that satisfy rule (1) -- each would still be running on its lane after the rest of the
 // batch is done -- but stay on lanes (not routed to chains).  In one launch the time slicing scatters them one per warp
-// over the whole grid, and the tail then runs ~2 000 warps with a single live lane each (one rank's share of C3-v2: the
-// 12 GiB of blocks below 4 MiB took 224 ms, the 1 339 blocks of 1..4 MiB alone, lane-packed, 106 ms).  So they get
+// over the whole grid, and the tail then runs ~2 000 warps with a single live lane each (one rank's share of C3-v2: its
+// 1..4 MiB blocks alone, lane-packed, take about half the time of the whole mixed launch).  So they get
 // their own queue and a second, lane-packed launch behind the short ones.  count1 = messages satisfying rule (1).
 __host__ __device__ __forceinline__ uint32_t plan_long_count(uint32_t count1, uint32_t chain, uint32_t n, uint32_t long_cap) {
     const uint32_t nl = count1 > chain ? count1 - chain : 0u;
@@ -1498,7 +1501,7 @@ __global__ void plan_hist_kernel(const uint64_t* __restrict__ len, uint64_t n, u
 // hist[0..B) counts -> cursor[0..B) start positions, longest bucket first; also decides how many of the
 // longest messages leave the lane queue for the chain kernel.  Single CTA of kPlanBuckets threads.
 //
-// Chain selection.  One chain on the chain kernel runs ~2x faster than on a lane (62 vs 30 MB/s fused, the
+// Chain selection.  One chain on the chain kernel runs ~2x faster than on a lane (the
 // one-warp issue limit of 0.5 instr/clk applied to 1 056 instead of 2 108 instructions per block), but a chain CTA
 // serves ONE message with three warps where a lane-kernel warp serves 32, and the two kernels slow each other
 // down while they share SMSPs.  So only true outliers go there -- the messages that would still be running on
@@ -1508,8 +1511,8 @@ __global__ void plan_hist_kernel(const uint64_t* __restrict__ len, uint64_t n, u
 //   (2) longer than half the longest message (anything shorter finishes on a lane before the longest one
 //       finishes on the chain kernel);
 //   (3) and only if ALL such messages fit (count <= max_chain, one CTA per SM): routing a part of a set of
-//       equally long messages leaves the makespan where it was and costs the interference (measured: 2048 x 4 MiB
-//       159 -> 332 ms with 148 of them moved over).
+//       equally long messages leaves the makespan where it was and costs the interference (2048 x 4 MiB with one
+//       SM's worth of them moved over took twice as long).
 // qctl = {lane entries available, head, tail, chain count}.
 __global__ void plan_scan_kernel(const uint32_t* __restrict__ hist, uint32_t* __restrict__ cursor, int* __restrict__ qctl,
                                  const unsigned long long* __restrict__ total_blocks, uint32_t n, uint32_t max_chain,
@@ -1545,9 +1548,8 @@ __global__ void plan_scan_kernel(const uint32_t* __restrict__ hist, uint32_t* __
     if (hist[rev]) atomicMax(&sh_top, (uint32_t)rev);
     __syncthreads();
     // rule (2): "longer than ratio8/8 of the longest" -- what stays on a lane must finish there before the longest
-    // message finishes on its chain: lane speed / chain speed is 30/71 for the fused digests (3/8), 39/71 and 76/148
-    // for SHA-256 / MD5 alone (4/8).  (Round 1 used 1/2 throughout: the 29 MB files of C3-v1 then took 1 s on their
-    // lanes while the 59 MB file took 0.84 s on its chain.)
+    // message finishes on its chain: lane speed / chain speed is about 3/8 for the fused digests and 4/8 for SHA-256 /
+    // MD5 alone (the one-warp issue limit applied to each kernel's instruction count per block).
     const unsigned long long half = plan_bucket_min_blocks(sh_top) / 8 * ratio8;
     if (thr < half) thr = half;
     const bool mine = plan_bucket_min_blocks((uint32_t)rev) >= thr;
@@ -1646,18 +1648,20 @@ __global__ void hex_rows_kernel(const uint32_t* __restrict__ in, uint64_t nwords
     }
 }
 
+static int g_sm_count = 132;  // set from the device by configure_kernels()
+
+int device_sm_count() { return g_sm_count; }
+
 int launch_hex_rows(const uint8_t* in, uint64_t nbytes, uint8_t* out, cudaStream_t st) {
     if (!nbytes) return 0;
     const uint64_t nwords = nbytes / 4;
     uint64_t g = (nwords + 255) / 256;
-    if (g > 148 * 16) g = 148 * 16;
+    if (g > (uint64_t)g_sm_count * 16) g = (uint64_t)g_sm_count * 16;
     hex_rows_kernel<<<(int)g, 256, 0, st>>>(reinterpret_cast<const uint32_t*>(in), nwords, reinterpret_cast<uint2*>(out));
     return 1;
 }
 
 // --------------------------------------------------------------------------------- launch wrappers
-
-static int g_sm_count = 148;
 
 static int grid_for(uint64_t n, int threads, int cap) {
     uint64_t g = (n + threads - 1) / threads;
@@ -1675,7 +1679,7 @@ int launch_trim(const uint8_t* base, const uint64_t* off, const uint64_t* len, u
 }
 
 
-static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS, B200H_LANE_MIN_CTAS, B200H_LANE_MIN_CTAS};  // [sha+md5, sha, md5]
+static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS, B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS};  // [sha+md5, sha, md5]
 
 // most long messages a second, lane-packed launch takes: one wave of lanes at one warp per SMSP
 uint32_t plan_long_cap() {
@@ -1705,10 +1709,10 @@ int launch_plan(const uint64_t* len, uint64_t n, uint32_t* ring, uint32_t* ring_
     cudaMemsetAsync(total, 0, sizeof(unsigned long long), st);
     cudaMemsetAsync(ring, 0xff, sizeof(uint32_t) * ring_capacity(n), st);
     if (ring_long) cudaMemsetAsync(ring_long, 0xff, sizeof(uint32_t) * kLongRingCapacity, st);
-    plan_hist_kernel<<<grid_for(n, 256, 148 * 4), 256, 0, st>>>(len, n, hist, total);
+    plan_hist_kernel<<<grid_for(n, 256, g_sm_count * 4), 256, 0, st>>>(len, n, hist, total);
     plan_scan_kernel<<<1, kPlanBuckets, 0, st>>>(hist, cursor, qctl, total, (uint32_t)n, max_chain, sm_count,
                                                  ring_long ? plan_long_cap() : 0u, ratio8);
-    plan_scatter_kernel<<<grid_for(n, 256, 148 * 4), 256, 0, st>>>(len, n, cursor, ring, ring_long, chain_list, qctl,
+    plan_scatter_kernel<<<grid_for(n, 256, g_sm_count * 4), 256, 0, st>>>(len, n, cursor, ring, ring_long, chain_list, qctl,
                                                                 fresh ? kFresh : 0u);
     return 3;
 }
@@ -1802,7 +1806,7 @@ int launch_lane_hash(const uint8_t* base, const uint64_t* off, const uint64_t* l
 
 int launch_fill_synth(uint8_t* dst, uint64_t nbytes, uint64_t seed, uint64_t start, cudaStream_t st) {
     if (!nbytes) return 0;
-    fill_synth_kernel<<<grid_for((nbytes >> 3) + 1, 256, 148 * 16), 256, 0, st>>>(dst, nbytes, seed * 0xD1342543DE82EF95ull,
+    fill_synth_kernel<<<grid_for((nbytes >> 3) + 1, 256, g_sm_count * 16), 256, 0, st>>>(dst, nbytes, seed * 0xD1342543DE82EF95ull,
                                                                                  start >> 3);
     return 1;
 }
@@ -1847,7 +1851,7 @@ cudaError_t configure_kernels() {
 }
 
 const char* kernel_build_info() {
-    return "b200hash kernels: sm_100a, lane_hash(persistent, time-sliced q=32, cp.async ring 2x128B per lane), " __DATE__;
+    return "b200hash kernels: sm_90a, lane_hash(persistent, time-sliced q=32, cp.async ring 2x128B per lane), " __DATE__;
 }
 
 }  // namespace b200h

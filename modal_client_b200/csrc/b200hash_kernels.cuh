@@ -23,7 +23,7 @@ enum : uint32_t {
 
 constexpr int kPlanBuckets = 512;
 constexpr unsigned long long kChainMinBlocks = 1024;  // 64 KiB: shorter messages never go to the chain kernel
-constexpr unsigned long long kChainRatio = 24000;     // lane kernel ~700 GB/s vs ~29 MB/s for one lane
+constexpr unsigned long long kChainRatio = 21000;     // H100: lane kernel ~540 GB/s fused vs ~26 MB/s for one lane
 constexpr uint32_t kMaxChain = 1184;                  // chain-list capacity (entries)
 constexpr int kSmFlagWords = 256;  // one word per SM: set by a chain CTA that serves a message (see F_YIELD_CHAIN_SMS)
 // hist, cursor, qctl[4], total_blocks (u64), chain words[2], qctl_long[8], sm_flags[kSmFlagWords]
@@ -84,6 +84,7 @@ int launch_fill_synth(uint8_t* dst, uint64_t nbytes, uint64_t seed, uint64_t sta
 int launch_hex_rows(const uint8_t* in, uint64_t nbytes, uint8_t* out, cudaStream_t st);
 
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
+int device_sm_count();             // SMs of the current device (as seen by configure_kernels)
 cudaError_t configure_kernels();  // one-time cudaFuncSetAttribute calls for the current device
 const char* kernel_build_info();
 

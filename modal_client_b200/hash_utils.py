@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ``modal/_utils/hash_utils.py`` with the arithmetic on the B200.
+"""Drop-in for the reference's ``modal/_utils/hash_utils.py`` with the arithmetic on the GPU.
 
 Same names, signatures, return types and stream semantics as the reference
 (py/modal/_utils/hash_utils.py:14-101); the hashlib objects are replaced by libb200hash calls:

@@ -1,5 +1,5 @@
 """One shared aiohttp session for object-store PUT/POST, as the reference keeps
-(py/modal/_utils/http_utils.py:35-51).  Networking itself is out of scope for the B200 path; this exists
+(py/modal/_utils/http_utils.py:35-51).  Networking itself is out of scope for the GPU hash path; this exists
 so the upload functions that consume the GPU digests have the same shape as the reference's."""
 from __future__ import annotations
 

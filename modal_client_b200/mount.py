@@ -1,4 +1,4 @@
-"""Mount creation on the B200 hash path: select files, checksum them, dedupe, upload, register.
+"""Mount creation on the GPU hash path: select files, checksum them, dedupe, upload, register.
 
 Counterpart of the upload half of ``_Mount`` (py/modal/mount.py): entries (``_MountFile`` :111-134, ``_MountDir``
 :136-196), ``_select_files`` (:103-108), ``_Mount._get_files`` (:465-485) and ``_Mount._load_mount`` (:487-622).

@@ -1,4 +1,4 @@
-"""NetworkFileSystem uploads on the B200 hash path.
+"""NetworkFileSystem uploads on the GPU hash path.
 
 Counterpart of the data path of ``_NetworkFileSystem`` (py/modal/network_file_system.py): ``write_file`` (:217-260),
 ``read_file`` (:262-276), ``add_local_file`` (:291-305) and ``add_local_dir`` (:307-335).  The reference hashes every

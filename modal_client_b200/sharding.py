@@ -43,7 +43,7 @@ def bind_process_to_gpu_node(device: int) -> bool:
     """One process per GPU: run this process (and every thread it starts later) on the CPUs next to its GPU, so that
     the payloads it allocates, the pinned staging ring and the packer threads all sit in the memory the GPU's DMA
     engine reads from.  torchrun does not do this; without it 8 ranks packing pageable payloads push most bytes
-    across the socket interconnect (measured: map-pump e2e 8 GPUs 64 -> see profiles/).  Returns whether it bound."""
+    across the socket interconnect.  Returns whether it bound."""
     import os
 
     cpus = gpu_node_cpus(device)

@@ -1,4 +1,4 @@
-"""``Volume.batch_upload()`` on the B200 hash path.
+"""``Volume.batch_upload()`` on the GPU hash path.
 
 Counterparts of ``_VolumeUploadContextManager`` (volumefs1: whole-file SHA-256 + MD5, dedupe through
 ``MountPutFile``, py/modal/volume.py:1181-1333) and ``_VolumeUploadContextManager2`` (volumefs2: SHA-256 of every

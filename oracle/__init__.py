@@ -1,7 +1,7 @@
-"""oracle/ -- TEST INFRASTRUCTURE ONLY (CPU checker for the B200 hash path).
+"""oracle/ -- TEST INFRASTRUCTURE ONLY (CPU checker for the GPU hash path).
 
 Nothing under ``modal_client_b200/`` may import this package.  Allowed users:
-``tests/``, ``__graft_entry__.smoke()``, and ``bench.py``'s ``cpu_baseline`` /
+``tests/``, ``__graft_entry__.smoke()``, ``oracle/gen_golden.py`` and ``bench.py``'s ``cpu_baseline`` /
 ``--impl reference`` legs.
 
 Two independent CPU statements of the reference's path live here:
@@ -11,8 +11,8 @@ Two independent CPU statements of the reference's path live here:
 * ``oracle.ref_port``  -- a Python restatement of the reference's *control flow*
   (``hash_utils._update`` / ``get_upload_hashes`` / ``_find_end_of_block`` / ``_gather_block`` /
   multipart ETag) on top of ``hashlib`` -- the very library the reference calls
-  (``/root/reference/py/modal/_utils/hash_utils.py:34,42,50,75,78``).
+  (``py/modal/_utils/hash_utils.py:34,42,50,75,78`` of the original project).
 
 Parity pinning: see ``tests/test_oracle.py`` (NIST / RFC known answers, hashlib cross-check,
-and ``tests/golden/*.json`` produced by the unmodified reference through ``oracle/ref_shim.py``).
+and ``tests/golden/*.json`` recorded from the unmodified original project by ``oracle/gen_golden.py``).
 """

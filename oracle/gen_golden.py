@@ -1,8 +1,8 @@
-"""oracle/gen_golden.py -- regenerates tests/golden/*.json from the UNMODIFIED reference.
+"""oracle/gen_golden.py -- regenerates tests/golden/*.json from the UNMODIFIED original project.
 
-Run in the build container only (needs /root/reference):  ``python -m oracle.gen_golden``
+Needs a checkout of it:  ``B200H_REFERENCE_ROOT=<modal-client checkout> python -m oracle.gen_golden``
 Inputs are stored as small recipes (modal_client_b200.synth.materialize), outputs are whatever the
-reference's own functions returned.  The GPU box never runs this; it only reads the JSON.
+original project's own functions returned.  The tests only read the JSON.
 """
 from __future__ import annotations
 
@@ -239,6 +239,42 @@ def gen_multipart(b, seg):
     return {"source": "py/modal/_utils/blob_utils.py:159-234 + bytes_io_segment_payload.py (unmodified)", "cases": out}
 
 
+def gen_port_samples(h, b):
+    """get_upload_hashes and _find_end_of_block on a few seeded payloads (tests/test_oracle.py compares the port)."""
+    out = []
+    for seed, n in [(900, 0), (901, 1), (902, 70001), (903, 300000)]:
+        data = materialize(synth(seed, n))
+        up = h.get_upload_hashes(io.BytesIO(data))
+        padded = data + bytes(9)
+        out.append({"input": synth(seed, n), "md5_base64": up.md5_base64, "sha256_base64": up.sha256_base64,
+                    "end_of_block_padded_9": b._find_end_of_block(lambda d=padded: io.BytesIO(d), 0, n + 9)})
+    return out
+
+
+def _source_constant(rel, name):
+    """A module constant of the original project read from its source (modules that cannot be imported without
+    the control plane); the right-hand sides are arithmetic literals."""
+    import re
+
+    path = os.path.join(os.path.dirname(ref_shim.package_dir()), "modal", rel)
+    m = re.search(rf"^{name}\s*(?::[^=]+)?=\s*\(?\s*([^#\n]+)", open(path).read(), flags=re.M)
+    return eval(m.group(1).strip().rstrip(")"))  # noqa: S307
+
+
+def gen_reference_values(h, b):
+    """Module constants that callers and tests patch, with the original project's values, and the seeded samples."""
+    consts = {"hash_utils.HASH_CHUNK_SIZE": h.HASH_CHUNK_SIZE}
+    for name in ["MAX_OBJECT_SIZE_BYTES", "MAX_ASYNC_OBJECT_SIZE_BYTES", "LARGE_FILE_LIMIT", "BLOB_MAX_PARALLELISM",
+                 "DEFAULT_SEGMENT_CHUNK_SIZE", "MULTIPART_UPLOAD_THRESHOLD", "BLOCK_SIZE"]:
+        consts[f"blob_utils.{name}"] = getattr(b, name)
+    for rel, name in [("mount.py", "MOUNT_PUT_FILE_CLIENT_TIMEOUT"), ("volume.py", "VOLUME_PUT_FILE_CLIENT_TIMEOUT"),
+                      ("network_file_system.py", "NETWORK_FILE_SYSTEM_PUT_FILE_CLIENT_TIMEOUT"),
+                      ("parallel_map.py", "MAP_INVOCATION_CHUNK_SIZE"), ("parallel_map.py", "SPAWN_MAP_INVOCATION_CHUNK_SIZE")]:
+        consts[f"{rel[:-3]}.{name}"] = _source_constant(rel, name)
+    return {"source": "py/modal/_utils/hash_utils.py, blob_utils.py, mount.py, volume.py, network_file_system.py, "
+                      "parallel_map.py (unmodified)", "constants": consts, "port_samples": gen_port_samples(h, b)}
+
+
 # ---------------------------------------------------------------------------------- mount file selection
 
 MOUNT_TREE = {  # relative path -> ("file", seed, size) | ("link", target relative to the tmp dir) ; dirs are implied
@@ -346,7 +382,7 @@ def main():
     os.makedirs(OUT, exist_ok=True)
     for name, doc in [("hash_utils.json", gen_hash_utils(h)), ("file_specs.json", gen_file_specs(b)),
                       ("blocks.json", gen_blocks(b)), ("multipart.json", gen_multipart(b, seg)),
-                      ("mount_select.json", gen_mount_select())]:
+                      ("mount_select.json", gen_mount_select()), ("reference_values.json", gen_reference_values(h, b))]:
         with open(os.path.join(OUT, name), "w") as f:
             json.dump(doc, f, indent=1, sort_keys=True)
             f.write("\n")

@@ -63,3 +63,26 @@ def test_e2e_leg_of_the_gpu_arm_runs_on_the_host_layer(fake_backend, monkeypatch
         assert base64.b64decode(r.content_sha256_base64) == hashlib.sha256(p).digest() == sha[i].tobytes()
         assert base64.b64decode(r.content_md5) == hashlib.md5(p).digest() == md5[i].tobytes()
     assert set(bench.run_map_pump.last_stats) == {"collect_s", "wait_context_s", "hash_call_s", "wait_hash_s"}
+
+
+def test_dump_outputs_writes_float32_digest_tables(tmp_path):
+    """The files --dump-outputs leaves behind: sha256.npy float32[n, 32] and md5.npy float32[n, 16], byte for byte the
+    digest table of the step."""
+    import numpy as np
+
+    sys.path.insert(0, ROOT)
+    import bench
+
+    rng = np.random.default_rng(5)
+    sha, md5 = rng.integers(0, 256, (7, 32), dtype=np.uint8), rng.integers(0, 256, (7, 16), dtype=np.uint8)
+    bench.dump_outputs(str(tmp_path / "out"), sha, md5)
+    assert sorted(os.listdir(tmp_path / "out")) == ["md5.npy", "sha256.npy"]
+    s, m = np.load(tmp_path / "out" / "sha256.npy"), np.load(tmp_path / "out" / "md5.npy")
+    assert s.dtype == np.float32 and s.shape == (7, 32) and np.array_equal(s.astype(np.uint8), sha)
+    assert m.dtype == np.float32 and m.shape == (7, 16) and np.array_equal(m.astype(np.uint8), md5)
+
+
+def test_reference_arm_rejects_dump_outputs(tmp_path):
+    out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--dump-outputs",
+                          str(tmp_path / "d")], capture_output=True, text=True, cwd=ROOT, timeout=120)
+    assert out.returncode != 0 and "--dump-outputs" in out.stderr and not (tmp_path / "d").exists()

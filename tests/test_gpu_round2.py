@@ -52,7 +52,8 @@ def test_host_outlier_plan_equals_device_plan(ctx):
         [1 << 20] * 40,
         [100_000] * 2000,
         [80 * 1024] * 700,
-        [2 << 20], [100], [0], [65536], [65535], [65536 - 64], [1 << 16] * 592, [1 << 16] * 593,
+        [2 << 20], [100], [0], [65536], [65535], [65536 - 64],
+        [1 << 16] * 528, [1 << 16] * 529,                # either side of the chain cap (4 per SM on 132 SMs)
         [3 << 20] * 344 + [1 << 20] * 995,               # more outlier candidates than 3/4 of the SMs in a mixed batch: none routed
         [16 << 20] * 200 + [100] * 10,                   # ... unless next to nothing is left for the lanes
         [8 << 20] * 3 + [1 << 20] * 200 + [3000] * 20000,  # chain + long lane queue + short lane queue

@@ -240,15 +240,3 @@ def test_mount_selection_matches_reference_golden(tmp_path):
     _, got = _selection_cases(tmp_path)
     assert got == golden["cases"]
     assert len(golden["cases"]["dir_recursive"]) == 10 and len(golden["cases"]["dir_flat"]) == 4
-
-
-def test_mount_selection_matches_live_reference(tmp_path):
-    from oracle import ref_shim
-
-    if not ref_shim.available() or not os.path.isfile(os.path.join(os.path.dirname(ref_shim.package_dir()), "modal", "mount.py")):
-        pytest.skip("no copy of the reference here")
-    gen_golden, got = _selection_cases(tmp_path)
-    ns = gen_golden.reference_mount_entries()
-    want = {name: gen_golden.normalise_selection(ns["_select_files"](entries), str(tmp_path))
-            for name, entries in gen_golden.mount_cases(ns, str(tmp_path)).items()}
-    assert got == want

@@ -1,7 +1,7 @@
 """The planner's routing policy, checked on the CPU.
 
 ``b200h_plan_preview`` runs the library's host-side planner (``plan_outliers_host``: the code that sizes the chain /
-long-queue launches without reading the device planner's answer back; on the GPU box
+long-queue launches without reading the device planner's answer back; on the GPU
 ``tests/test_gpu_round2.py::test_host_outlier_plan_equals_device_plan`` pins it to the device kernels).  Here it is
 compared with a plain-Python restatement of the rules as DESIGN.md 5.3 / 5.4 states them, on random batches and on the
 scenarios the design quotes."""
@@ -10,8 +10,8 @@ import pytest
 
 from modal_client_b200 import _lib
 
-SMS = 148
-MIN_BLOCKS, RATIO, MAX_CHAIN_CAP, LONG_RING = 1024, 24000, 1184, 32768
+SMS = 132  # H100 SXM
+MIN_BLOCKS, RATIO, MAX_CHAIN_CAP, LONG_RING = 1024, 21000, 1184, 32768
 
 
 def _bucket(length: int) -> int:
@@ -79,11 +79,11 @@ def test_documented_routing_scenarios(name, lengths, flags, expect):
 
 
 def test_c3v2_share_routes_its_8mib_blocks_and_queues_the_1_to_4_mib_ones():
-    """One rank's share of C3-v2 (profiles/r2_c3v2_probe.txt): 93 blocks of 8 MiB among 131 002 smaller ones, 1 339 of
+    """One rank's share of C3-v2: 93 blocks of 8 MiB among 131 002 smaller ones, 1 339 of
     them between 1 and 4 MiB: the 8 MiB blocks get an SM each (93 <= 3/4 of the SMs), the 1-4 MiB blocks form the long
     lane queue, the rest is the ordinary queue."""
     rng = np.random.default_rng(11)
-    small = rng.integers(1_000, 180_000, 131_002 - 1_339)  # ~12 GiB in all: rule (1) starts at ~0.55 MB
+    small = rng.integers(1_000, 180_000, 131_002 - 1_339)  # ~12 GiB in all: rule (1) starts at ~0.7 MB
     mid = rng.integers(1 << 20, 4 << 20, 1_339)
     lengths = np.concatenate([[8 << 20] * 93, mid, small]).astype(np.uint64)
     rng.shuffle(lengths)

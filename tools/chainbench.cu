@@ -2,7 +2,7 @@
 //   (a) SHA-256 rounds only, W+K rows read from shared memory (the schedule expanded elsewhere),
 //   (b) full SHA-256 (schedule + rounds), (c) MD5, (d) fused SHA-256 + MD5 (the lane kernel's compress<>),
 // message words read from shared memory.  One CTA, NW warps (one per SMSP when NW <= 4).
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/chainbench tools/chainbench.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/chainbench tools/chainbench.cu
 #include <cstdio>
 #include "../modal_client_b200/csrc/b200hash_kernels.cu"
 
@@ -127,8 +127,10 @@ static void run(const char* name, int warps) {
     cudaMemcpy(&c, cyc, 8, cudaMemcpyDeviceToHost);
     cudaError_t e = cudaGetLastError();
     const double cpb = (double)c / nb;
-    printf("%-34s warps=%d  %8.1f cycles/block  -> %6.1f MB/s per chain at 1.965 GHz  (%s)\n", name, warps, cpb,
-           64.0 * 1965.0 / cpb, cudaGetErrorString(e));
+    int khz = 0;  // the SM clock the cycle count is converted at (the device's maximum)
+    cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+    printf("%-34s warps=%d  %8.1f cycles/block  -> %6.1f MB/s per chain at %.3f GHz  (%s)\n", name, warps, cpb,
+           64.0 * (khz / 1e3) / cpb, khz / 1e6, cudaGetErrorString(e));
     cudaFree(out);
     cudaFree(cyc);
 }

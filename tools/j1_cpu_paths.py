@@ -5,7 +5,7 @@ buffer for every block: `BytesIO(buffer)` in FileUploadSpec2.from_fileobj, py/mo
        (iii) hashlib.md5 per 64 MiB part on a thread pool, (i) get_upload_hashes(open(path)) on one thread
   C3-v2  the first ~8 GiB of the 100 GiB / 1 Mi-file tree as files in /dev/shm, FileUploadSpec2.from_path for all of them
 The bytes are the ones tools/j1_matrix.py hashes on the GPU (same generator, same seeds); the block / part digests are
-compared with a GPU pass over the same files (b200h_hash_files).  Appends rows to gpurun_out/r2_j1_cpu_paths.jsonl."""
+compared with a GPU pass over the same files (b200h_hash_files).  Appends rows to j1_out/r2_j1_cpu_paths.jsonl."""
 import asyncio
 import hashlib
 import json
@@ -24,7 +24,7 @@ from modal_client_b200 import _lib
 from oracle import ref_shim
 
 GiB = float(1 << 30)
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", "r2_j1_cpu_paths.jsonl")
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "j1_out", "r2_j1_cpu_paths.jsonl")
 ref_hash, ref_blob, _ = ref_shim.load()
 ctx = _lib.Context(0)
 dev = torch.device("cuda:0")

@@ -13,7 +13,7 @@ machine), and for each configuration reports
            Semaphore(cpu_count) -- as BASELINE.md section 3 prescribes, on a bounded prefix (stated per row).
 C3 is STRONG scaling (the 100 GiB / 1 Mi-file tree is split over the ranks by sharding.shard_assignment), C5 is weak
 (8 GiB per GPU per point), C4 is one 10 GiB stream on one GPU.  One JSON line per row on stdout (rank 0) and appended
-to gpurun_out/j1_n<N>.jsonl.  Environment: J1_C3_GIB (100), J1_C3_FILES (1048576), J1_C5_BYTES (8 GiB), J1_C5_KMAX (10),
+to j1_out/j1_n<N>.jsonl.  Environment: J1_C3_GIB (100), J1_C3_FILES (1048576), J1_C5_BYTES (8 GiB), J1_C5_KMAX (10),
 J1_C4_GIB (10), J1_E2E_CAP (12.5 GiB), J1_CPU_PREFIX (8 GiB)."""
 import asyncio
 import io
@@ -41,7 +41,7 @@ if world > 1:
 ctx = _lib.Context(local, pinned_bytes=512 << 20, device_bytes=8 << 30)
 st = torch.cuda.Stream(device=dev)
 torch.cuda.set_stream(st)
-PEAK = 6489.6
+PEAK = 3350.0  # GB/s, NVIDIA H100 SXM data sheet
 try:
     PEAK = float(json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:
@@ -49,7 +49,7 @@ except Exception:
 E2E_CAP = int(float(os.environ.get("J1_E2E_CAP", 12.5)) * GiB)
 CPU_PREFIX = int(float(os.environ.get("J1_CPU_PREFIX", 8)) * GiB)
 BOTH = _lib.SHA256 | _lib.MD5
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", f"j1_n{world}.jsonl")
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "j1_out", f"j1_n{world}.jsonl")
 os.makedirs(os.path.dirname(OUT), exist_ok=True)
 
 

@@ -1,6 +1,6 @@
 """tools/j1_table.py -- merge the JSON lines of tools/j1_matrix.py (one file per GPU count) into the markdown table the
 round-2 review asked for: per configuration GPU kernel GiB/s, GPU e2e GiB/s, fraction of the HBM roofline per GPU, the
-reference's CPU path beside it.    python tools/j1_table.py profiles/r2_j1_n1.jsonl profiles/r2_j1_n2.jsonl ..."""
+reference's CPU path beside it.    python tools/j1_table.py j1_n1.jsonl j1_n2.jsonl ..."""
 import json
 import sys
 from collections import OrderedDict

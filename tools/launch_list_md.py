@@ -1,5 +1,5 @@
 """tools/launch_list_md.py -- turn an `ncu --metrics gpu__time_duration.sum --csv` launch list into the per-kernel
-share table kept under profiles/.   usage: python tools/launch_list_md.py launches.csv out.md "<title line>" """
+share table in markdown.   usage: python tools/launch_list_md.py launches.csv out.md "<title line>" """
 import csv
 import re
 import sys

@@ -1,5 +1,5 @@
 """tools/ncu_summary.py -- condense an .ncu-rep (ncu --set full) into the few numbers DESIGN.md cites.
-usage: python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r1_lane_hash.md"""
+usage: python tools/ncu_summary.py prof.ncu-rep summary.md"""
 import csv
 import io
 import subprocess
@@ -35,7 +35,7 @@ def main():
     raw = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout
     rows = list(csv.reader(io.StringIO(raw)))
     hdr, units = rows[0], rows[1]
-    lines = [f"# ncu summary of `{rep.split('/')[-1]}`\n", "Captured with `ncu --set full --clock-control none --import-source on` on a B200 (see the command in DESIGN.md).\n"]
+    lines = [f"# ncu summary of `{rep.split('/')[-1]}`\n", "Captured with `ncu --set full --clock-control none --import-source on` (see the command in DESIGN.md).\n"]
     for r in rows[2:]:
         d = dict(zip(hdr, r))
         lines.append(f"\n## {d.get('Kernel Name', '?')}  (grid {d.get('Grid Size')}, block {d.get('Block Size')})\n")

@@ -1,6 +1,6 @@
 // tools/outlier_bench.cu -- one (or a few) long messages through the launch wrappers directly: lane kernel vs
 // chain kernel, with the planner's routing decision printed.  Includes the kernel translation unit.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/outlier_bench tools/outlier_bench.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/outlier_bench tools/outlier_bench.cu
 #include <cstdio>
 #include <vector>
 #include "../modal_client_b200/csrc/b200hash_kernels.cu"
@@ -13,7 +13,7 @@ int main(int argc, char** argv) {
     const uint64_t n = argc > 1 ? atoll(argv[1]) : 1;
     const uint64_t size = argc > 2 ? atoll(argv[2]) : (16ull << 20);
     const uint64_t nsmall = argc > 3 ? atoll(argv[3]) : 0;  // extra 100 KiB messages sharing the batch
-    const uint32_t cap = argc > 4 ? (uint32_t)atoi(argv[4]) : 592u;  // chain CTAs available to the planner
+    const uint32_t cap = argc > 4 ? (uint32_t)atoi(argv[4]) : 528u;  // chain CTAs available to the planner
     const uint64_t ssz = 100 * 1024;
     CK(configure_kernels());
     const uint64_t N = n + nsmall;

@@ -3,7 +3,7 @@ null control plane around a stand-in for the hash call that behaves like b200h_h
 it is entered through ctypes (GIL released), serialises the calls of one context on a mutex, holds a process-wide
 "packing" mutex for PACK seconds per 4 096 payloads (the host's staging-copy capacity is one shared resource) and then
 spends TAIL seconds on its own (last H2D chunk + kernel + D2H).  Everything is inside C, so the GIL traffic of the
-real path is reproduced; the digests are zeros.  With PACK=0.030 TAIL=0.015 (33 GiB/s of packing, the B200 host's
+real path is reproduced; the digests are zeros.  With PACK=0.030 TAIL=0.015 (33 GiB/s of packing, one measured host's
 measured figure) the floor is 0.75 s per 100 000 x 256 KiB; the round-2 pump as measured on the box (1.04-1.12 s) comes
 out at 1.01-1.07 s in this model, which is what makes it usable for host-side work when no GPU is at hand.
 

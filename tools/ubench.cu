@@ -1,6 +1,6 @@
 // tools/ubench.cu -- issue-rate microbenchmarks for the INT32 instruction forms the hash kernel uses.
 // Each test runs 8 independent accumulators per thread (no dependency stalls), 16 warps/SM... and reports
-// warp-instructions per cycle per SMSP.   nvcc -arch=sm_100a -o ubench ubench.cu
+// warp-instructions per cycle per SMSP.   nvcc -arch=sm_90a -o ubench ubench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -107,15 +107,17 @@ void run(const char* name, int warps_per_smsp) {
     uint32_t* out;
     long long* cyc;
     int threads = 128 * warps_per_smsp;  // one CTA per SM, warps spread over the 4 SMSPs
-    cudaMalloc(&out, 148 * threads * 4);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&out, (size_t)sms * threads * 4);
     cudaMalloc(&cyc, 8);
-    k<MODE><<<148, threads>>>(out, 1, 12345, cyc);
+    k<MODE><<<sms, threads>>>(out, 1, 12345, cyc);
     cudaDeviceSynchronize();
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
     cudaEventRecord(e0);
-    k<MODE><<<148, threads>>>(out, 1, 12345, cyc);
+    k<MODE><<<sms, threads>>>(out, 1, 12345, cyc);
     cudaEventRecord(e1);
     cudaDeviceSynchronize();
     long long c;
