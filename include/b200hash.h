@@ -114,6 +114,23 @@ int b200h_hash_fixed_parts(b200h_ctx* ctx, const uint8_t* base, uint64_t len, ui
                            uint8_t* sha256_out, uint8_t* md5_out, uint64_t* trimmed_len_out,
                            uint8_t etag_md5_out[16], uint64_t* nparts_out);
 
+/* Same split, but the buffer [d_base, d_base + len) and every output are DEVICE memory on ctx's device, and the work is
+ * only enqueued on `cuda_stream` (a cudaStream_t; NULL = the context's compute stream).  The parts are cut by the same
+ * code as b200h_hash_fixed_parts and b200h_hash_files(part_len > 0).  Outputs (each may be NULL): d_sha256[nparts*32],
+ * d_md5[nparts*16] (both 16-byte aligned), d_trimmed_len[nparts] (== the part length unless B200H_TRIM_ZEROS),
+ * d_etag_md5[16] (16-byte aligned; MD5 over the concatenated raw part MD5s, md5("") for len == 0; requires B200H_MD5,
+ * and d_md5 when len > 0).  *nparts_out = ceil(len / part_len), returned on the host.  No B200H_HEX_OUT here.
+ * The part lengths are known on the host, so outliers are routed there (as b200h_hash_batch_device_hl does) and the
+ * call ONLY ENQUEUES -- except with B200H_TRIM_ZEROS and outlier routing on: the lengths that matter are then the
+ * trimmed ones, which exist on the device only, and the planner's count is read back (one synchronisation of
+ * `cuda_stream`, counted by b200h_plan_sync_count).  B200H_TRIM_ZEROS | B200H_NO_OUTLIERS only enqueues.
+ * The part table (16 bytes per part) travels to the device with the work.
+ * Replaces: the per-8MiB-block loop of _gather_blocks (blob_utils.py:622-645) for a buffer that already lives in HBM,
+ * which the reference would first copy to host memory. */
+int b200h_hash_fixed_parts_device(b200h_ctx* ctx, const void* d_base, uint64_t len, uint64_t part_len, uint32_t flags,
+                                  void* d_sha256, void* d_md5, uint64_t* d_trimmed_len, void* d_etag_md5,
+                                  uint64_t* nparts_out, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

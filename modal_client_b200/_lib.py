@@ -33,6 +33,7 @@ ABI_SYMBOLS = (
     "b200h_profile_enable", "b200h_profile_read", "b200h_dedupe_host", "b200h_dedupe_device",
     "b200h_last_outlier_count", "b200h_hash_batch_device_hl", "b200h_combine_stats", "b200h_plan_sync_count",
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
+    "b200h_hash_fixed_parts_device",
 )
 
 
@@ -98,6 +99,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_plan_sync_count.restype = u64
         L.b200h_hash_fixed_parts.argtypes = [vp, vp, u64, u64, u32, vp, vp, vp, vp, ctypes.POINTER(u64)]
         L.b200h_hash_fixed_parts.restype = i32
+        L.b200h_hash_fixed_parts_device.argtypes = [vp, vp, u64, u64, u32, vp, vp, vp, vp, ctypes.POINTER(u64), vp]
+        L.b200h_hash_fixed_parts_device.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -343,6 +346,17 @@ class Context:
         self._check(rc, "b200h_hash_fixed_parts")
         assert got.value == nparts
         return sha, md5, trimmed, (etag.tobytes() if want_etag else None)
+
+    def hash_fixed_parts_device(self, d_base: int, nbytes: int, part_len: int, flags: int, d_sha: int = 0, d_md5: int = 0,
+                                d_trimmed: int = 0, d_etag: int = 0, stream: int = 0) -> int:
+        """``hash_fixed_parts`` over device memory: raw device addresses in and out (a CUDA tensor's data_ptr()), work
+        enqueued on ``stream``.  Outputs hold ceil(nbytes / part_len) rows; returns that part count."""
+        got = ctypes.c_uint64()
+        rc = self._L.b200h_hash_fixed_parts_device(self._h, d_base or None, nbytes, part_len, flags, d_sha or None,
+                                                   d_md5 or None, d_trimmed or None, d_etag or None, ctypes.byref(got),
+                                                   stream or None)
+        self._check(rc, "b200h_hash_fixed_parts_device")
+        return int(got.value)
 
     # -- files: stat + read + hash entirely inside the library (native reader threads, no mmap / Python I/O)
     @staticmethod

@@ -43,6 +43,7 @@ from ._logging import logger
 from ._wire import BlobCreateRequest
 from .async_utils import asyncnullcontext, bounded_map, gather_cancel_on_error, retry
 from .bytes_io_segment_payload import BytesIOSegmentPayload, KnownBytesBody
+from .device_file import DeviceFile
 from .exception import ExecutionError
 from .hash_utils import UploadHashes, get_upload_hashes
 from .http_utils import ClientSessionRegistry
@@ -230,6 +231,8 @@ async def perform_multipart_upload(
         readers: list[BinaryIO] = [BytesIO(view) for _ in part_urls]
         for rdr in readers:
             rdr.seek(start_pos)
+    elif isinstance(data_file, DeviceFile):  # no file name to open again: readers over the same device bytes
+        readers = [data_file.reopen() for _ in part_urls]
     else:
         readers = [open(data_file.name, "rb") for _ in part_urls]
 
@@ -729,6 +732,17 @@ def _blocks_of(view: np.ndarray) -> list[FileUploadBlock]:
     if view.size == 0:
         return []
     sha, _, trimmed, _ = get_context().hash_fixed_parts(view, BLOCK_SIZE, _lib.SHA256 | _lib.TRIM_ZEROS)
+    return _blocks_from_table(sha, trimmed)
+
+
+def _blocks_of_device(fp: DeviceFile) -> list[FileUploadBlock]:
+    """The same blocks of a buffer in GPU memory, trimmed and hashed where it is: only the (trimmed length, SHA-256)
+    table crosses to the host."""
+    sha, _, trimmed = fp.hash_parts(BLOCK_SIZE, _lib.SHA256 | _lib.TRIM_ZEROS)
+    return _blocks_from_table(sha, trimmed)
+
+
+def _blocks_from_table(sha: np.ndarray, trimmed: np.ndarray) -> list[FileUploadBlock]:
     return [
         FileUploadBlock(start=i * BLOCK_SIZE, end=i * BLOCK_SIZE + int(trimmed[i]), contents_sha256=sha[i].tobytes())
         for i in range(len(trimmed))
@@ -757,8 +771,12 @@ class FileUploadSpec2:
 
     @staticmethod
     async def from_fileobj(
-        source_fp: BinaryIO | BytesIO, mount_filename: PurePosixPath, hash_semaphore: asyncio.Semaphore, mode: int
+        source_fp: BinaryIO | BytesIO | DeviceFile, mount_filename: PurePosixPath, hash_semaphore: asyncio.Semaphore,
+        mode: int
     ) -> "FileUploadSpec2":
+        if isinstance(source_fp, DeviceFile):
+            # every use gets its own reader over the same device bytes (the missing-block PUTs run concurrently)
+            return await FileUploadSpec2._create(source_fp.reopen, repr(source_fp), mount_filename, mode, hash_semaphore)
         try:
             fileno = source_fp.fileno()
 
@@ -799,6 +817,8 @@ async def _gather_blocks(source: _FileUploadSource2, size: int, hash_semaphore: 
 
     def run() -> list[FileUploadBlock]:
         with source() as fp:
+            if isinstance(fp, DeviceFile):
+                return _blocks_of_device(fp)
             return _with_view(fp, lambda view: _blocks_of(view[:size]))
 
     async with hash_semaphore:

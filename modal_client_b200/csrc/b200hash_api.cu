@@ -149,6 +149,7 @@ struct b200h_ctx {
     size_t dwave_cap = 0;  // per slot
     size_t dwave_want = 0;
     DevBuf d_off, d_len, d_order, d_order_long, d_trim, d_sha, d_md5, d_scratch, d_small, d_states, d_dedupe, d_keys, d_trimctl, d_hex;
+    DevBuf d_parts;  // part table of b200h_hash_fixed_parts_device: offsets | lengths | the ETag message (offset, length)
     uint64_t* h_meta = nullptr;  // pinned: offsets then lengths
     size_t h_meta_cap = 0;       // in uint64 elements
     uint64_t launches = 0;
@@ -774,6 +775,21 @@ int hash_batch_host_impl(b200h_ctx* ctx, const uint8_t* base, const uint64_t* of
 
 constexpr uint32_t kPublicFlags = 7u | B200H_NO_OUTLIERS | B200H_HEX_OUT;
 
+// The fixed-size part layout shared by b200h_hash_fixed_parts, b200h_hash_fixed_parts_device and
+// b200h_hash_files(part_len > 0): part i of a `len`-byte object starts at i * part_len and holds
+// min(part_len, len - i * part_len) bytes, so only the last part may be short and an empty object has no parts.
+// Appends the parts to off / ln and returns how many there are.  part_len must be > 0.
+uint64_t split_fixed_parts(uint64_t len, uint64_t part_len, std::vector<uint64_t>& off, std::vector<uint64_t>& ln) {
+    const uint64_t nparts = len / part_len + (len % part_len != 0);
+    off.reserve(off.size() + nparts);
+    ln.reserve(ln.size() + nparts);
+    for (uint64_t o = 0; o < len; o += part_len) {
+        off.push_back(o);
+        ln.push_back(std::min(part_len, len - o));
+    }
+    return nparts;
+}
+
 // A small request from one of possibly many concurrent callers: merge it with whatever else arrives while the context
 // is busy, run ONE batch, hand every caller its rows.  (See Combiner.)
 int combined_hash_batch_host(b200h_ctx* ctx, const uint8_t* base, const uint64_t* off, const uint64_t* len, uint64_t n,
@@ -979,7 +995,8 @@ void b200h_destroy(b200h_ctx* ctx) {
         cudaEventDestroy(pr.second);
     }
     for (DevBuf* b : {&ctx->d_off, &ctx->d_len, &ctx->d_order, &ctx->d_trim, &ctx->d_sha, &ctx->d_md5, &ctx->d_scratch,
-                      &ctx->d_small, &ctx->d_states, &ctx->d_dedupe, &ctx->d_keys, &ctx->d_trimctl, &ctx->d_hex, &ctx->d_order_long})
+                      &ctx->d_small, &ctx->d_states, &ctx->d_dedupe, &ctx->d_keys, &ctx->d_trimctl, &ctx->d_hex, &ctx->d_order_long,
+                      &ctx->d_parts})
         if (b->p) cudaFree(b->p);
     for (auto& r : ctx->stream_pool) stream_res_destroy(r);
     ctx->stream_pool.clear();
@@ -1081,7 +1098,8 @@ int b200h_hash_fixed_parts(b200h_ctx* ctx, const uint8_t* base, uint64_t len, ui
     B200H_RANGE("b200h_hash_fixed_parts");
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (part_len == 0) return fail(ctx, B200H_E_INVALID, "part_len must be > 0");
-    const uint64_t nparts = (len + part_len - 1) / part_len;
+    std::vector<uint64_t> off, ln;
+    const uint64_t nparts = split_fixed_parts(len, part_len, off, ln);
     if (nparts_out) *nparts_out = nparts;
     if (nparts == 0) {
         if (etag_md5_out) {
@@ -1092,13 +1110,54 @@ int b200h_hash_fixed_parts(b200h_ctx* ctx, const uint8_t* base, uint64_t len, ui
         }
         return 0;
     }
-    std::vector<uint64_t> off(nparts), ln(nparts);
-    for (uint64_t i = 0; i < nparts; ++i) {
-        off[i] = i * part_len;
-        ln[i] = std::min(part_len, len - off[i]);
-    }
     return hash_batch_host_impl(ctx, base, off.data(), ln.data(), nparts, flags & kPublicFlags, sha256_out, md5_out,
                                 trimmed_len_out, etag_md5_out);
+}
+
+int b200h_hash_fixed_parts_device(b200h_ctx* ctx, const void* d_base, uint64_t len, uint64_t part_len, uint32_t flags,
+                                  void* d_sha256, void* d_md5, uint64_t* d_trimmed_len, void* d_etag_md5,
+                                  uint64_t* nparts_out, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_hash_fixed_parts_device");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (part_len == 0) return fail(ctx, B200H_E_INVALID, "part_len must be > 0");
+    if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
+    if (d_etag_md5 && !(flags & B200H_MD5)) return fail(ctx, B200H_E_INVALID, "etag requires B200H_MD5");
+    if (((uintptr_t)d_sha256 | (uintptr_t)d_md5 | (uintptr_t)d_etag_md5) & 15u)
+        return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
+    if (len && !d_base) return fail(ctx, B200H_E_INVALID, "d_base must not be NULL");
+    std::vector<uint64_t> table;  // offsets, then lengths, then the ETag message {offset, length}
+    std::vector<uint64_t> ln;
+    const uint64_t nparts = split_fixed_parts(len, part_len, table, ln);
+    if (d_etag_md5 && nparts && !d_md5) return fail(ctx, B200H_E_INVALID, "etag requires the part MD5 output d_md5");
+    if (nparts_out) *nparts_out = nparts;
+    if (nparts == 0 && !d_etag_md5) return 0;
+    if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
+        return fail(ctx, B200H_E_INVALID, "flags select neither SHA256 nor MD5");
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    const uint64_t etag_len = nparts * 16;
+    table.insert(table.end(), ln.begin(), ln.end());
+    table.push_back(0);
+    table.push_back(etag_len);
+    // The part table is context scratch like the planner's: it is rewritten only after the last batch that read it.
+    if (ctx->scratch_used) CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_scratch, 0));
+    if (int rc = ensure_dev(ctx, ctx->d_parts, table.size() * sizeof(uint64_t))) return rc;
+    uint64_t* d_table = (uint64_t*)ctx->d_parts.p;
+    CU_TRY(ctx, cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    uint8_t* o_sha = (flags & B200H_SHA256) ? (uint8_t*)d_sha256 : nullptr;
+    uint8_t* o_md5 = (flags & B200H_MD5) ? (uint8_t*)d_md5 : nullptr;
+    if (int rc = enqueue_device_batch(ctx, (const uint8_t*)d_base, d_table, d_table + nparts, nparts, flags & kPublicFlags,
+                                      o_sha, o_md5, d_trimmed_len, nullptr, st, ln.data()))
+        return rc;
+    if (d_etag_md5) {
+        // MD5 over the concatenated raw part MD5s, on the device like the host entry's (an empty object: md5(""))
+        const uint8_t* etag_src = nparts ? o_md5 : (const uint8_t*)d_table;
+        if (int rc = enqueue_device_batch(ctx, etag_src, d_table + 2 * nparts, d_table + 2 * nparts + 1, 1, B200H_MD5,
+                                          nullptr, (uint8_t*)d_etag_md5, nullptr, nullptr, st, &etag_len))
+            return rc;
+    }
+    return 0;
 }
 
 // ---------------------------------------------------------------------------------------------- files
@@ -1148,11 +1207,7 @@ int b200h_hash_files(b200h_ctx* ctx, const char* const* paths, uint64_t n, const
             len.push_back(sizes[f]);
             file_of.push_back(f);
         } else {
-            for (uint64_t o = 0; o < sizes[f]; o += part_len) {
-                off.push_back(o);
-                len.push_back(std::min(part_len, sizes[f] - o));
-                file_of.push_back(f);
-            }
+            file_of.resize(file_of.size() + split_fixed_parts(sizes[f], part_len, off, len), f);
         }
     }
     if (off.empty()) return 0;

@@ -7,7 +7,9 @@ zero-trimmed 8 MiB block, ``VolumePutFiles2`` missing-block loop, :1345-1574).  
 hashes file by file (ThreadPoolExecutor) or block by block (``to_thread`` under a semaphore); here every path
 queued in the batch is handed to ``blob_utils.get_file_upload_specs`` / ``file_upload_specs2`` -- ONE GPU
 batch for the whole tree -- before the first RPC goes out.  File objects (``BytesIO`` / open files) keep the
-per-object spec builders.
+per-object spec builders.  A ``DeviceFile`` (the bytes of a CUDA tensor) is hashed in GPU memory by the volumefs2
+uploader, and only the trimmed bytes of the blocks the server is missing are copied to the host; the volumefs1 uploader
+reads it like any other stream.
 """
 from __future__ import annotations
 
@@ -49,7 +51,8 @@ class _BatchBase:
         return self
 
     def put_file(self, local_file: Path | str | BinaryIO | BytesIO, remote_path: PurePosixPath | str, mode: int | None = None):
-        """Queue one file (path or readable file object; objects must stay readable until the batch exits)."""
+        """Queue one file (path or readable file object, ``DeviceFile`` included; objects must stay readable and
+        unchanged until the batch exits)."""
         remote = PurePosixPath(remote_path).as_posix()
         if remote.endswith("/"):
             raise ValueError(f"remote_path ({remote}) must refer to a file - cannot end with /")
