@@ -131,6 +131,38 @@ int b200h_hash_fixed_parts_device(b200h_ctx* ctx, const void* d_base, uint64_t l
                                   void* d_sha256, void* d_md5, uint64_t* d_trimmed_len, void* d_etag_md5,
                                   uint64_t* nparts_out, void* cuda_stream);
 
+/* One piece of a segmented device file: len bytes at d_ptr (device memory on ctx's device; may be NULL if len == 0). */
+typedef struct b200h_segment {
+    const void* d_ptr;
+    uint64_t len;
+} b200h_segment;
+
+/* The same split over nfiles virtual files that live in device memory as many buffers: file f is the concatenation of
+ * segs[file_first_seg[f] .. file_first_seg[f+1]) (segs and file_first_seg[nfiles + 1] are host arrays;
+ * file_first_seg[0] == 0, it never decreases and file_first_seg[nfiles] == nsegs).  Every file is cut into
+ * ceil(size / part_len) parts exactly as b200h_hash_fixed_parts_device cuts one buffer; rows are flattened file-major
+ * (like b200h_hash_files), so the parts of all files form ONE batch.  Empty segments and zero-byte files (no rows) are
+ * allowed.  Flags: B200H_SHA256 / B200H_MD5 / B200H_TRIM_ZEROS / B200H_NO_OUTLIERS; no B200H_HEX_OUT, no ETag.
+ * Outputs as in b200h_hash_fixed_parts_device (d_sha256 / d_md5 16-byte aligned, each may be NULL);
+ * *nparts_out = the total row count, returned on the host.
+ * A part that lies inside one segment is hashed where it is (its start need not be aligned).  A part that spans
+ * segments is first copied into one of the context's HBM wave slots (device_bytes / 2 each, the buffers the *_host
+ * entry points stage through) by one gather kernel launch.  When those parts do not fit one slot, the call is split
+ * into waves over contiguous ranges of rows, each costing about one more part's hash time; b200h_segment_parts_preview
+ * shows the split.  Every non-empty segment's first and last byte must be device memory on ctx's device
+ * (cudaPointerGetAttributes); a NULL or foreign pointer is B200H_E_INVALID, and every argument is checked before any
+ * work is enqueued.
+ * The call ONLY ENQUEUES on `cuda_stream` -- except with B200H_TRIM_ZEROS and outlier routing on, where the planner's
+ * count is read back once per wave (synchronising `cuda_stream`, counted by b200h_plan_sync_count);
+ * B200H_TRIM_ZEROS | B200H_NO_OUTLIERS only enqueues.  Growing the wave slots or the part table allocates, which
+ * synchronises the device.
+ * Replaces: the per-8MiB-block loop of _gather_blocks (blob_utils.py:622-645) for a file that lives in HBM as many
+ * buffers (a safetensors image of a state dict), which the reference would serialise in host memory first -- and, with
+ * nfiles > 1, the one-file-at-a-time spec building of the volumefs2 uploader (py/modal/volume.py:1380-1390). */
+int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                    uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
+                                    uint64_t* d_trimmed_len, uint64_t* nparts_out, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.
@@ -202,6 +234,13 @@ int b200h_pack_preview(const uint8_t* base, const uint64_t* offsets, const uint6
  * context nor a GPU.  flags: B200H_SHA256 / B200H_MD5 / B200H_NO_OUTLIERS.  Diagnostic. */
 int b200h_plan_preview(const uint64_t* lengths, uint64_t n, uint32_t flags, uint32_t sm_count, uint32_t* n_chain_out,
                        uint32_t* n_long_out);
+/* How b200h_hash_segment_parts_device splits files made of segments of these lengths, for wave slots of wave_bytes
+ * bytes: the row count, the wave count, and for each of the first out_cap rows (seg_out / wave_out may be NULL) the
+ * segment the part is hashed in place in (UINT64_MAX: the part spans segments and is gathered) and its wave.  The
+ * same code builds the device entry's tables; no context, no GPU.  Argument rules as there (wave_bytes > 0). */
+int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
+                                uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out, uint64_t* nwaves_out,
+                                uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap);
 /* Kernels launched by this context so far (all kinds). */
 uint64_t b200h_launch_count(b200h_ctx* ctx);
 /* Combining queue of b200h_hash_batch_host: GPU batches issued for, and caller requests served by, the small-request

@@ -2,8 +2,8 @@
 
 Drop-in modules (same names as the reference's ``modal/_utils``): ``hash_utils``, ``blob_utils``,
 ``bytes_io_segment_payload``, ``function_utils``, ``parallel_map``.  Additions: ``batch`` (digest
-tables), ``device_file`` (``DeviceFile``: a CUDA tensor as an upload source), ``sharding`` (multi-GPU), ``_lib``
-(ctypes binding of libb200hash.so, C ABI in include/b200hash.h).
+tables), ``device_file`` (``DeviceFile``: a CUDA tensor, or a safetensors image of many, as an upload source),
+``sharding`` (multi-GPU), ``_lib`` (ctypes binding of libb200hash.so, C ABI in include/b200hash.h).
 All arithmetic runs in hand-written sm_90a CUDA; there is no CPU fallback.
 """
 __version__ = "0.1.0"

@@ -33,7 +33,7 @@ ABI_SYMBOLS = (
     "b200h_profile_enable", "b200h_profile_read", "b200h_dedupe_host", "b200h_dedupe_device",
     "b200h_last_outlier_count", "b200h_hash_batch_device_hl", "b200h_combine_stats", "b200h_plan_sync_count",
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
-    "b200h_hash_fixed_parts_device",
+    "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
 )
 
 
@@ -101,6 +101,11 @@ def load_library() -> ctypes.CDLL:
         L.b200h_hash_fixed_parts.restype = i32
         L.b200h_hash_fixed_parts_device.argtypes = [vp, vp, u64, u64, u32, vp, vp, vp, vp, ctypes.POINTER(u64), vp]
         L.b200h_hash_fixed_parts_device.restype = i32
+        L.b200h_hash_segment_parts_device.argtypes = [vp, vp, u64, vp, u64, u64, u32, vp, vp, vp, ctypes.POINTER(u64), vp]
+        L.b200h_hash_segment_parts_device.restype = i32
+        L.b200h_segment_parts_preview.argtypes = [vp, u64, vp, u64, u64, u64, ctypes.POINTER(u64), ctypes.POINTER(u64),
+                                                  vp, vp, u64]
+        L.b200h_segment_parts_preview.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -180,6 +185,37 @@ def pack_preview(base, offsets, lengths, threads: int = 16, slot_bytes: int = 25
     if rc != 0:
         raise B200HashError(f"b200h_pack_preview failed ({rc})")
     return dst, out[: ln.size]
+
+
+#: segment_parts_preview's marker for a part that spans segments and is gathered into a wave slot
+GATHERED = np.iinfo(np.uint64).max
+
+
+def _segment_args(file_first_seg):
+    ffs = np.ascontiguousarray(file_first_seg, dtype=np.uint64)
+    if ffs.ndim != 1 or ffs.size < 1:
+        raise ValueError("file_first_seg needs nfiles + 1 entries")
+    return ffs, ffs.size - 1
+
+
+def segment_parts_preview(seg_lens, file_first_seg, part_len: int, wave_bytes: int):
+    """How ``Context.hash_segment_parts_device`` splits these files (file f = segments file_first_seg[f] ..
+    file_first_seg[f+1]) for wave slots of ``wave_bytes``: -> (seg uint64[nparts]: the segment each part is hashed in
+    place in, or ``GATHERED``; wave uint32[nparts]; number of waves).  The library's own host code; no GPU."""
+    L = load_library()
+    ln = np.ascontiguousarray(seg_lens, dtype=np.uint64)
+    ffs, nfiles = _segment_args(file_first_seg)
+    n, w = ctypes.c_uint64(), ctypes.c_uint64()
+    rc = L.b200h_segment_parts_preview(_np_ptr(ln), ln.size, _np_ptr(ffs), nfiles, part_len, wave_bytes, ctypes.byref(n),
+                                       ctypes.byref(w), None, None, 0)
+    if rc != 0:
+        raise B200HashError(f"b200h_segment_parts_preview failed ({rc})")
+    seg, wave = np.empty(n.value, np.uint64), np.empty(n.value, np.uint32)
+    if n.value:
+        rc = L.b200h_segment_parts_preview(_np_ptr(ln), ln.size, _np_ptr(ffs), nfiles, part_len, wave_bytes, None, None,
+                                           _np_ptr(seg), _np_ptr(wave), n.value)
+        assert rc == 0
+    return seg, wave, int(w.value)
 
 
 class Context:
@@ -356,6 +392,25 @@ class Context:
                                                    d_md5 or None, d_trimmed or None, d_etag or None, ctypes.byref(got),
                                                    stream or None)
         self._check(rc, "b200h_hash_fixed_parts_device")
+        return int(got.value)
+
+    def hash_segment_parts_device(self, seg_ptrs, seg_lens, file_first_seg, part_len: int, flags: int, d_sha: int = 0,
+                                  d_md5: int = 0, d_trimmed: int = 0, stream: int = 0) -> int:
+        """``hash_fixed_parts_device`` over files made of device buffers: file f is the concatenation of segments
+        file_first_seg[f] .. file_first_seg[f+1] (segment s: seg_lens[s] bytes at device address seg_ptrs[s]).  Every
+        file's parts, file-major, form one batch; outputs hold that many rows.  Returns the row count."""
+        ptrs = np.ascontiguousarray(seg_ptrs, dtype=np.uint64)
+        lens = np.ascontiguousarray(seg_lens, dtype=np.uint64)
+        if ptrs.shape != lens.shape or ptrs.ndim != 1:
+            raise ValueError("seg_ptrs and seg_lens must be 1-D and of equal length")
+        segs = np.empty((lens.size, 2), np.uint64)  # b200h_segment {d_ptr, len}
+        segs[:, 0], segs[:, 1] = ptrs, lens
+        ffs, nfiles = _segment_args(file_first_seg)
+        got = ctypes.c_uint64()
+        rc = self._L.b200h_hash_segment_parts_device(self._h, _np_ptr(segs) if lens.size else None, lens.size, _np_ptr(ffs),
+                                                     nfiles, part_len, flags, d_sha or None, d_md5 or None,
+                                                     d_trimmed or None, ctypes.byref(got), stream or None)
+        self._check(rc, "b200h_hash_segment_parts_device")
         return int(got.value)
 
     # -- files: stat + read + hash entirely inside the library (native reader threads, no mmap / Python I/O)

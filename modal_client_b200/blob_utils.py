@@ -43,7 +43,7 @@ from ._logging import logger
 from ._wire import BlobCreateRequest
 from .async_utils import asyncnullcontext, bounded_map, gather_cancel_on_error, retry
 from .bytes_io_segment_payload import BytesIOSegmentPayload, KnownBytesBody
-from .device_file import DeviceFile
+from .device_file import DeviceFile, hash_parts_many
 from .exception import ExecutionError
 from .hash_utils import UploadHashes, get_upload_hashes
 from .http_utils import ClientSessionRegistry
@@ -903,6 +903,34 @@ async def file_upload_specs2(
         finally:
             if gc_was_on:
                 gc.enable()
+        return out
+
+    return await asyncio.to_thread(run)
+
+
+async def device_file_specs2(
+    items: Sequence[tuple[DeviceFile, PurePosixPath, int]],
+) -> list[FileUploadSpec2]:
+    """Batched ``FileUploadSpec2.from_fileobj`` for the ``DeviceFile``s of one ``batch_upload``: the blocks of ALL of
+    them, whatever tensors they are made of, are trimmed and hashed by one ``b200h_hash_segment_parts_device`` call,
+    and only that table comes to the host.  A single file is ``from_fileobj`` itself."""
+    if not items:
+        return []
+    if len(items) == 1:
+        fp, remote, mode = items[0]
+        return [await FileUploadSpec2.from_fileobj(fp, remote, asyncio.Semaphore(1), mode)]
+
+    def run() -> list[FileUploadSpec2]:
+        files = [fp for fp, _, _ in items]
+        sha, _, trimmed = hash_parts_many(files, BLOCK_SIZE, _lib.SHA256 | _lib.TRIM_ZEROS, ctx=get_context())
+        out, row = [], 0
+        for fp, remote, mode in items:
+            n = -(-fp.nbytes // BLOCK_SIZE)
+            out.append(FileUploadSpec2(source=fp.reopen, source_description=repr(fp),
+                                       path=PurePosixPath(remote).as_posix(),
+                                       blocks=_blocks_from_table(sha[row : row + n], trimmed[row : row + n]),
+                                       mode=mode & 0o7777, size=fp.nbytes))
+            row += n
         return out
 
     return await asyncio.to_thread(run)

@@ -150,6 +150,7 @@ struct b200h_ctx {
     size_t dwave_want = 0;
     DevBuf d_off, d_len, d_order, d_order_long, d_trim, d_sha, d_md5, d_scratch, d_small, d_states, d_dedupe, d_keys, d_trimctl, d_hex;
     DevBuf d_parts;  // part table of b200h_hash_fixed_parts_device: offsets | lengths | the ETag message (offset, length)
+                     // (b200h_hash_segment_parts_device: absolute addresses | lengths | gather tiles)
     uint64_t* h_meta = nullptr;  // pinned: offsets then lengths
     size_t h_meta_cap = 0;       // in uint64 elements
     uint64_t launches = 0;
@@ -667,7 +668,8 @@ int hash_batch_host_impl(b200h_ctx* ctx, const uint8_t* base, const uint64_t* of
     for (size_t wi = 0; wi < waves.size(); ++wi) {
         const Wave& w = waves[wi];
         const int slot = (int)(wi & 1);
-        if (wi >= 2) CU_TRY(ctx, cudaStreamWaitEvent(ctx->s_copy, ctx->ev_consumed[slot], 0));
+        // the slot's last reader: an earlier wave of this batch, or b200h_hash_segment_parts_device on another stream
+        CU_TRY(ctx, cudaStreamWaitEvent(ctx->s_copy, ctx->ev_consumed[slot], 0));
         // a segment wave is message w.i0 restricted to [seg_start, seg_start + bytes), placed at device offset 0
         const uint64_t seg_off1 = w.seg ? off[w.i0] + w.seg_start : 0, seg_len1 = w.bytes, seg_doff1 = 0;
         const uint64_t seg_file1 = (w.seg && file_of) ? file_of[w.i0] : 0;
@@ -788,6 +790,78 @@ uint64_t split_fixed_parts(uint64_t len, uint64_t part_len, std::vector<uint64_t
         ln.push_back(std::min(part_len, len - o));
     }
     return nparts;
+}
+
+constexpr uint64_t kInPlace = ~0ull;
+
+// Where every part of a segmented batch is hashed: b200h_segment_parts_preview reports it, and
+// b200h_hash_segment_parts_device builds its tables from it.  File f is the concatenation of segments
+// [file_first_seg[f], file_first_seg[f + 1]); its parts are cut by split_fixed_parts and listed file-major.  A part
+// that lies inside one segment is hashed where it is; a part that spans two or more segments is gathered into a wave
+// slot at the next multiple of 16.  Waves are contiguous ranges of parts: a new wave starts at the gathered part that
+// would take the current wave's staging beyond wave_cap (a wave always takes its first gathered part, so a part larger
+// than wave_cap gets a wave of its own).  Parts without a gathered part between them share a wave.
+struct SegmentParts {
+    std::vector<uint64_t> off, len;  // part i: bytes [off[i], off[i] + len[i]) of its file
+    std::vector<uint64_t> seg;       // the segment holding the part's first byte
+    std::vector<uint64_t> seg_off;   // offset of that byte inside the segment
+    std::vector<uint64_t> stage;     // offset of a gathered part in its wave slot; kInPlace for an in-place part
+    std::vector<uint32_t> wave;      // the wave of every part
+    std::vector<uint64_t> wave_first;  // first part of every wave, then nparts
+    std::vector<uint64_t> wave_bytes;  // staged bytes of every wave
+};
+
+// Fills `p`; returns 0, or B200H_E_INVALID with the reason in `err`.
+int layout_segment_parts(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
+                         uint64_t part_len, uint64_t wave_cap, SegmentParts& p, std::string& err) {
+    if (part_len == 0) return err = "part_len must be > 0", B200H_E_INVALID;
+    if (wave_cap == 0) return err = "wave_bytes must be > 0", B200H_E_INVALID;
+    if (nsegs && !seg_lens) return err = "segments must not be NULL", B200H_E_INVALID;
+    if (!file_first_seg) return err = "file_first_seg must not be NULL (it has nfiles + 1 entries)", B200H_E_INVALID;
+    if (file_first_seg[0] != 0) return err = "file_first_seg[0] must be 0", B200H_E_INVALID;
+    if (file_first_seg[nfiles] != nsegs) return err = "file_first_seg[nfiles] must equal nsegs", B200H_E_INVALID;
+    for (uint64_t f = 0; f < nfiles; ++f)
+        if (file_first_seg[f + 1] < file_first_seg[f]) return err = "file_first_seg must not decrease", B200H_E_INVALID;
+    for (uint64_t f = 0; f < nfiles; ++f) {
+        const uint64_t a = file_first_seg[f], b = file_first_seg[f + 1];
+        uint64_t size = 0;
+        for (uint64_t s = a; s < b; ++s) {
+            if (size + seg_lens[s] < size) return err = "a file is larger than 2^64 - 1 bytes", B200H_E_INVALID;
+            size += seg_lens[s];
+        }
+        const size_t first = p.off.size();
+        split_fixed_parts(size, part_len, p.off, p.len);
+        uint64_t s = a, s_start = 0;  // segment s holds file bytes [s_start, s_start + seg_lens[s])
+        for (size_t i = first; i < p.off.size(); ++i) {
+            while (s_start + seg_lens[s] <= p.off[i]) s_start += seg_lens[s++];  // skips empty segments too
+            p.seg.push_back(s);
+            p.seg_off.push_back(p.off[i] - s_start);
+            p.stage.push_back(p.off[i] + p.len[i] <= s_start + seg_lens[s] ? kInPlace : 0);
+        }
+    }
+    const uint64_t nparts = p.off.size();
+    p.wave.resize(nparts);
+    uint64_t used = 0;
+    for (uint64_t i = 0; i < nparts; ++i) {
+        if (i == 0) {
+            p.wave_first.push_back(0);
+            p.wave_bytes.push_back(0);
+        }
+        if (p.stage[i] != kInPlace) {
+            const uint64_t need = (p.len[i] + 15) & ~15ull;
+            if (used && used + need > wave_cap) {
+                p.wave_first.push_back(i);
+                p.wave_bytes.push_back(0);
+                used = 0;
+            }
+            p.stage[i] = used;
+            used += need;
+            p.wave_bytes.back() = used;
+        }
+        p.wave[i] = (uint32_t)(p.wave_first.size() - 1);
+    }
+    p.wave_first.push_back(nparts);
+    return 0;
 }
 
 // A small request from one of possibly many concurrent callers: merge it with whatever else arrives while the context
@@ -1156,6 +1230,108 @@ int b200h_hash_fixed_parts_device(b200h_ctx* ctx, const void* d_base, uint64_t l
         if (int rc = enqueue_device_batch(ctx, etag_src, d_table + 2 * nparts, d_table + 2 * nparts + 1, 1, B200H_MD5,
                                           nullptr, (uint8_t*)d_etag_md5, nullptr, nullptr, st, &etag_len))
             return rc;
+    }
+    return 0;
+}
+
+int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                    uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
+                                    uint64_t* d_trimmed_len, uint64_t* nparts_out, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_hash_segment_parts_device");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
+    if (((uintptr_t)d_sha256 | (uintptr_t)d_md5) & 15u)
+        return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
+    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
+    std::vector<uint64_t> seg_lens(nsegs);
+    for (uint64_t s = 0; s < nsegs; ++s) {
+        if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
+        seg_lens[s] = segs[s].len;
+    }
+    SegmentParts p;
+    std::string err;
+    if (int rc = layout_segment_parts(seg_lens.data(), nsegs, file_first_seg, nfiles, part_len,
+                                      std::max(ctx->dwave_cap, ctx->dwave_want), p, err))
+        return fail(ctx, rc, err);
+    const uint64_t nparts = p.off.size();
+    if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
+        return fail(ctx, B200H_E_INVALID, "flags select neither SHA256 nor MD5");
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    // A pointer that is not memory of this device would fault the kernels; reject it before anything is enqueued.
+    // (Both ends of every segment are checked; the allocation in between is the caller's promise.)
+    for (uint64_t s = 0; s < nsegs; ++s) {
+        if (!segs[s].len) continue;
+        for (const uint8_t* q : {(const uint8_t*)segs[s].d_ptr, (const uint8_t*)segs[s].d_ptr + (segs[s].len - 1)}) {
+            cudaPointerAttributes at;
+            const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess &&
+                            (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == ctx->device;
+            cudaGetLastError();
+            if (!ok)
+                return fail(ctx, B200H_E_INVALID,
+                            "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
+        }
+    }
+    if (nparts_out) *nparts_out = nparts;
+    if (nparts == 0) return 0;
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    uint64_t stage_max = 0;
+    for (uint64_t b : p.wave_bytes) stage_max = std::max(stage_max, b);
+    if (stage_max)
+        if (int rc = ensure_wave(ctx, stage_max)) return rc;
+
+    // device table: part addresses | part lengths | gather tiles (after the gather, every part is an absolute address)
+    const size_t nwaves = p.wave_bytes.size();
+    std::vector<uint64_t> table(2 * nparts);
+    std::vector<uint64_t> wave_tiles(nwaves + 1, 0);  // tiles of wave w: [wave_tiles[w], wave_tiles[w + 1])
+    std::vector<GatherTile> tiles;
+    for (size_t w = 0; w < nwaves; ++w) {
+        uint8_t* slot = ctx->dwave[w & 1];
+        for (uint64_t i = p.wave_first[w]; i < p.wave_first[w + 1]; ++i) {
+            table[nparts + i] = p.len[i];
+            if (p.stage[i] == kInPlace) {
+                table[i] = (uint64_t)(uintptr_t)segs[p.seg[i]].d_ptr + p.seg_off[i];
+                continue;
+            }
+            table[i] = (uint64_t)(uintptr_t)(slot + p.stage[i]);
+            uint64_t s = p.seg[i], so = p.seg_off[i], done = 0;
+            while (done < p.len[i]) {
+                const uint64_t piece = std::min(seg_lens[s] - so, p.len[i] - done);
+                for (uint64_t t = 0; t < piece; t += kGatherTileBytes)
+                    tiles.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + so + t, table[i] + done + t,
+                                     std::min(kGatherTileBytes, piece - t)});
+                done += piece;
+                ++s;
+                so = 0;
+            }
+        }
+        wave_tiles[w + 1] = tiles.size();
+    }
+    const size_t table_bytes = table.size() * sizeof(uint64_t), tiles_bytes = tiles.size() * sizeof(GatherTile);
+    // The table is context scratch like the planner's: it is rewritten only after the last batch that read it.
+    if (ctx->scratch_used) CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_scratch, 0));
+    if (int rc = ensure_dev(ctx, ctx->d_parts, table_bytes + tiles_bytes)) return rc;
+    uint64_t* d_table = (uint64_t*)ctx->d_parts.p;
+    GatherTile* d_tiles = (GatherTile*)(d_table + table.size());
+    CU_TRY(ctx, cudaMemcpyAsync(d_table, table.data(), table_bytes, cudaMemcpyHostToDevice, st));
+    if (tiles_bytes) CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tiles_bytes, cudaMemcpyHostToDevice, st));
+    uint8_t* o_sha = (flags & B200H_SHA256) ? (uint8_t*)d_sha256 : nullptr;
+    uint8_t* o_md5 = (flags & B200H_MD5) ? (uint8_t*)d_md5 : nullptr;
+    for (size_t w = 0; w < nwaves; ++w) {
+        const uint64_t i0 = p.wave_first[w], cnt = p.wave_first[w + 1] - i0;
+        const int slot = (int)(w & 1);
+        const bool staged = wave_tiles[w + 1] > wave_tiles[w];
+        if (staged) {
+            // the slot is shared with the *_host entry points and the previous waves: wait for its last reader
+            CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_consumed[slot], 0));
+            ctx->launches += launch_gather_segments(d_tiles + wave_tiles[w], wave_tiles[w + 1] - wave_tiles[w], st);
+            CU_TRY(ctx, cudaGetLastError());
+        }
+        if (int rc = enqueue_device_batch(ctx, nullptr, d_table + i0, d_table + nparts + i0, cnt, flags & kPublicFlags,
+                                          o_sha ? o_sha + 32 * i0 : nullptr, o_md5 ? o_md5 + 16 * i0 : nullptr,
+                                          d_trimmed_len ? d_trimmed_len + i0 : nullptr, nullptr, st, p.len.data() + i0))
+            return rc;
+        if (staged) CU_TRY(ctx, cudaEventRecord(ctx->ev_consumed[slot], st));
     }
     return 0;
 }
@@ -1531,6 +1707,22 @@ int b200h_plan_preview(const uint64_t* lengths, uint64_t n, uint32_t flags, uint
     const uint32_t n_chain = plan_outliers_host(lengths, n, max_chain, sm_count, long_cap, plan_ratio8(flags & 3u), &n_long);
     if (n_chain_out) *n_chain_out = n_chain;
     if (n_long_out) *n_long_out = n_long;
+    return 0;
+}
+
+int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
+                                uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out, uint64_t* nwaves_out,
+                                uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap) {
+    SegmentParts p;
+    std::string err;
+    if (int rc = layout_segment_parts(seg_lens, nsegs, file_first_seg, nfiles, part_len, wave_bytes, p, err)) return rc;
+    const uint64_t nparts = p.off.size();
+    if (nparts_out) *nparts_out = nparts;
+    if (nwaves_out) *nwaves_out = p.wave_bytes.size();
+    for (uint64_t i = 0; i < std::min(nparts, out_cap); ++i) {
+        if (seg_out) seg_out[i] = p.stage[i] == kInPlace ? p.seg[i] : kInPlace;
+        if (wave_out) wave_out[i] = p.wave[i];
+    }
     return 0;
 }
 

@@ -1661,6 +1661,45 @@ int launch_hex_rows(const uint8_t* in, uint64_t nbytes, uint8_t* out, cudaStream
     return 1;
 }
 
+// One tile of gather_segments_kernel: dst[0..len) = src[0..len), V-wide where both pointers agree mod sizeof(V).
+// The bytes before dst's first V boundary and after the last whole V go one at a time.
+template <typename V>
+__device__ __forceinline__ void copy_tile(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t len) {
+    constexpr uint32_t W = sizeof(V);
+    const uint32_t head = min(len, (uint32_t)((W - ((uintptr_t)dst & (W - 1))) & (W - 1)));
+    const uint32_t nv = (len - head) / W;
+    for (uint32_t i = threadIdx.x; i < head; i += blockDim.x) dst[i] = src[i];
+    const V* sv = reinterpret_cast<const V*>(src + head);
+    V* dv = reinterpret_cast<V*>(dst + head);
+    for (uint32_t i = threadIdx.x; i < nv; i += blockDim.x) dv[i] = sv[i];
+    for (uint32_t i = head + nv * W + threadIdx.x; i < len; i += blockDim.x) dst[i] = src[i];
+}
+
+// Copies the pieces of the parts that straddle segments into a wave slot (b200h_hash_segment_parts_device): one CTA
+// per tile at a time.  The widest access both addresses allow: 16 bytes when source and destination agree mod 16
+// (the destination of a part's first piece always is 16-byte aligned), down to single bytes.
+__global__ void __launch_bounds__(256) gather_segments_kernel(const GatherTile* __restrict__ tiles, uint64_t ntiles) {
+    for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const GatherTile g = tiles[t];
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(g.src);
+        uint8_t* dst = reinterpret_cast<uint8_t*>(g.dst);
+        const uint32_t len = (uint32_t)g.len;
+        const uint32_t phase = (uint32_t)(g.src ^ g.dst);
+        if (!(phase & 15u)) copy_tile<uint4>(src, dst, len);
+        else if (!(phase & 7u)) copy_tile<uint2>(src, dst, len);
+        else if (!(phase & 3u)) copy_tile<uint32_t>(src, dst, len);
+        else if (!(phase & 1u)) copy_tile<uint16_t>(src, dst, len);
+        else copy_tile<uint8_t>(src, dst, len);
+    }
+}
+
+int launch_gather_segments(const GatherTile* tiles, uint64_t ntiles, cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t g = ntiles < (uint64_t)g_sm_count * 16 ? ntiles : (uint64_t)g_sm_count * 16;
+    gather_segments_kernel<<<(int)g, 256, 0, st>>>(tiles, ntiles);
+    return 1;
+}
+
 // --------------------------------------------------------------------------------- launch wrappers
 
 static int grid_for(uint64_t n, int threads, int cap) {

@@ -82,6 +82,13 @@ int launch_dedupe(const void* d_keys, uint64_t n, uint32_t key_bytes, uint32_t* 
 int launch_fill_synth(uint8_t* dst, uint64_t nbytes, uint64_t seed, uint64_t start, cudaStream_t st);
 // out[2*nbytes] = lowercase ASCII hex of in[nbytes] (nbytes a multiple of 4, both 8-byte aligned)
 int launch_hex_rows(const uint8_t* in, uint64_t nbytes, uint8_t* out, cudaStream_t st);
+// One piece of device memory to copy: absolute addresses, len <= kGatherTileBytes.
+struct GatherTile {
+    uint64_t src, dst, len;
+};
+constexpr uint64_t kGatherTileBytes = 64 << 10;
+// Every tile's copy, in one launch (any alignment of src and dst).
+int launch_gather_segments(const GatherTile* tiles, uint64_t ntiles, cudaStream_t st);
 
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)

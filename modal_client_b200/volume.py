@@ -8,8 +8,9 @@ hashes file by file (ThreadPoolExecutor) or block by block (``to_thread`` under 
 queued in the batch is handed to ``blob_utils.get_file_upload_specs`` / ``file_upload_specs2`` -- ONE GPU
 batch for the whole tree -- before the first RPC goes out.  File objects (``BytesIO`` / open files) keep the
 per-object spec builders.  A ``DeviceFile`` (the bytes of a CUDA tensor) is hashed in GPU memory by the volumefs2
-uploader, and only the trimmed bytes of the blocks the server is missing are copied to the host; the volumefs1 uploader
-reads it like any other stream.
+uploader -- all of a batch's ``DeviceFile``s, safetensors images of whole state dicts included, in one device call
+(``blob_utils.device_file_specs2``) -- and only the trimmed bytes of the blocks the server is missing are copied to the
+host; the volumefs1 uploader reads it like any other stream.
 """
 from __future__ import annotations
 
@@ -28,6 +29,7 @@ from . import _wire, blob_utils
 from ._logging import logger
 from .async_utils import bounded_map, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
+from .device_file import DeviceFile
 from .exception import ExecutionError
 from .http_utils import ClientSessionRegistry
 
@@ -175,9 +177,14 @@ class VolumeUploadContextManager2(_BatchBase):
         if exc_val:
             return
         specs: list[FileUploadSpec2] = await blob_utils.file_upload_specs2(self._paths)
+        # every DeviceFile of the batch: one device call; the specs keep put_file order
+        device_specs = iter(await blob_utils.device_file_specs2([o for o in self._fileobjs if isinstance(o[0], DeviceFile)]))
         one_at_a_time = asyncio.Semaphore(1)
         for fp, remote, mode in self._fileobjs:
-            specs.append(await FileUploadSpec2.from_fileobj(fp, remote, one_at_a_time, mode))
+            if isinstance(fp, DeviceFile):
+                specs.append(next(device_specs))
+            else:
+                specs.append(await FileUploadSpec2.from_fileobj(fp, remote, one_at_a_time, mode))
         await self._put_file_specs(specs)
 
     async def _put_file_specs(self, file_specs: list[FileUploadSpec2]):
