@@ -163,6 +163,23 @@ int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, u
                                     uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
                                     uint64_t* d_trimmed_len, uint64_t* nparts_out, void* cuda_stream);
 
+/* CRC-32 of n device ranges: d_crc_out[i] (a DEVICE array of n uint32, 4-byte aligned) = zlib.crc32 of
+ * ranges[i].len bytes at ranges[i].d_ptr (IEEE polynomial, reflected, initial value and final XOR 0xFFFFFFFF): the
+ * checksum a zip archive stores for every record, such as those of a torch.save file.  Any start alignment, any length
+ * (0 gives 0).  `ranges` is a host array; every non-empty range's first and last byte, and the first and last word of
+ * d_crc_out, must be device memory on ctx's device (cudaPointerGetAttributes): a NULL or foreign pointer is
+ * B200H_E_INVALID, and every argument is checked before any work is enqueued.
+ * The work is spread by bytes, not by ranges: every range is cut into 16 KiB chunks and the grid's warps take equal runs
+ * of them, so one huge range occupies the whole GPU and many small ranges share warps.  One kernel launch
+ * (crc32_chunks_kernel) per call whatever n is, none when every range is empty.  The host writes each range's length
+ * term to d_crc_out first (CRC arithmetic on the lengths; the library never hashes bytes on the CPU) and the kernel
+ * XORs the bytes' contribution into it.  The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream):
+ * its small range table lives in a stream-ordered allocation (cudaMallocAsync / cudaFreeAsync), so it never
+ * synchronises.
+ * Replaces: the CRC-32 torch.save computes on the host over every storage after copying it there
+ * (torch/serialization.py _save -> PyTorchStreamWriter::writeRecord), for a checkpoint that lives in HBM. */
+int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, uint32_t* d_crc_out, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

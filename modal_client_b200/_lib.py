@@ -34,6 +34,7 @@ ABI_SYMBOLS = (
     "b200h_last_outlier_count", "b200h_hash_batch_device_hl", "b200h_combine_stats", "b200h_plan_sync_count",
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
+    "b200h_crc32_device",
 )
 
 
@@ -42,7 +43,7 @@ class B200HashError(RuntimeError):
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    srcs = [os.path.join(CSRC, f) for f in ("b200hash_kernels.cu", "b200hash_dedupe.cu", "b200hash_api.cu",
+    srcs = [os.path.join(CSRC, f) for f in ("b200hash_kernels.cu", "b200hash_dedupe.cu", "b200hash_crc32.cu", "b200hash_api.cu",
                                             "b200blob_host.cpp", "b200pack_copy.cpp", "b200hash_kernels.cuh", "b200pack_team.h")]
     srcs += [os.path.join(os.path.dirname(_PKG), "include", h) for h in ("b200hash.h", "b200blob.h")]
     stale = not os.path.exists(LIB_PATH) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
@@ -106,6 +107,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_segment_parts_preview.argtypes = [vp, u64, vp, u64, u64, u64, ctypes.POINTER(u64), ctypes.POINTER(u64),
                                                   vp, vp, u64]
         L.b200h_segment_parts_preview.restype = i32
+        L.b200h_crc32_device.argtypes = [vp, vp, u64, vp, vp]
+        L.b200h_crc32_device.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -412,6 +415,19 @@ class Context:
                                                      d_trimmed or None, ctypes.byref(got), stream or None)
         self._check(rc, "b200h_hash_segment_parts_device")
         return int(got.value)
+
+    def crc32_device(self, ptrs, lens, d_out: int, stream: int = 0) -> None:
+        """zlib.crc32 of every device range (lens[i] bytes at device address ptrs[i]) into the device uint32 array at
+        ``d_out``, computed on the device; the work is only enqueued on ``stream``."""
+        p = np.ascontiguousarray(ptrs, dtype=np.uint64)
+        ln = np.ascontiguousarray(lens, dtype=np.uint64)
+        if p.shape != ln.shape or p.ndim != 1:
+            raise ValueError("ptrs and lens must be 1-D and of equal length")
+        ranges = np.empty((ln.size, 2), np.uint64)  # b200h_segment {d_ptr, len}
+        ranges[:, 0], ranges[:, 1] = p, ln
+        rc = self._L.b200h_crc32_device(self._h, _np_ptr(ranges) if ln.size else None, ln.size, d_out or None,
+                                        stream or None)
+        self._check(rc, "b200h_crc32_device")
 
     # -- files: stat + read + hash entirely inside the library (native reader threads, no mmap / Python I/O)
     @staticmethod

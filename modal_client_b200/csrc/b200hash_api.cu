@@ -1336,6 +1336,64 @@ int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, u
     return 0;
 }
 
+int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, uint32_t* d_crc_out, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_crc32_device");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (n && !ranges) return fail(ctx, B200H_E_INVALID, "ranges must not be NULL");
+    if (n && !d_crc_out) return fail(ctx, B200H_E_INVALID, "d_crc_out must not be NULL");
+    if ((uintptr_t)d_crc_out & 3u) return fail(ctx, B200H_E_INVALID, "d_crc_out must be 4-byte aligned");
+    for (uint64_t i = 0; i < n; ++i) {
+        if (ranges[i].len && !ranges[i].d_ptr) return fail(ctx, B200H_E_INVALID, "range " + std::to_string(i) + " is NULL");
+        if ((uintptr_t)ranges[i].d_ptr + ranges[i].len < (uintptr_t)ranges[i].d_ptr)
+            return fail(ctx, B200H_E_INVALID, "range " + std::to_string(i) + " wraps the address space");
+    }
+    if (n == 0) return 0;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    // A pointer that is not memory of this device would fault the kernel; reject it before anything is enqueued.
+    // (Both ends of every range and of the output are checked; the allocation in between is the caller's promise.)
+    auto on_device = [&](const void* q) {
+        cudaPointerAttributes at;
+        const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess &&
+                        (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == ctx->device;
+        cudaGetLastError();
+        return ok;
+    };
+    for (uint64_t i = 0; i < n; ++i) {
+        if (!ranges[i].len) continue;
+        const uint8_t* p = (const uint8_t*)ranges[i].d_ptr;
+        if (!on_device(p) || !on_device(p + (ranges[i].len - 1)))
+            return fail(ctx, B200H_E_INVALID,
+                        "range " + std::to_string(i) + " is not device memory on cuda:" + std::to_string(ctx->device));
+    }
+    if (!on_device(d_crc_out) || !on_device(d_crc_out + (n - 1)))
+        return fail(ctx, B200H_E_INVALID, "d_crc_out is not device memory on cuda:" + std::to_string(ctx->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    // device table: ranges | chunk prefix (n + 1); the output starts as every range's length term
+    std::vector<CrcRange> rs(n);
+    std::vector<uint64_t> first(n + 1, 0);
+    std::vector<uint32_t> init(n);
+    for (uint64_t i = 0; i < n; ++i) {
+        rs[i] = {(uint64_t)(uintptr_t)ranges[i].d_ptr, ranges[i].len};
+        first[i + 1] = first[i] + (ranges[i].len + kCrcChunkBytes - 1) / kCrcChunkBytes;
+        init[i] = crc32_length_term(ranges[i].len);
+    }
+    CU_TRY(ctx, cudaMemcpyAsync(d_crc_out, init.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    if (first[n] == 0) return 0;
+    // stream-ordered allocation: no synchronisation, and no scratch shared with other streams' calls
+    const size_t rs_bytes = n * sizeof(CrcRange), bytes = rs_bytes + (n + 1) * sizeof(uint64_t);
+    void* d_table = nullptr;
+    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
+    CrcRange* d_ranges = (CrcRange*)d_table;
+    uint64_t* d_first = (uint64_t*)((uint8_t*)d_table + rs_bytes);
+    CU_TRY(ctx, cudaMemcpyAsync(d_ranges, rs.data(), rs_bytes, cudaMemcpyHostToDevice, st));
+    CU_TRY(ctx, cudaMemcpyAsync(d_first, first.data(), (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_crc32(d_ranges, d_first, n, first[n], d_crc_out, st);
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaFreeAsync(d_table, st));
+    return 0;
+}
+
 // ---------------------------------------------------------------------------------------------- files
 
 int b200h_stat_files(b200h_ctx* ctx, const char* const* paths, uint64_t n, uint64_t* sizes_out, uint32_t* modes_out) {

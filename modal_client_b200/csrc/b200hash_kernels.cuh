@@ -90,6 +90,20 @@ constexpr uint64_t kGatherTileBytes = 64 << 10;
 // Every tile's copy, in one launch (any alignment of src and dst).
 int launch_gather_segments(const GatherTile* tiles, uint64_t ntiles, cudaStream_t st);
 
+// CRC-32 of device ranges (b200hash_crc32.cu).  A range of L bytes is ceil(L / kCrcChunkBytes) chunks, cut from its end.
+struct CrcRange {
+    uint64_t ptr, len;
+};
+constexpr uint64_t kCrcChunkBytes = 16 << 10;
+// first[n + 1]: range r owns chunks [first[r], first[r + 1]), nchunks = first[n].  out[r] must hold
+// crc32_length_term(len_r) before the launch; the kernel XORs the bytes' contribution into it.  Launches nothing when
+// nchunks == 0; returns the number of kernels launched.
+int launch_crc32(const CrcRange* ranges, const uint64_t* first, uint64_t n, uint64_t nchunks, uint32_t* out,
+                 cudaStream_t st);
+// zlib.crc32 of `len` zero-contribution bytes: the 0xFFFFFFFF start register shifted through len bytes, XOR 0xFFFFFFFF
+// (host arithmetic on CRC values; no data involved)
+uint32_t crc32_length_term(uint64_t len);
+
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)
 cudaError_t configure_kernels();  // one-time cudaFuncSetAttribute calls for the current device

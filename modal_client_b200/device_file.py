@@ -94,6 +94,26 @@ class _TensorBytes:
         return torch.frombuffer(bytearray(data), dtype=torch.uint8).to(f"cuda:{ctx.device}")
 
     @classmethod
+    def _pinned(cls, n: int):
+        import torch
+
+        return torch.empty(n, dtype=torch.uint8, pin_memory=True)
+
+    @classmethod
+    def _empty(cls, n: int, ctx):
+        import torch
+
+        return torch.empty(n, dtype=torch.uint8, device=f"cuda:{ctx.device}")
+
+    @classmethod
+    def _current_stream(cls, ctx) -> int:
+        """The current stream as the library takes it.  PyTorch's default stream is the legacy NULL stream, but a NULL
+        stream means the context's own stream to the library, so it is named cudaStreamLegacy (1) instead."""
+        import torch
+
+        return torch.cuda.current_stream(ctx.device).cuda_stream or 1
+
+    @classmethod
     def _check_tensor(cls, tensor, ctx, label: str):
         """Raises ``ValueError`` unless ``tensor`` can be a segment; returns the context (``get_context()`` if None)."""
         if getattr(getattr(tensor, "device", None), "type", None) != cls.device_type:
@@ -257,6 +277,224 @@ def safetensors_layout(tensors: Mapping, metadata: Mapping | None = None):
     return len(text).to_bytes(8, "little") + text, ordered
 
 
+# -------------------------------------------------------------------------------------------- torch.save
+#
+# A torch.save file is a zip archive of stored (uncompressed) records: data.pkl, a few small ones, one ``data/<key>``
+# record per storage holding the whole untyped storage, ``version`` and last ``.data/serialization_id``, then the
+# central directory.  ``torch.save`` under ``torch.serialization.skip_data()`` writes all of it except the storage
+# bytes, which it skips with ``seek(n, SEEK_CUR)``; in that skeleton the CRC-32 of every data record is 0, and so is
+# its contribution to the last 20 digits of the serialization id.  DeviceFile.torch_save keeps the skeleton's pieces
+# on the host, takes the storages where they are, has their CRC-32s computed on the device and writes them (and the
+# id they determine) into the skeleton.
+
+_ZIP_LOCAL, _ZIP_CENTRAL, _ZIP_DESCRIPTOR = 0x04034B50, 0x02014B50, 0x08074B50
+_ZIP_END, _ZIP64_END, _ZIP64_LOCATOR = 0x06054B50, 0x06064B50, 0x07064B50
+_ID_RECORD = ".data/serialization_id"
+_MASK64 = (1 << 64) - 1
+
+
+class _SkeletonWriter:
+    """The ``f`` torch.save writes into under ``skip_data()``: keeps its writes as pieces and the skipped spans as
+    gaps (where the storages go), never a checkpoint-sized buffer."""
+
+    def __init__(self):
+        self.pieces: list[tuple[int, bytearray]] = []  # (file offset, bytes), in file order
+        self.gaps: list[tuple[int, int]] = []  # (file offset, length) of every skipped span
+        self.pos = 0
+
+    def write(self, b) -> int:
+        b = memoryview(b).cast("B")
+        if self.pieces and self.pieces[-1][0] + len(self.pieces[-1][1]) == self.pos:
+            self.pieces[-1][1].extend(b)
+        else:
+            self.pieces.append((self.pos, bytearray(b)))
+        self.pos += len(b)
+        return len(b)
+
+    def seek(self, offset: int, whence: int = os.SEEK_SET) -> int:
+        if whence != os.SEEK_CUR or offset < 0:
+            raise ValueError("torch.save skeleton: only forward relative seeks are expected")
+        if offset:
+            self.gaps.append((self.pos, offset))
+        self.pos += offset
+        return self.pos
+
+    def tell(self) -> int:
+        return self.pos
+
+    def flush(self):
+        pass
+
+
+class _Skeleton:
+    """Read / patch the skeleton's bytes by file offset (every field lies inside one piece)."""
+
+    def __init__(self, pieces):
+        self.pieces = pieces
+        self.starts = [o for o, _ in pieces]
+
+    def _at(self, off: int, n: int):
+        k = bisect.bisect_right(self.starts, off) - 1
+        if k < 0 or off + n > self.starts[k] + len(self.pieces[k][1]):
+            raise ValueError(f"torch.save layout: bytes [{off}, {off + n}) are not in the skeleton")
+        return self.pieces[k][1], off - self.starts[k]
+
+    def read(self, off: int, n: int) -> bytes:
+        buf, at = self._at(off, n)
+        return bytes(buf[at : at + n])
+
+    def u(self, off: int, n: int) -> int:
+        return int.from_bytes(self.read(off, n), "little")
+
+    def patch(self, off: int, data: bytes):
+        buf, at = self._at(off, len(data))
+        buf[at : at + len(data)] = data
+
+
+class _ZipRecord:
+    __slots__ = ("name", "flags", "crc", "size", "local", "data", "crc_at")
+
+
+def _parse_zip(sk: _Skeleton, size: int) -> list[_ZipRecord]:
+    """The records of the archive in file order, from its central directory (ZIP64 records included); raises
+    ``ValueError`` on anything torch.save does not write (compression, extra bytes between records, ...)."""
+    tail_start, tail = sk.pieces[-1][0], sk.pieces[-1][1]
+    end = bytes(tail).rfind(_ZIP_END.to_bytes(4, "little"))
+    if end < 0:
+        raise ValueError("torch.save layout: no end-of-central-directory record")
+    end += tail_start
+    count, cd_off = sk.u(end + 10, 2), sk.u(end + 16, 4)
+    if count == 0xFFFF or cd_off == 0xFFFFFFFF:
+        loc = end - 20
+        if sk.u(loc, 4) != _ZIP64_LOCATOR:
+            raise ValueError("torch.save layout: ZIP64 locator missing")
+        z64 = sk.u(loc + 8, 8)
+        if sk.u(z64, 4) != _ZIP64_END:
+            raise ValueError("torch.save layout: ZIP64 end record missing")
+        count, cd_off = sk.u(z64 + 32, 8), sk.u(z64 + 48, 8)
+    records, at = [], cd_off
+    for _ in range(count):
+        if sk.u(at, 4) != _ZIP_CENTRAL:
+            raise ValueError(f"torch.save layout: no central directory entry at {at}")
+        r = _ZipRecord()
+        r.flags, method, r.crc = sk.u(at + 8, 2), sk.u(at + 10, 2), sk.u(at + 16, 4)
+        comp, r.size, nlen, xlen, clen = (sk.u(at + 20, 4), sk.u(at + 24, 4), sk.u(at + 28, 2), sk.u(at + 30, 2),
+                                          sk.u(at + 32, 2))
+        r.local = sk.u(at + 42, 4)
+        r.name = sk.read(at + 46, nlen).decode("utf-8")
+        x, x_end = at + 46 + nlen, at + 46 + nlen + xlen
+        while x < x_end:  # the ZIP64 extra field holds the 32-bit fields that overflowed, in this order
+            tag, n = sk.u(x, 2), sk.u(x + 2, 2)
+            if tag == 1:
+                y = x + 4
+                for field in ("size", "comp", "local"):
+                    v = {"size": r.size, "comp": comp, "local": r.local}[field]
+                    if v == 0xFFFFFFFF:
+                        v, y = sk.u(y, 8), y + 8
+                        if field == "comp":
+                            comp = v
+                        else:
+                            setattr(r, field, v)
+            x += 4 + n
+        if method != 0 or comp != r.size:
+            raise ValueError(f"torch.save layout: record {r.name!r} is not stored uncompressed")
+        if sk.u(r.local, 4) != _ZIP_LOCAL:
+            raise ValueError(f"torch.save layout: no local header for {r.name!r}")
+        r.data = r.local + 30 + sk.u(r.local + 26, 2) + sk.u(r.local + 28, 2)
+        if r.flags & 8:  # CRC and sizes follow the data in a descriptor; the local header's CRC stays 0
+            r.crc_at = [r.data + r.size + 4, at + 16]
+            if sk.u(r.data + r.size, 4) != _ZIP_DESCRIPTOR or sk.u(r.data + r.size + 4, 4) != r.crc:
+                raise ValueError(f"torch.save layout: bad data descriptor for {r.name!r}")
+        else:
+            r.crc_at = [r.local + 14, at + 16]
+            if sk.u(r.local + 14, 4) != r.crc:
+                raise ValueError(f"torch.save layout: local and central CRC of {r.name!r} differ")
+        records.append(r)
+        at = x_end + clen
+    if [r.local for r in records] != sorted(r.local for r in records) or (records and records[-1].data > size):
+        raise ValueError("torch.save layout: records out of order")
+    return records
+
+
+def _id_combine(records) -> int:
+    """The value behind the last 20 digits of the serialization id: c10::hash_combine over the CRC-32 of every
+    non-empty record written before it (torch's writer leaves empty records out)."""
+    s = 0
+    for r in (r for r in records if r.size):
+        s = (s ^ ((r.crc + 0x9E3779B9 + (s << 6) + (s >> 2)) & _MASK64)) & _MASK64
+    return s
+
+
+class _StorageKeys:
+    """A pickle module whose Pickler records, for every storage key torch.save's ``persistent_id`` hands out, the
+    storage it stands for -- so the data records are matched to their storages by torch's own traversal.  Subclassed by
+    torch's PyTorchPickler; pickles exactly as ``pickle.Pickler`` does."""
+
+    __name__ = "torch_save_keys"  # torch.save reads the pickle module's name
+
+    def __init__(self):
+        import pickle
+
+        import torch
+
+        keys = self.keys = {}
+
+        class Pickler(pickle.Pickler):
+            def __init__(self, *args, **kwargs):
+                torch_pid = self.persistent_id  # torch's method: wrapped before the C pickler looks it up
+
+                def persistent_id(obj):
+                    if isinstance(obj, torch.Tensor) and obj.device.type == "meta":  # skip_data would drop its storage
+                        raise ValueError("DeviceFile.torch_save: a tensor lives on meta, which holds no bytes to save")
+                    got = torch_pid(obj)
+                    if got is not None and got[0] == "storage":
+                        keys.setdefault(got[2], getattr(obj, "_untyped_storage", obj))
+                    return got
+
+                self.persistent_id = persistent_id
+                super().__init__(*args, **kwargs)
+
+        self.Pickler = Pickler
+
+
+def torch_save_layout(obj):
+    """(skeleton pieces [(offset, bytearray)], [(offset, untyped storage)] in file order, size, parsed records, whether
+    CRCs are computed) of ``torch.save(obj)``: the archive without its storage bytes, checked against what the code
+    that fills them in assumes."""
+    import torch
+    from torch.utils.serialization import config
+
+    w, keys = _SkeletonWriter(), _StorageKeys()
+    with torch.serialization.skip_data():
+        torch.save(obj, w, pickle_module=keys)
+    size = w.pos
+    if not w.pieces or w.pieces[-1][0] + len(w.pieces[-1][1]) != size:
+        raise ValueError("torch.save layout: the archive does not end in written bytes")
+    sk = _Skeleton(w.pieces)
+    records = _parse_zip(sk, size)
+    prefix = records[0].name.split("/", 1)[0] + "/" if records else ""
+    data = [r for r in records if r.name.startswith(prefix + "data/")]
+    if [r.name for r in data] != [f"{prefix}data/{k}" for k in keys.keys]:
+        raise ValueError("torch.save layout: data records do not follow the storage keys")
+    gaps = dict(w.gaps)
+    storages = []
+    for r, (key, st) in zip(data, keys.keys.items()):
+        if r.size != st.nbytes() or (r.size and gaps.pop(r.data, None) != r.size):
+            raise ValueError(f"torch.save layout: record {r.name!r} does not span its storage's bytes")
+        storages.append((r.data, st))
+    if gaps:
+        raise ValueError("torch.save layout: skipped bytes outside the data records")
+    compute_crc = bool(config.save.compute_crc32)
+    if records:
+        rid = records[-1]
+        if rid.name != prefix + _ID_RECORD or rid.size != 40 or not sk.read(rid.data, 40).isdigit():
+            raise ValueError("torch.save layout: the last record is not a 40-digit serialization id")
+        if compute_crc and (any(r.crc for r in data if r.size) or
+                            _id_combine(records[:-1]) != int(sk.read(rid.data + 20, 20))):
+            raise ValueError("torch.save layout: the serialization id does not combine the records' CRC-32s")
+    return sk, storages, size, records, compute_crc
+
+
 class DeviceFile(io.RawIOBase):
     """Read-only, seekable ``BinaryIO`` over the raw bytes of one contiguous CUDA tensor (any dtype), in memory order,
     or (``DeviceFile.safetensors``) over the safetensors image of many.
@@ -285,6 +523,87 @@ class DeviceFile(io.RawIOBase):
             ctx = cls._Source._check_tensor(t, ctx, f"DeviceFile.safetensors[{name!r}]")
         head = cls._Source._to_device(header, ctx or get_context())
         return cls._over(cls._Source([head] + [t for _, t in ordered], bounce_bytes))
+
+    @classmethod
+    def torch_save(cls, obj, *, ctx=None, bounce_bytes: int = BOUNCE_BYTES) -> "DeviceFile":
+        """A file whose bytes are exactly ``torch.save(obj, io.BytesIO()).getvalue()`` (records named ``archive/...``),
+        made of the storages where they are.  ``obj`` is anything torch.save takes: a state dict, a training
+        checkpoint ``{"model": ..., "optim": opt.state_dict(), "step": n}``, nested containers.
+
+        The archive's skeleton (``torch.save`` under ``torch.serialization.skip_data()``: pickle, headers, central
+        directory) is built on the host.  Every storage is one segment over its whole untyped storage, in place when it
+        is on the context's CUDA device; CPU storages (optimizer ``step`` tensors) are staged to the device together
+        with the skeleton's pieces, in one buffer.  Storages on another device raise ``ValueError``.  The CRC-32 of
+        every storage is computed on the device (one ``b200h_crc32_device`` call, ordered after the current stream) and
+        written into the skeleton with the serialization id it determines; the id record's own CRC-32 comes from the
+        device too.  Construction therefore synchronises the current stream twice to read the CRC values back, and not
+        at all when ``torch.utils.serialization.config.save.compute_crc32`` is False (the skeleton is then the file) or
+        nothing holds a storage.  Only CRC values cross to the host.  The legacy (non-zip) format is not produced."""
+        import torch
+
+        ctx = ctx or get_context()
+        dev = getattr(ctx, "device", None)
+        sk, storages, size, records, compute_crc = torch_save_layout(obj)
+        here, staged = [], []  # (file offset, untyped storage) in place / to stage
+        for off, st in storages:
+            where = st.device
+            if where.type == cls._Source.device_type and (where.index == dev or dev in (None, -1)):
+                here.append((off, st))
+            elif where.type == "cpu":
+                staged.append((off, st))
+            else:
+                raise ValueError(f"DeviceFile.torch_save: a storage lives on {where}, but the file is built on "
+                                 f"{cls._Source.device_type}:{dev}")
+        as_u8 = lambda st: torch.empty(0, dtype=torch.uint8, device=st.device).set_(st)  # noqa: E731
+        # one device buffer: the skeleton's pieces, then the staged storages (16-byte aligned); its host twin is pinned
+        layout, at = [], 0
+        for off, piece in sk.pieces:
+            layout.append((off, at, len(piece)))
+            at += len(piece)
+        skel_bytes = at
+        for off, st in staged:
+            at = (at + 15) & ~15
+            layout.append((off, at, st.nbytes()))
+            at += st.nbytes()
+        host, buf = cls._Source._pinned(max(at, 1)), cls._Source._empty(max(at, 1), ctx)
+        seg_of = {off: buf[a : a + n] for off, a, n in layout}
+        for (off, a, n), (_, st) in zip(layout[len(sk.pieces) :], staged):
+            host[a : a + n].copy_(torch.empty(0, dtype=torch.uint8).set_(st))
+        if staged:
+            buf[skel_bytes:at].copy_(host[skel_bytes:at], non_blocking=True)
+        for off, st in here:
+            seg_of[off] = as_u8(st)
+        hv = host.numpy()
+        data = sorted(storages, key=lambda x: x[0])
+        if compute_crc and data:
+            stream = cls._Source._current_stream(ctx)
+            rec_at = {r.data: r for r in records}
+            crc = cls._Source._empty(4 * len(data), ctx).view(torch.int32)
+            ctx.crc32_device([seg_of[off].data_ptr() if seg_of[off].numel() else 0 for off, _ in data],
+                             [seg_of[off].numel() for off, _ in data], crc.data_ptr(), stream)
+            for (off, _), c in zip(data, crc.cpu().numpy().view(np.uint32).tolist()):  # synchronisation 1
+                rec_at[off].crc = c
+                for field in rec_at[off].crc_at:
+                    sk.patch(field, c.to_bytes(4, "little"))
+            rid = records[-1]
+            digits = sk.read(rid.data, 20) + b"%020d" % _id_combine(records[:-1])
+            sk.patch(rid.data, digits)
+            k = bisect.bisect_right(sk.starts, rid.data) - 1
+            a = layout[k][1] + rid.data - sk.starts[k]  # where the id's digits sit in the device buffer
+            hv[a : a + 40] = np.frombuffer(digits, np.uint8)
+            buf[a : a + 40].copy_(host[a : a + 40], non_blocking=True)
+            ctx.crc32_device([buf[a:].data_ptr()], [40], crc.data_ptr(), stream)
+            rid.crc = int(crc[:1].cpu().numpy().view(np.uint32)[0])  # synchronisation 2
+            for field in rid.crc_at:
+                sk.patch(field, rid.crc.to_bytes(4, "little"))
+        for (off, piece), (_, a, n) in zip(sk.pieces, layout):
+            hv[a : a + n] = np.frombuffer(piece, np.uint8)
+        buf[:skel_bytes].copy_(host[:skel_bytes], non_blocking=True)
+        segments = [seg_of[off] for off in sorted(seg_of)]
+        src = cls._Source(segments, bounce_bytes)
+        src.keep = (buf, host)
+        assert src.nbytes == size
+        return cls._over(src)
 
     @classmethod
     def _over(cls, src) -> "DeviceFile":
