@@ -125,6 +125,9 @@ int b200h_hash_fixed_parts(b200h_ctx* ctx, const uint8_t* base, uint64_t len, ui
  * trimmed ones, which exist on the device only, and the planner's count is read back (one synchronisation of
  * `cuda_stream`, counted by b200h_plan_sync_count).  B200H_TRIM_ZEROS | B200H_NO_OUTLIERS only enqueues.
  * The part table (16 bytes per part) travels to the device with the work.
+ * This is the one-segment case of b200h_hash_segment_parts_device (segment {d_base, len}; every part is hashed where
+ * it is), plus the ETag.  A d_base range whose first or last byte is not device memory on ctx's device is
+ * B200H_E_INVALID, rejected before anything is enqueued.
  * Replaces: the per-8MiB-block loop of _gather_blocks (blob_utils.py:622-645) for a buffer that already lives in HBM,
  * which the reference would first copy to host memory. */
 int b200h_hash_fixed_parts_device(b200h_ctx* ctx, const void* d_base, uint64_t len, uint64_t part_len, uint32_t flags,
@@ -166,7 +169,7 @@ int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, u
 /* CRC-32 of n device ranges: d_crc_out[i] (a DEVICE array of n uint32, 4-byte aligned) = zlib.crc32 of
  * ranges[i].len bytes at ranges[i].d_ptr (IEEE polynomial, reflected, initial value and final XOR 0xFFFFFFFF): the
  * checksum a zip archive stores for every record, such as those of a torch.save file.  Any start alignment, any length
- * (0 gives 0).  `ranges` is a host array; every non-empty range's first and last byte, and the first and last word of
+ * (0 gives 0).  `ranges` is a host array; every non-empty range's first and last byte, and the first and last byte of
  * d_crc_out, must be device memory on ctx's device (cudaPointerGetAttributes): a NULL or foreign pointer is
  * B200H_E_INVALID, and every argument is checked before any work is enqueued.
  * The work is spread by bytes, not by ranges: every range is cut into 16 KiB chunks and the grid's warps take equal runs

@@ -201,6 +201,17 @@ def _segment_args(file_first_seg):
     return ffs, ffs.size - 1
 
 
+def _segments(ptrs, lens) -> np.ndarray:
+    """The b200h_segment {d_ptr, len} array of device ranges ptrs[i], lens[i], as uint64[n, 2]."""
+    p = np.ascontiguousarray(ptrs, dtype=np.uint64)
+    ln = np.ascontiguousarray(lens, dtype=np.uint64)
+    if p.shape != ln.shape or p.ndim != 1:
+        raise ValueError("pointers and lengths must be 1-D and of equal length")
+    segs = np.empty((ln.size, 2), np.uint64)
+    segs[:, 0], segs[:, 1] = p, ln
+    return segs
+
+
 def segment_parts_preview(seg_lens, file_first_seg, part_len: int, wave_bytes: int):
     """How ``Context.hash_segment_parts_device`` splits these files (file f = segments file_first_seg[f] ..
     file_first_seg[f+1]) for wave slots of ``wave_bytes``: -> (seg uint64[nparts]: the segment each part is hashed in
@@ -402,15 +413,10 @@ class Context:
         """``hash_fixed_parts_device`` over files made of device buffers: file f is the concatenation of segments
         file_first_seg[f] .. file_first_seg[f+1] (segment s: seg_lens[s] bytes at device address seg_ptrs[s]).  Every
         file's parts, file-major, form one batch; outputs hold that many rows.  Returns the row count."""
-        ptrs = np.ascontiguousarray(seg_ptrs, dtype=np.uint64)
-        lens = np.ascontiguousarray(seg_lens, dtype=np.uint64)
-        if ptrs.shape != lens.shape or ptrs.ndim != 1:
-            raise ValueError("seg_ptrs and seg_lens must be 1-D and of equal length")
-        segs = np.empty((lens.size, 2), np.uint64)  # b200h_segment {d_ptr, len}
-        segs[:, 0], segs[:, 1] = ptrs, lens
+        segs = _segments(seg_ptrs, seg_lens)
         ffs, nfiles = _segment_args(file_first_seg)
         got = ctypes.c_uint64()
-        rc = self._L.b200h_hash_segment_parts_device(self._h, _np_ptr(segs) if lens.size else None, lens.size, _np_ptr(ffs),
+        rc = self._L.b200h_hash_segment_parts_device(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
                                                      nfiles, part_len, flags, d_sha or None, d_md5 or None,
                                                      d_trimmed or None, ctypes.byref(got), stream or None)
         self._check(rc, "b200h_hash_segment_parts_device")
@@ -419,13 +425,8 @@ class Context:
     def crc32_device(self, ptrs, lens, d_out: int, stream: int = 0) -> None:
         """zlib.crc32 of every device range (lens[i] bytes at device address ptrs[i]) into the device uint32 array at
         ``d_out``, computed on the device; the work is only enqueued on ``stream``."""
-        p = np.ascontiguousarray(ptrs, dtype=np.uint64)
-        ln = np.ascontiguousarray(lens, dtype=np.uint64)
-        if p.shape != ln.shape or p.ndim != 1:
-            raise ValueError("ptrs and lens must be 1-D and of equal length")
-        ranges = np.empty((ln.size, 2), np.uint64)  # b200h_segment {d_ptr, len}
-        ranges[:, 0], ranges[:, 1] = p, ln
-        rc = self._L.b200h_crc32_device(self._h, _np_ptr(ranges) if ln.size else None, ln.size, d_out or None,
+        ranges = _segments(ptrs, lens)
+        rc = self._L.b200h_crc32_device(self._h, _np_ptr(ranges) if len(ranges) else None, len(ranges), d_out or None,
                                         stream or None)
         self._check(rc, "b200h_crc32_device")
 

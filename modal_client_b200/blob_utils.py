@@ -913,12 +913,9 @@ async def device_file_specs2(
 ) -> list[FileUploadSpec2]:
     """Batched ``FileUploadSpec2.from_fileobj`` for the ``DeviceFile``s of one ``batch_upload``: the blocks of ALL of
     them, whatever tensors they are made of, are trimmed and hashed by one ``b200h_hash_segment_parts_device`` call,
-    and only that table comes to the host.  A single file is ``from_fileobj`` itself."""
+    and only that table comes to the host."""
     if not items:
         return []
-    if len(items) == 1:
-        fp, remote, mode = items[0]
-        return [await FileUploadSpec2.from_fileobj(fp, remote, asyncio.Semaphore(1), mode)]
 
     def run() -> list[FileUploadSpec2]:
         files = [fp for fp, _, _ in items]

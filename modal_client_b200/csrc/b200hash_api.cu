@@ -149,8 +149,8 @@ struct b200h_ctx {
     size_t dwave_cap = 0;  // per slot
     size_t dwave_want = 0;
     DevBuf d_off, d_len, d_order, d_order_long, d_trim, d_sha, d_md5, d_scratch, d_small, d_states, d_dedupe, d_keys, d_trimctl, d_hex;
-    DevBuf d_parts;  // part table of b200h_hash_fixed_parts_device: offsets | lengths | the ETag message (offset, length)
-                     // (b200h_hash_segment_parts_device: absolute addresses | lengths | gather tiles)
+    DevBuf d_parts;  // part table of b200h_hash_segment_parts_device: absolute addresses | lengths | gather tiles
+                     // (b200h_hash_fixed_parts_device: the ETag message {offset, length} after the lengths)
     uint64_t* h_meta = nullptr;  // pinned: offsets then lengths
     size_t h_meta_cap = 0;       // in uint64 elements
     uint64_t launches = 0;
@@ -864,6 +864,114 @@ int layout_segment_parts(const uint64_t* seg_lens, uint64_t nsegs, const uint64_
     return 0;
 }
 
+// A pointer that is not memory of ctx's device would fault the kernels, so every device range an entry point takes is
+// checked before anything is enqueued: its first and last byte (the allocation in between is the caller's promise).
+bool device_range_ok(b200h_ctx* ctx, const void* ptr, uint64_t len) {
+    if (!len) return true;
+    for (const uint8_t* q : {(const uint8_t*)ptr, (const uint8_t*)ptr + (len - 1)}) {
+        cudaPointerAttributes at;
+        const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess &&
+                        (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == ctx->device;
+        cudaGetLastError();
+        if (!ok) return false;
+    }
+    return true;
+}
+
+// b200h_hash_segment_parts_device with ctx->mu held, on stream `st`.  d_etag_msg != NULL (b200h_hash_fixed_parts_device):
+// two more words, the ETag message {0, nparts * 16}, ride the part-table upload, even when there are no parts, and
+// *d_etag_msg points at them.
+int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                              uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
+                              uint64_t* d_trimmed_len, uint64_t* nparts_out, cudaStream_t st, const uint64_t** d_etag_msg) {
+    if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
+    if (((uintptr_t)d_sha256 | (uintptr_t)d_md5) & 15u)
+        return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
+    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
+    std::vector<uint64_t> seg_lens(nsegs);
+    for (uint64_t s = 0; s < nsegs; ++s) {
+        if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
+        seg_lens[s] = segs[s].len;
+    }
+    SegmentParts p;
+    std::string err;
+    if (int rc = layout_segment_parts(seg_lens.data(), nsegs, file_first_seg, nfiles, part_len,
+                                      std::max(ctx->dwave_cap, ctx->dwave_want), p, err))
+        return fail(ctx, rc, err);
+    const uint64_t nparts = p.off.size();
+    if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
+        return fail(ctx, B200H_E_INVALID, "flags select neither SHA256 nor MD5");
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    for (uint64_t s = 0; s < nsegs; ++s)
+        if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
+            return fail(ctx, B200H_E_INVALID,
+                        "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
+    if (nparts_out) *nparts_out = nparts;
+    if (nparts == 0 && !d_etag_msg) return 0;
+    uint64_t stage_max = 0;
+    for (uint64_t b : p.wave_bytes) stage_max = std::max(stage_max, b);
+    if (stage_max)
+        if (int rc = ensure_wave(ctx, stage_max)) return rc;
+
+    // device table: part addresses | part lengths | [ETag message] | gather tiles (after the gather, every part is an
+    // absolute address)
+    const size_t nwaves = p.wave_bytes.size();
+    std::vector<uint64_t> table(2 * nparts);
+    if (d_etag_msg) table.insert(table.end(), {0, nparts * 16});
+    std::vector<uint64_t> wave_tiles(nwaves + 1, 0);  // tiles of wave w: [wave_tiles[w], wave_tiles[w + 1])
+    std::vector<GatherTile> tiles;
+    for (size_t w = 0; w < nwaves; ++w) {
+        uint8_t* slot = ctx->dwave[w & 1];
+        for (uint64_t i = p.wave_first[w]; i < p.wave_first[w + 1]; ++i) {
+            table[nparts + i] = p.len[i];
+            if (p.stage[i] == kInPlace) {
+                table[i] = (uint64_t)(uintptr_t)segs[p.seg[i]].d_ptr + p.seg_off[i];
+                continue;
+            }
+            table[i] = (uint64_t)(uintptr_t)(slot + p.stage[i]);
+            uint64_t s = p.seg[i], so = p.seg_off[i], done = 0;
+            while (done < p.len[i]) {
+                const uint64_t piece = std::min(seg_lens[s] - so, p.len[i] - done);
+                for (uint64_t t = 0; t < piece; t += kGatherTileBytes)
+                    tiles.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + so + t, table[i] + done + t,
+                                     std::min(kGatherTileBytes, piece - t)});
+                done += piece;
+                ++s;
+                so = 0;
+            }
+        }
+        wave_tiles[w + 1] = tiles.size();
+    }
+    const size_t table_bytes = table.size() * sizeof(uint64_t), tiles_bytes = tiles.size() * sizeof(GatherTile);
+    // The table is context scratch like the planner's: it is rewritten only after the last batch that read it.
+    if (ctx->scratch_used) CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_scratch, 0));
+    if (int rc = ensure_dev(ctx, ctx->d_parts, table_bytes + tiles_bytes)) return rc;
+    uint64_t* d_table = (uint64_t*)ctx->d_parts.p;
+    GatherTile* d_tiles = (GatherTile*)(d_table + table.size());
+    CU_TRY(ctx, cudaMemcpyAsync(d_table, table.data(), table_bytes, cudaMemcpyHostToDevice, st));
+    if (tiles_bytes) CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tiles_bytes, cudaMemcpyHostToDevice, st));
+    if (d_etag_msg) *d_etag_msg = d_table + 2 * nparts;
+    uint8_t* o_sha = (flags & B200H_SHA256) ? (uint8_t*)d_sha256 : nullptr;
+    uint8_t* o_md5 = (flags & B200H_MD5) ? (uint8_t*)d_md5 : nullptr;
+    for (size_t w = 0; w < nwaves; ++w) {
+        const uint64_t i0 = p.wave_first[w], cnt = p.wave_first[w + 1] - i0;
+        const int slot = (int)(w & 1);
+        const bool staged = wave_tiles[w + 1] > wave_tiles[w];
+        if (staged) {
+            // the slot is shared with the *_host entry points and the previous waves: wait for its last reader
+            CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_consumed[slot], 0));
+            ctx->launches += launch_gather_segments(d_tiles + wave_tiles[w], wave_tiles[w + 1] - wave_tiles[w], st);
+            CU_TRY(ctx, cudaGetLastError());
+        }
+        if (int rc = enqueue_device_batch(ctx, nullptr, d_table + i0, d_table + nparts + i0, cnt, flags & kPublicFlags,
+                                          o_sha ? o_sha + 32 * i0 : nullptr, o_md5 ? o_md5 + 16 * i0 : nullptr,
+                                          d_trimmed_len ? d_trimmed_len + i0 : nullptr, nullptr, st, p.len.data() + i0))
+            return rc;
+        if (staged) CU_TRY(ctx, cudaEventRecord(ctx->ev_consumed[slot], st));
+    }
+    return 0;
+}
+
 // A small request from one of possibly many concurrent callers: merge it with whatever else arrives while the context
 // is busy, run ONE batch, hand every caller its rows.  (See Combiner.)
 int combined_hash_batch_host(b200h_ctx* ctx, const uint8_t* base, const uint64_t* off, const uint64_t* len, uint64_t n,
@@ -1195,40 +1303,25 @@ int b200h_hash_fixed_parts_device(b200h_ctx* ctx, const void* d_base, uint64_t l
     B200H_RANGE("b200h_hash_fixed_parts_device");
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (part_len == 0) return fail(ctx, B200H_E_INVALID, "part_len must be > 0");
-    if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
+    const uint64_t nparts = len / part_len + (len % part_len != 0);
     if (d_etag_md5 && !(flags & B200H_MD5)) return fail(ctx, B200H_E_INVALID, "etag requires B200H_MD5");
-    if (((uintptr_t)d_sha256 | (uintptr_t)d_md5 | (uintptr_t)d_etag_md5) & 15u)
-        return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
-    if (len && !d_base) return fail(ctx, B200H_E_INVALID, "d_base must not be NULL");
-    std::vector<uint64_t> table;  // offsets, then lengths, then the ETag message {offset, length}
-    std::vector<uint64_t> ln;
-    const uint64_t nparts = split_fixed_parts(len, part_len, table, ln);
     if (d_etag_md5 && nparts && !d_md5) return fail(ctx, B200H_E_INVALID, "etag requires the part MD5 output d_md5");
-    if (nparts_out) *nparts_out = nparts;
-    if (nparts == 0 && !d_etag_md5) return 0;
-    if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
-        return fail(ctx, B200H_E_INVALID, "flags select neither SHA256 nor MD5");
-    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    if ((uintptr_t)d_etag_md5 & 15u) return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
+    if (len && !d_base) return fail(ctx, B200H_E_INVALID, "d_base must not be NULL");
+    // the one-segment case of b200h_hash_segment_parts_device: every part is hashed where it is
+    const b200h_segment seg = {d_base, len};
+    const uint64_t file_first_seg[2] = {0, 1};
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    const uint64_t etag_len = nparts * 16;
-    table.insert(table.end(), ln.begin(), ln.end());
-    table.push_back(0);
-    table.push_back(etag_len);
-    // The part table is context scratch like the planner's: it is rewritten only after the last batch that read it.
-    if (ctx->scratch_used) CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_scratch, 0));
-    if (int rc = ensure_dev(ctx, ctx->d_parts, table.size() * sizeof(uint64_t))) return rc;
-    uint64_t* d_table = (uint64_t*)ctx->d_parts.p;
-    CU_TRY(ctx, cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-    uint8_t* o_sha = (flags & B200H_SHA256) ? (uint8_t*)d_sha256 : nullptr;
-    uint8_t* o_md5 = (flags & B200H_MD5) ? (uint8_t*)d_md5 : nullptr;
-    if (int rc = enqueue_device_batch(ctx, (const uint8_t*)d_base, d_table, d_table + nparts, nparts, flags & kPublicFlags,
-                                      o_sha, o_md5, d_trimmed_len, nullptr, st, ln.data()))
+    const uint64_t* d_etag_msg = nullptr;
+    if (int rc = hash_segment_parts_locked(ctx, &seg, 1, file_first_seg, 1, part_len, flags, d_sha256, d_md5, d_trimmed_len,
+                                           nparts_out, st, d_etag_md5 ? &d_etag_msg : nullptr))
         return rc;
     if (d_etag_md5) {
         // MD5 over the concatenated raw part MD5s, on the device like the host entry's (an empty object: md5(""))
-        const uint8_t* etag_src = nparts ? o_md5 : (const uint8_t*)d_table;
-        if (int rc = enqueue_device_batch(ctx, etag_src, d_table + 2 * nparts, d_table + 2 * nparts + 1, 1, B200H_MD5,
-                                          nullptr, (uint8_t*)d_etag_md5, nullptr, nullptr, st, &etag_len))
+        const uint64_t etag_len = nparts * 16;
+        const uint8_t* etag_src = nparts ? (const uint8_t*)d_md5 : (const uint8_t*)d_etag_msg;
+        if (int rc = enqueue_device_batch(ctx, etag_src, d_etag_msg, d_etag_msg + 1, 1, B200H_MD5, nullptr,
+                                          (uint8_t*)d_etag_md5, nullptr, nullptr, st, &etag_len))
             return rc;
     }
     return 0;
@@ -1240,100 +1333,9 @@ int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, u
     if (!ctx) return B200H_E_INVALID;
     B200H_RANGE("b200h_hash_segment_parts_device");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
-    if (((uintptr_t)d_sha256 | (uintptr_t)d_md5) & 15u)
-        return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
-    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
-    std::vector<uint64_t> seg_lens(nsegs);
-    for (uint64_t s = 0; s < nsegs; ++s) {
-        if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
-        seg_lens[s] = segs[s].len;
-    }
-    SegmentParts p;
-    std::string err;
-    if (int rc = layout_segment_parts(seg_lens.data(), nsegs, file_first_seg, nfiles, part_len,
-                                      std::max(ctx->dwave_cap, ctx->dwave_want), p, err))
-        return fail(ctx, rc, err);
-    const uint64_t nparts = p.off.size();
-    if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
-        return fail(ctx, B200H_E_INVALID, "flags select neither SHA256 nor MD5");
-    CU_TRY(ctx, cudaSetDevice(ctx->device));
-    // A pointer that is not memory of this device would fault the kernels; reject it before anything is enqueued.
-    // (Both ends of every segment are checked; the allocation in between is the caller's promise.)
-    for (uint64_t s = 0; s < nsegs; ++s) {
-        if (!segs[s].len) continue;
-        for (const uint8_t* q : {(const uint8_t*)segs[s].d_ptr, (const uint8_t*)segs[s].d_ptr + (segs[s].len - 1)}) {
-            cudaPointerAttributes at;
-            const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess &&
-                            (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == ctx->device;
-            cudaGetLastError();
-            if (!ok)
-                return fail(ctx, B200H_E_INVALID,
-                            "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
-        }
-    }
-    if (nparts_out) *nparts_out = nparts;
-    if (nparts == 0) return 0;
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    uint64_t stage_max = 0;
-    for (uint64_t b : p.wave_bytes) stage_max = std::max(stage_max, b);
-    if (stage_max)
-        if (int rc = ensure_wave(ctx, stage_max)) return rc;
-
-    // device table: part addresses | part lengths | gather tiles (after the gather, every part is an absolute address)
-    const size_t nwaves = p.wave_bytes.size();
-    std::vector<uint64_t> table(2 * nparts);
-    std::vector<uint64_t> wave_tiles(nwaves + 1, 0);  // tiles of wave w: [wave_tiles[w], wave_tiles[w + 1])
-    std::vector<GatherTile> tiles;
-    for (size_t w = 0; w < nwaves; ++w) {
-        uint8_t* slot = ctx->dwave[w & 1];
-        for (uint64_t i = p.wave_first[w]; i < p.wave_first[w + 1]; ++i) {
-            table[nparts + i] = p.len[i];
-            if (p.stage[i] == kInPlace) {
-                table[i] = (uint64_t)(uintptr_t)segs[p.seg[i]].d_ptr + p.seg_off[i];
-                continue;
-            }
-            table[i] = (uint64_t)(uintptr_t)(slot + p.stage[i]);
-            uint64_t s = p.seg[i], so = p.seg_off[i], done = 0;
-            while (done < p.len[i]) {
-                const uint64_t piece = std::min(seg_lens[s] - so, p.len[i] - done);
-                for (uint64_t t = 0; t < piece; t += kGatherTileBytes)
-                    tiles.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + so + t, table[i] + done + t,
-                                     std::min(kGatherTileBytes, piece - t)});
-                done += piece;
-                ++s;
-                so = 0;
-            }
-        }
-        wave_tiles[w + 1] = tiles.size();
-    }
-    const size_t table_bytes = table.size() * sizeof(uint64_t), tiles_bytes = tiles.size() * sizeof(GatherTile);
-    // The table is context scratch like the planner's: it is rewritten only after the last batch that read it.
-    if (ctx->scratch_used) CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_scratch, 0));
-    if (int rc = ensure_dev(ctx, ctx->d_parts, table_bytes + tiles_bytes)) return rc;
-    uint64_t* d_table = (uint64_t*)ctx->d_parts.p;
-    GatherTile* d_tiles = (GatherTile*)(d_table + table.size());
-    CU_TRY(ctx, cudaMemcpyAsync(d_table, table.data(), table_bytes, cudaMemcpyHostToDevice, st));
-    if (tiles_bytes) CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tiles_bytes, cudaMemcpyHostToDevice, st));
-    uint8_t* o_sha = (flags & B200H_SHA256) ? (uint8_t*)d_sha256 : nullptr;
-    uint8_t* o_md5 = (flags & B200H_MD5) ? (uint8_t*)d_md5 : nullptr;
-    for (size_t w = 0; w < nwaves; ++w) {
-        const uint64_t i0 = p.wave_first[w], cnt = p.wave_first[w + 1] - i0;
-        const int slot = (int)(w & 1);
-        const bool staged = wave_tiles[w + 1] > wave_tiles[w];
-        if (staged) {
-            // the slot is shared with the *_host entry points and the previous waves: wait for its last reader
-            CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_consumed[slot], 0));
-            ctx->launches += launch_gather_segments(d_tiles + wave_tiles[w], wave_tiles[w + 1] - wave_tiles[w], st);
-            CU_TRY(ctx, cudaGetLastError());
-        }
-        if (int rc = enqueue_device_batch(ctx, nullptr, d_table + i0, d_table + nparts + i0, cnt, flags & kPublicFlags,
-                                          o_sha ? o_sha + 32 * i0 : nullptr, o_md5 ? o_md5 + 16 * i0 : nullptr,
-                                          d_trimmed_len ? d_trimmed_len + i0 : nullptr, nullptr, st, p.len.data() + i0))
-            return rc;
-        if (staged) CU_TRY(ctx, cudaEventRecord(ctx->ev_consumed[slot], st));
-    }
-    return 0;
+    return hash_segment_parts_locked(ctx, segs, nsegs, file_first_seg, nfiles, part_len, flags, d_sha256, d_md5,
+                                     d_trimmed_len, nparts_out, cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp,
+                                     nullptr);
 }
 
 int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, uint32_t* d_crc_out, void* cuda_stream) {
@@ -1350,23 +1352,11 @@ int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, 
     }
     if (n == 0) return 0;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
-    // A pointer that is not memory of this device would fault the kernel; reject it before anything is enqueued.
-    // (Both ends of every range and of the output are checked; the allocation in between is the caller's promise.)
-    auto on_device = [&](const void* q) {
-        cudaPointerAttributes at;
-        const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess &&
-                        (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == ctx->device;
-        cudaGetLastError();
-        return ok;
-    };
-    for (uint64_t i = 0; i < n; ++i) {
-        if (!ranges[i].len) continue;
-        const uint8_t* p = (const uint8_t*)ranges[i].d_ptr;
-        if (!on_device(p) || !on_device(p + (ranges[i].len - 1)))
+    for (uint64_t i = 0; i < n; ++i)
+        if (!device_range_ok(ctx, ranges[i].d_ptr, ranges[i].len))
             return fail(ctx, B200H_E_INVALID,
                         "range " + std::to_string(i) + " is not device memory on cuda:" + std::to_string(ctx->device));
-    }
-    if (!on_device(d_crc_out) || !on_device(d_crc_out + (n - 1)))
+    if (!device_range_ok(ctx, d_crc_out, n * sizeof(uint32_t)))
         return fail(ctx, B200H_E_INVALID, "d_crc_out is not device memory on cuda:" + std::to_string(ctx->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
     // device table: ranges | chunk prefix (n + 1); the output starts as every range's length term

@@ -7,10 +7,10 @@ table -- go wherever the upload functions accept a ``BinaryIO``, without first c
 image is never assembled, neither in host memory nor in HBM.
 
 * volumefs2 (``VolumeUploadContextManager2.put_file`` / ``FileUploadSpec2.from_fileobj``) recognises it and trims and
-  hashes its 8 MiB blocks in place (``hash_parts``): one tensor with one ``b200h_hash_fixed_parts_device`` call, a
-  file made of several tensors with one ``b200h_hash_segment_parts_device`` call, which gathers only the blocks that
-  straddle tensor boundaries.  Only the (trimmed length, SHA-256) table comes to the host, and afterwards only the
-  trimmed bytes of the blocks the server reports missing are read.
+  hashes its 8 MiB blocks in place (``hash_parts``) with one ``b200h_hash_segment_parts_device`` call, whatever
+  tensors the file is made of; only the blocks that straddle tensor boundaries are gathered.  Only the (trimmed
+  length, SHA-256) table comes to the host, and afterwards only the trimmed bytes of the blocks the server reports
+  missing are read.
 * every other consumer (volumefs1 ``put_file``, ``get_file_upload_spec_from_fileobj``, ``blob_upload_file``) reads it
   like any other stream.  Those digests are one serial chain over the whole object and gain nothing from the GPU.
 
@@ -152,20 +152,6 @@ class _TensorBytes:
                 dst[done : done + k] = bounce[:k]
                 done += k
             self.bytes_to_host += n
-
-    def hash_parts(self, ctx, part_len: int, flags: int):
-        """``Context.hash_fixed_parts`` over the bytes where they are; only the digest table comes back."""
-        if part_len <= 0:
-            raise ValueError("part_len must be > 0")
-        if len(self.segments) > 1:
-            return _hash_sources([self], ctx, part_len, flags)
-        n = -(-self.nbytes // part_len)
-        with self.lock, self._on_stream():
-            d_sha, d_md5, d_trim = _outputs(n, flags, self.segments[0].device)
-            got = ctx.hash_fixed_parts_device(self.segments[0].data_ptr(), self.nbytes, part_len, flags, _ptr(d_sha),
-                                              _ptr(d_md5), _ptr(d_trim), 0, self.stream_handle)
-            assert got == n
-            return _fetch(d_sha, d_md5, d_trim)
 
 
 def _outputs(n: int, flags: int, device):
@@ -627,11 +613,11 @@ class DeviceFile(io.RawIOBase):
         return DeviceFile._over(self._src)
 
     def hash_parts(self, part_len: int, flags: int = _lib.SHA256 | _lib.MD5, ctx=None):
-        """Split the bytes into ceil(size / part_len) parts and digest them where they are
-        (``b200h_hash_fixed_parts_device`` for one tensor, ``b200h_hash_segment_parts_device`` for several).
+        """Split the bytes into ceil(size / part_len) parts and digest them where they are, with one
+        ``b200h_hash_segment_parts_device`` call whatever tensors the file is made of.
         -> (sha uint8[n,32] | None, md5 uint8[n,16] | None, trimmed uint64[n]); nothing but this table leaves the
         device."""
-        return self._src.hash_parts(ctx or get_context(), part_len, flags)
+        return _hash_sources([self._src], ctx or get_context(), part_len, flags)
 
     # ---- BinaryIO
     def readable(self) -> bool:

@@ -1,6 +1,6 @@
 """DeviceFile and the volumefs2 device path, on the CPU: the file-object semantics, the block table built from one
-``hash_fixed_parts_device`` call, and the upload rounds, with the oracle-backed context and a CPU tensor standing in
-for GPU memory (only the stream, the pinned bounce buffer and the wait are replaced)."""
+``hash_segment_parts_device`` call, and the upload rounds, with the oracle-backed context and CPU tensors standing in
+for GPU memory.  The fake context, fixture and host-memory source here serve the other device-file CPU tests too."""
 import asyncio
 import contextlib
 import ctypes
@@ -8,6 +8,7 @@ import hashlib
 import io
 import random
 import types
+import zlib
 from pathlib import PurePosixPath
 
 import numpy as np
@@ -24,26 +25,41 @@ from tests.test_volume_upload import FakeVolumeStub, _add_block_route
 
 
 class FakeDeviceContext(FakeContext):
-    """The oracle-backed context plus a stand-in for ``Context.hash_fixed_parts_device``."""
+    """The oracle-backed context plus stand-ins for ``Context.hash_segment_parts_device`` and ``crc32_device``.
+    Segment, range and output addresses are HOST addresses (CPU tensors standing in for device memory), so the host
+    logic around the calls runs on the CPU.  The split is checked by the library's own preview, the digests come from
+    the oracle and the CRCs from zlib."""
 
-    def hash_fixed_parts_device(self, d_base, nbytes, part_len, flags, d_sha=0, d_md5=0, d_trimmed=0, d_etag=0,
-                                stream=0):
-        """``d_base`` and the outputs are HOST addresses (a CPU tensor's data_ptr() standing in for device memory),
-        so the host logic around the call runs on the CPU."""
-        self.calls.append(("hash_fixed_parts_device", part_len, flags))
-        if part_len <= 0:
-            raise _lib.B200HashError("b200h_hash_fixed_parts_device failed (-1): part_len must be > 0")
-        data = np.frombuffer(ctypes.string_at(d_base, nbytes), np.uint8) if nbytes else np.zeros(0, np.uint8)
-        starts = np.arange(0, nbytes, part_len, dtype=np.uint64)
-        lens = np.minimum(part_len, nbytes - starts).astype(np.uint64)
-        s, m, e = c_oracle.hash_batch(data, starts, lens, sha=bool(flags & _lib.SHA256), md5=bool(flags & _lib.MD5),
+    def hash_segment_parts_device(self, seg_ptrs, seg_lens, file_first_seg, part_len, flags, d_sha=0, d_md5=0,
+                                  d_trimmed=0, stream=0):
+        self.calls.append(("hash_segment_parts_device", len(file_first_seg) - 1, part_len, flags))
+        seg, _, _ = _lib.segment_parts_preview(seg_lens, file_first_seg, part_len, 1 << 30)  # raises like the entry
+        images = [b"".join(ctypes.string_at(int(p), int(n)) if n else b"" for p, n in
+                           zip(seg_ptrs[file_first_seg[f] : file_first_seg[f + 1]],
+                               seg_lens[file_first_seg[f] : file_first_seg[f + 1]]))
+                  for f in range(len(file_first_seg) - 1)]
+        data = np.frombuffer(b"".join(images) or b"\0", np.uint8)
+        starts, lens, at = [], [], 0
+        for img in images:
+            for o in range(0, len(img), part_len):
+                starts.append(at + o)
+                lens.append(min(part_len, len(img) - o))
+            at += len(img)
+        assert len(starts) == len(seg)
+        s, m, e = c_oracle.hash_batch(data, np.array(starts, np.uint64), np.array(lens, np.uint64),
+                                      sha=bool(flags & _lib.SHA256), md5=bool(flags & _lib.MD5),
                                       trim=bool(flags & _lib.TRIM_ZEROS))
         for addr, table in ((d_sha, s), (d_md5, m), (d_trimmed, e)):
             if addr and table is not None and len(table):
                 ctypes.memmove(addr, np.ascontiguousarray(table).tobytes(), table.nbytes)
-        if d_etag:
-            ctypes.memmove(d_etag, c_oracle.md5(m.tobytes() if m is not None and len(m) else b""), 16)
-        return int(starts.size)
+        return len(starts)
+
+    def crc32_device(self, ptrs, lens, d_out, stream=0):
+        self.calls.append(("crc32_device", len(lens)))
+        crcs = np.array([zlib.crc32(ctypes.string_at(int(p), int(n))) if n else 0 for p, n in zip(ptrs, lens)],
+                        np.uint32)
+        if len(crcs):
+            ctypes.memmove(d_out, crcs.tobytes(), crcs.nbytes)
 
 
 @pytest.fixture
@@ -56,9 +72,13 @@ def fake_device_backend(monkeypatch):
     return ctx
 
 
-class _HostTensorBytes(device_file._TensorBytes):
-    def __init__(self, tensor, bounce_bytes):
-        self._attach(tensor, bounce_bytes)
+class _HostSegments(device_file._TensorBytes):
+    """Segments in CPU tensors: only the stream, the pinned and device buffers, the wait and the uploads change."""
+
+    device_type = "cpu"
+
+    def __init__(self, tensors, bounce_bytes):
+        self._attach(tensors, bounce_bytes)
         self.stream_handle = 0
 
     def _on_stream(self):
@@ -70,11 +90,36 @@ class _HostTensorBytes(device_file._TensorBytes):
     def _wait(self):
         pass
 
+    @classmethod
+    def _to_device(cls, data, ctx):
+        return torch.frombuffer(bytearray(data), dtype=torch.uint8)
+
+    @classmethod
+    def _pinned(cls, n):
+        return torch.empty(n, dtype=torch.uint8)
+
+    @classmethod
+    def _empty(cls, n, ctx):
+        return torch.empty(n, dtype=torch.uint8)
+
+    @classmethod
+    def _current_stream(cls, ctx):
+        return 0
+
+
+class HostDeviceFile(DeviceFile):
+    _Source = _HostSegments
+
+
+def host_segments_file(chunks, bounce_bytes=1 << 20) -> DeviceFile:
+    """A DeviceFile whose "device" bytes are CPU tensors holding ``chunks``, one segment each."""
+    return DeviceFile._over(_HostSegments([torch.frombuffer(bytearray(c), dtype=torch.uint8) if c else
+                                           torch.empty(0, dtype=torch.uint8) for c in chunks], bounce_bytes))
+
 
 def host_device_file(data: bytes, bounce_bytes: int = 1 << 20) -> DeviceFile:
-    """A DeviceFile whose "device" bytes are a CPU tensor holding ``data``."""
-    t = torch.frombuffer(bytearray(data), dtype=torch.uint8) if data else torch.empty(0, dtype=torch.uint8)
-    return DeviceFile._over(_HostTensorBytes(t, bounce_bytes))
+    """A DeviceFile whose "device" bytes are one CPU tensor holding ``data``."""
+    return host_segments_file([data], bounce_bytes)
 
 
 # ------------------------------------------------------------------------------------------------ C ABI
@@ -172,7 +217,8 @@ def test_spec2_from_device_file_equals_spec2_from_bytesio(fake_device_backend, g
         assert f.bytes_to_host == 0  # only the digest table was fetched
         with dev.source() as rd:
             assert rd.read() == data
-    assert ("hash_fixed_parts_device", blob_utils.BLOCK_SIZE, _lib.SHA256 | _lib.TRIM_ZEROS) in fake_device_backend.calls
+    assert ("hash_segment_parts_device", 1, blob_utils.BLOCK_SIZE, _lib.SHA256 | _lib.TRIM_ZEROS) in \
+        fake_device_backend.calls
 
 
 def test_spec2_device_file_block_edges(fake_device_backend, monkeypatch):

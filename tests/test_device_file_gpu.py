@@ -110,6 +110,11 @@ def test_fixed_parts_device_blank_block_fixture_and_argument_checks(ctx, golden)
         ctx.hash_fixed_parts_device(d.data_ptr(), 100, 64, _lib.SHA256 | _lib.HEX_OUT, out.data_ptr())
     with pytest.raises(_lib.B200HashError, match="etag"):
         ctx.hash_fixed_parts_device(d.data_ptr(), 100, 64, _lib.SHA256, out.data_ptr(), 0, 0, out.data_ptr() + 32)
+    host = np.zeros(4096, np.uint8)
+    launches = ctx.launch_count
+    with pytest.raises(_lib.B200HashError, match=r"\(-1\)"):  # host memory: rejected before anything is enqueued
+        ctx.hash_fixed_parts_device(host.ctypes.data, 100, 64, _lib.SHA256, out.data_ptr())
+    assert ctx.launch_count == launches
 
 
 def test_fixed_parts_device_synchronises_only_where_the_header_says(ctx):

@@ -3,7 +3,6 @@ safetensors library, the part / wave split of b200h_segment_parts_preview agains
 volumefs2 path with one ``hash_segment_parts_device`` call per batch, with CPU tensors standing in for GPU memory and
 the oracle standing in for the GPU."""
 import asyncio
-import contextlib
 import ctypes
 import hashlib
 import io
@@ -20,85 +19,12 @@ safetensors_torch = pytest.importorskip("safetensors.torch")
 
 from modal_client_b200 import DeviceFile, _lib, blob_utils, device_file, volume  # noqa: E402
 from modal_client_b200.synth import synth_bytes  # noqa: E402
-from oracle import c_oracle  # noqa: E402
 from tests.blob_server import running_blob_server  # noqa: E402
-from tests.test_device_file_cpu import FakeDeviceContext, _trimmed_total, _volume_server  # noqa: E402
+from tests.test_device_file_cpu import (  # noqa: E402,F401 (fake_device_backend: a fixture)
+    FakeDeviceContext, HostDeviceFile, _trimmed_total, _volume_server, fake_device_backend, host_segments_file)
 from tests.test_volume_upload import FakeVolumeStub  # noqa: E402
 
 GATHERED = int(_lib.GATHERED)
-
-
-class SegmentFakeContext(FakeDeviceContext):
-    """FakeDeviceContext plus ``hash_segment_parts_device``: segment addresses are HOST addresses (CPU tensors standing
-    in for device memory), the split is checked by the library's own preview, the digests come from the oracle."""
-
-    def hash_segment_parts_device(self, seg_ptrs, seg_lens, file_first_seg, part_len, flags, d_sha=0, d_md5=0,
-                                  d_trimmed=0, stream=0):
-        self.calls.append(("hash_segment_parts_device", len(file_first_seg) - 1, part_len, flags))
-        seg, _, _ = _lib.segment_parts_preview(seg_lens, file_first_seg, part_len, 1 << 30)  # raises like the entry
-        images = [b"".join(ctypes.string_at(int(p), int(n)) if n else b"" for p, n in
-                           zip(seg_ptrs[file_first_seg[f] : file_first_seg[f + 1]],
-                               seg_lens[file_first_seg[f] : file_first_seg[f + 1]]))
-                  for f in range(len(file_first_seg) - 1)]
-        data = np.frombuffer(b"".join(images) or b"\0", np.uint8)
-        starts, lens, at = [], [], 0
-        for img in images:
-            for o in range(0, len(img), part_len):
-                starts.append(at + o)
-                lens.append(min(part_len, len(img) - o))
-            at += len(img)
-        assert len(starts) == len(seg)
-        s, m, e = c_oracle.hash_batch(data, np.array(starts, np.uint64), np.array(lens, np.uint64),
-                                      sha=bool(flags & _lib.SHA256), md5=bool(flags & _lib.MD5),
-                                      trim=bool(flags & _lib.TRIM_ZEROS))
-        for addr, table in ((d_sha, s), (d_md5, m), (d_trimmed, e)):
-            if addr and table is not None and len(table):
-                ctypes.memmove(addr, np.ascontiguousarray(table).tobytes(), table.nbytes)
-        return len(starts)
-
-
-@pytest.fixture
-def fake_segment_backend(monkeypatch):
-    from modal_client_b200 import _backend
-
-    ctx = SegmentFakeContext()
-    monkeypatch.setattr(_backend, "_override", ctx)
-    return ctx
-
-
-class _HostSegments(device_file._TensorBytes):
-    """Segments in CPU tensors: only the stream, the pinned bounce buffer, the wait and the header upload change."""
-
-    device_type = "cpu"
-
-    def __init__(self, tensors, bounce_bytes):
-        self._attach(tensors, bounce_bytes)
-        self.stream_handle = 0
-
-    def _on_stream(self):
-        return contextlib.nullcontext()
-
-    def _new_bounce(self, n):
-        return torch.empty(n, dtype=torch.uint8)
-
-    def _wait(self):
-        pass
-
-    def _after(self, other):
-        pass
-
-    @classmethod
-    def _to_device(cls, data, ctx):
-        return torch.frombuffer(bytearray(data), dtype=torch.uint8)
-
-
-class HostDeviceFile(DeviceFile):
-    _Source = _HostSegments
-
-
-def host_segments_file(chunks, bounce_bytes=1 << 20) -> DeviceFile:
-    return DeviceFile._over(_HostSegments([torch.frombuffer(bytearray(c), dtype=torch.uint8) if c else
-                                           torch.empty(0, dtype=torch.uint8) for c in chunks], bounce_bytes))
 
 
 # every dtype safetensors.torch.save stores, as this torch spells it
@@ -243,7 +169,7 @@ def test_safetensors_image_equals_the_library(seed):
     sd = _rand_state_dict(rng, rng.choice([0, 1, 2, 5, 17, 64]))
     for metadata in (None, {}, {"format": "pt"}, {"ß": "ü \"q\"", "a": "1", "B": ""}):
         want = safetensors_torch.save(sd, metadata)
-        f = HostDeviceFile.safetensors(sd, metadata, ctx=SegmentFakeContext(), bounce_bytes=rng.choice([1, 7, 100]))
+        f = HostDeviceFile.safetensors(sd, metadata, ctx=FakeDeviceContext(), bounce_bytes=rng.choice([1, 7, 100]))
         got = f.read()
         if not sd and metadata == {}:
             # safetensors 0.7.0 writes the invalid header '{},"__metadata__":{}}' here; ours is the JSON it means
@@ -268,7 +194,7 @@ def test_safetensors_random_reads_across_segment_edges():
     sd = _rand_state_dict(rng, 40)
     want = safetensors_torch.save(sd)
     for bounce in (1, 5, 64, 4096):
-        f, ref = HostDeviceFile.safetensors(sd, ctx=SegmentFakeContext(), bounce_bytes=bounce), io.BytesIO(want)
+        f, ref = HostDeviceFile.safetensors(sd, ctx=FakeDeviceContext(), bounce_bytes=bounce), io.BytesIO(want)
         for _ in range(150):
             op = rng.randrange(3)
             if op == 0:
@@ -301,15 +227,15 @@ def test_safetensors_dtype_order_and_header():
 def test_safetensors_shared_storage_is_read_twice():
     base = _rand_tensor(random.Random(2), torch.float32, (64,))
     sd = {"a": base[:40], "b": base[40:], "c": base[10:20]}
-    f = HostDeviceFile.safetensors(sd, ctx=SegmentFakeContext())
+    f = HostDeviceFile.safetensors(sd, ctx=FakeDeviceContext())
     back = safetensors_torch.load(f.read())
     assert all(_bytes_of(back[k]) == _bytes_of(sd[k]) for k in sd)
     disjoint = {"a": base[:40], "b": base[40:]}
-    assert HostDeviceFile.safetensors(disjoint, ctx=SegmentFakeContext()).read() == safetensors_torch.save(disjoint)
+    assert HostDeviceFile.safetensors(disjoint, ctx=FakeDeviceContext()).read() == safetensors_torch.save(disjoint)
 
 
 def test_safetensors_rejections_name_what_is_wrong():
-    ctx = SegmentFakeContext()
+    ctx = FakeDeviceContext()
     ok = torch.zeros(4)
     with pytest.raises(ValueError, match="'w'.*CUDA"):
         DeviceFile.safetensors({"w": ok})  # a CPU tensor where GPU memory is expected
@@ -346,12 +272,12 @@ def _edge_state_dicts(BS: int):
     yield _rand_state_dict(rng, 50)
 
 
-def test_spec2_of_safetensors_file_equals_spec2_of_bytesio(fake_segment_backend, monkeypatch):
+def test_spec2_of_safetensors_file_equals_spec2_of_bytesio(fake_device_backend, monkeypatch):
     BS = 4096
     monkeypatch.setattr(blob_utils, "BLOCK_SIZE", BS)
     for sd in _edge_state_dicts(BS):
         image = safetensors_torch.save(sd)
-        f = HostDeviceFile.safetensors(sd, ctx=fake_segment_backend)
+        f = HostDeviceFile.safetensors(sd, ctx=fake_device_backend)
         sem = asyncio.Semaphore(1)
         dev = asyncio.run(blob_utils.FileUploadSpec2.from_fileobj(f, PurePosixPath("/m.safetensors"), sem, 0o644))
         host = asyncio.run(blob_utils.FileUploadSpec2.from_fileobj(io.BytesIO(image), PurePosixPath("/m.safetensors"),
@@ -360,23 +286,23 @@ def test_spec2_of_safetensors_file_equals_spec2_of_bytesio(fake_segment_backend,
         assert f.bytes_to_host == 0  # only the digest table was fetched
         with dev.source() as rd:
             assert rd.read() == image
-    assert ("hash_segment_parts_device", 1, BS, _lib.SHA256 | _lib.TRIM_ZEROS) in fake_segment_backend.calls
+    assert ("hash_segment_parts_device", 1, BS, _lib.SHA256 | _lib.TRIM_ZEROS) in fake_device_backend.calls
 
 
-def test_batch_of_device_files_makes_one_call(fake_segment_backend, monkeypatch):
+def test_batch_of_device_files_makes_one_call(fake_device_backend, monkeypatch):
     BS = 4096
     monkeypatch.setattr(blob_utils, "BLOCK_SIZE", BS)
     sds = list(_edge_state_dicts(BS))
     images = [safetensors_torch.save(sd) for sd in sds]
     plain = [synth_bytes(40 + i, n) for i, n in enumerate((0, 1, BS, 3 * BS + 1))]
     for k in (1, 2, 5, len(sds) + len(plain)):
-        files = [HostDeviceFile.safetensors(sd, ctx=fake_segment_backend) for sd in sds]
+        files = [HostDeviceFile.safetensors(sd, ctx=fake_device_backend) for sd in sds]
         files += [host_segments_file([p]) for p in plain]
         datas = images + plain
         items = [(f, PurePosixPath(f"/f{i}"), 0o600) for i, f in enumerate(files[:k])]
-        fake_segment_backend.calls.clear()
+        fake_device_backend.calls.clear()
         specs = asyncio.run(blob_utils.device_file_specs2(items))
-        dev_calls = [c for c in fake_segment_backend.calls if c[0].startswith("hash_")]
+        dev_calls = [c for c in fake_device_backend.calls if c[0].startswith("hash_")]
         assert len(dev_calls) == (1 if any(len(d) for d in datas[:k]) else 0)
         for spec, data, (f, remote, _) in zip(specs, datas, items):
             want = asyncio.run(blob_utils.FileUploadSpec2.from_fileobj(io.BytesIO(data), remote, asyncio.Semaphore(1),
@@ -385,7 +311,7 @@ def test_batch_of_device_files_makes_one_call(fake_segment_backend, monkeypatch)
             assert f.bytes_to_host == 0
 
 
-def test_v2_round_puts_only_missing_blocks_of_a_safetensors_file(fake_segment_backend, monkeypatch):
+def test_v2_round_puts_only_missing_blocks_of_a_safetensors_file(fake_device_backend, monkeypatch):
     BS = 4096
     monkeypatch.setattr(blob_utils, "BLOCK_SIZE", BS)
     sd = _rand_state_dict(random.Random(21), 40)
@@ -397,7 +323,7 @@ def test_v2_round_puts_only_missing_blocks_of_a_safetensors_file(fake_segment_ba
     async def run():
         async with _volume_server(BS) as (stub, _):
             client = types.SimpleNamespace(stub=stub)
-            f = HostDeviceFile.safetensors(sd, ctx=fake_segment_backend, bounce_bytes=1000)
+            f = HostDeviceFile.safetensors(sd, ctx=fake_device_backend, bounce_bytes=1000)
             extra = host_segments_file([b"x" * 100, synth_bytes(2, 2 * BS)])
             async with volume.VolumeUploadContextManager2("vo-s", client) as batch:
                 batch.put_file(io.BytesIO(b"plain"), "/p")
@@ -407,12 +333,12 @@ def test_v2_round_puts_only_missing_blocks_of_a_safetensors_file(fake_segment_ba
             assert stub.volume_files["/ckpt/extra.bin"][0] == b"x" * 100 + synth_bytes(2, 2 * BS)
             assert stub.volume_files["/p"][0] == b"plain"
             assert f.bytes_to_host == _trimmed_total(image, BS)
-            assert sum(c[0] == "hash_segment_parts_device" for c in fake_segment_backend.calls) == 1
+            assert sum(c[0] == "hash_segment_parts_device" for c in fake_device_backend.calls) == 1
             # one tensor changes: only the blocks holding its bytes travel again
             sd["big"][7] ^= 0xFF
             image2 = safetensors_torch.save(sd)
             changed = [i for i in range(nblocks) if image2[i * BS : (i + 1) * BS] != image[i * BS : (i + 1) * BS]]
-            g = HostDeviceFile.safetensors(sd, ctx=fake_segment_backend)
+            g = HostDeviceFile.safetensors(sd, ctx=fake_device_backend)
             before = stub.block_puts
             async with volume.VolumeUploadContextManager2("vo-s", client, force=True) as batch:
                 batch.put_file(g, "/ckpt/model.safetensors")
@@ -423,7 +349,7 @@ def test_v2_round_puts_only_missing_blocks_of_a_safetensors_file(fake_segment_ba
     asyncio.run(run())
 
 
-def test_v1_put_file_of_a_safetensors_file(fake_segment_backend, monkeypatch):
+def test_v1_put_file_of_a_safetensors_file(fake_device_backend, monkeypatch):
     monkeypatch.setattr(blob_utils, "LARGE_FILE_LIMIT", 4000)
     sd = _rand_state_dict(random.Random(8), 30)
     sd["w"] = torch.frombuffer(bytearray(synth_bytes(3, 20_000)), dtype=torch.uint8)
@@ -434,7 +360,7 @@ def test_v1_put_file_of_a_safetensors_file(fake_segment_backend, monkeypatch):
             stub = FakeVolumeStub(host, store, 8 << 20)
             client = types.SimpleNamespace(stub=stub)
             async with volume.VolumeUploadContextManager("vo-1", client) as batch:
-                batch.put_file(HostDeviceFile.safetensors(sd, ctx=fake_segment_backend, bounce_bytes=1 << 12), "/m")
+                batch.put_file(HostDeviceFile.safetensors(sd, ctx=fake_device_backend, bounce_bytes=1 << 12), "/m")
             got, _, sha = stub.volume_files["/m"]
             assert got == image and sha == hashlib.sha256(image).hexdigest()
             await blob_utils.ClientSessionRegistry.close_session()

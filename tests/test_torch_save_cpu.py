@@ -8,7 +8,6 @@ import pickle
 import random
 import types
 import zipfile
-import zlib
 from pathlib import PurePosixPath
 
 import numpy as np
@@ -16,50 +15,12 @@ import pytest
 import torch
 from torch.utils.serialization import config
 
-from modal_client_b200 import DeviceFile, _lib, blob_utils, device_file, volume
+from modal_client_b200 import _lib, blob_utils, device_file, volume
 from modal_client_b200.synth import synth_bytes
-from tests.test_device_file_cpu import _trimmed_total, _volume_server
-from tests.test_segment_parts_cpu import SegmentFakeContext, _HostSegments, host_segments_file
+from tests.test_device_file_cpu import (  # noqa: F401 (fake_device_backend: a fixture)
+    FakeDeviceContext, HostDeviceFile, _trimmed_total, _volume_server, fake_device_backend, host_segments_file)
 
 safetensors_torch = pytest.importorskip("safetensors.torch")
-
-
-class CrcFakeContext(SegmentFakeContext):
-    """SegmentFakeContext plus ``crc32_device`` over HOST addresses (CPU tensors standing in for device memory)."""
-
-    def crc32_device(self, ptrs, lens, d_out, stream=0):
-        self.calls.append(("crc32_device", len(lens)))
-        crcs = np.array([zlib.crc32(ctypes.string_at(int(p), int(n))) if n else 0 for p, n in zip(ptrs, lens)],
-                        np.uint32)
-        if len(crcs):
-            ctypes.memmove(d_out, crcs.tobytes(), crcs.nbytes)
-
-
-class _HostSave(_HostSegments):
-    @classmethod
-    def _pinned(cls, n):
-        return torch.empty(n, dtype=torch.uint8)
-
-    @classmethod
-    def _empty(cls, n, ctx):
-        return torch.empty(n, dtype=torch.uint8)
-
-    @classmethod
-    def _current_stream(cls, ctx):
-        return 0
-
-
-class HostSaveFile(DeviceFile):
-    _Source = _HostSave
-
-
-@pytest.fixture
-def fake_crc_backend(monkeypatch):
-    from modal_client_b200 import _backend
-
-    ctx = CrcFakeContext()
-    monkeypatch.setattr(_backend, "_override", ctx)
-    return ctx
 
 
 def saved(obj) -> bytes:
@@ -124,8 +85,8 @@ CASES = dict(_cases())
 def test_image_equals_torch_save(name):
     obj = CASES[name]
     want = saved(obj)
-    ctx = CrcFakeContext()
-    f = HostSaveFile.torch_save(obj, ctx=ctx, bounce_bytes=random.Random(name).choice([1, 7, 100, 1 << 20]))
+    ctx = FakeDeviceContext()
+    f = HostDeviceFile.torch_save(obj, ctx=ctx, bounce_bytes=random.Random(name).choice([1, 7, 100, 1 << 20]))
     assert f.nbytes == len(want)
     got = f.read()
     assert got == want
@@ -139,7 +100,7 @@ def test_image_equals_torch_save(name):
 
 def test_keys_ten_and_up_follow_nine():
     sd = {f"k{i}": torch.full((2,), float(i)) for i in range(12)}
-    names = zipfile.ZipFile(io.BytesIO(HostSaveFile.torch_save(sd, ctx=CrcFakeContext()).read())).namelist()
+    names = zipfile.ZipFile(io.BytesIO(HostDeviceFile.torch_save(sd, ctx=FakeDeviceContext()).read())).namelist()
     data = [n for n in names if n.startswith("archive/data/")]
     assert data == [f"archive/data/{i}" for i in range(12)]
 
@@ -148,8 +109,8 @@ def test_without_crc32_the_skeleton_is_the_file(monkeypatch):
     monkeypatch.setattr(config.save, "compute_crc32", False)
     obj = _adam_state()
     want = saved(obj)
-    ctx = CrcFakeContext()
-    f = HostSaveFile.torch_save(obj, ctx=ctx)
+    ctx = FakeDeviceContext()
+    f = HostDeviceFile.torch_save(obj, ctx=ctx)
     assert f.read() == want
     assert not [c for c in ctx.calls if c[0] == "crc32_device"]
     assert all(i.CRC == 0 for i in zipfile.ZipFile(io.BytesIO(want)).infolist())
@@ -171,7 +132,7 @@ def test_random_reads_across_segment_edges():
     obj = {"sd": _state_dict(9, 30), "opt": _adam_state()}
     want = saved(obj)
     for bounce in (1, 5, 64, 4096):
-        f, ref = HostSaveFile.torch_save(obj, ctx=CrcFakeContext(), bounce_bytes=bounce), io.BytesIO(want)
+        f, ref = HostDeviceFile.torch_save(obj, ctx=FakeDeviceContext(), bounce_bytes=bounce), io.BytesIO(want)
         for _ in range(150):
             op = rng.randrange(3)
             if op == 0:
@@ -191,7 +152,7 @@ def test_random_reads_across_segment_edges():
 def test_torch_load_round_trip():
     obj = _adam_state()
     obj["views"] = CASES["views"]
-    back = torch.load(io.BytesIO(HostSaveFile.torch_save(obj, ctx=CrcFakeContext()).read()), weights_only=True)
+    back = torch.load(io.BytesIO(HostDeviceFile.torch_save(obj, ctx=FakeDeviceContext()).read()), weights_only=True)
     for k, t in obj["model"].items():
         assert torch.equal(back["model"][k], t)
     assert back["optim"]["param_groups"] == obj["optim"]["param_groups"]
@@ -205,7 +166,7 @@ def test_torch_load_round_trip():
 
 def test_rejections_name_the_device():
     with pytest.raises(ValueError, match="meta"):
-        HostSaveFile.torch_save({"w": torch.zeros(4, device="meta")}, ctx=CrcFakeContext())
+        HostDeviceFile.torch_save({"w": torch.zeros(4, device="meta")}, ctx=FakeDeviceContext())
 
 
 def test_layout_check_rejects_a_compressed_archive():
@@ -239,12 +200,12 @@ def _edge_checkpoints(BS: int):
     yield _state_dict(11, 30)
 
 
-def test_spec2_of_torch_save_file_equals_spec2_of_bytesio(fake_crc_backend, monkeypatch):
+def test_spec2_of_torch_save_file_equals_spec2_of_bytesio(fake_device_backend, monkeypatch):
     BS = 4096
     monkeypatch.setattr(blob_utils, "BLOCK_SIZE", BS)
     for obj in _edge_checkpoints(BS):
         image = saved(obj)
-        f = HostSaveFile.torch_save(obj, ctx=fake_crc_backend)
+        f = HostDeviceFile.torch_save(obj, ctx=fake_device_backend)
         sem = asyncio.Semaphore(1)
         dev = asyncio.run(blob_utils.FileUploadSpec2.from_fileobj(f, PurePosixPath("/c.pt"), sem, 0o644))
         host = asyncio.run(blob_utils.FileUploadSpec2.from_fileobj(io.BytesIO(image), PurePosixPath("/c.pt"), sem,
@@ -255,19 +216,19 @@ def test_spec2_of_torch_save_file_equals_spec2_of_bytesio(fake_crc_backend, monk
             assert rd.read() == image
 
 
-def test_batch_of_torch_save_safetensors_and_plain_makes_one_call(fake_crc_backend, monkeypatch):
+def test_batch_of_torch_save_safetensors_and_plain_makes_one_call(fake_device_backend, monkeypatch):
     BS = 4096
     monkeypatch.setattr(blob_utils, "BLOCK_SIZE", BS)
     ckpt = _adam_state()
     sd = {"w": torch.frombuffer(bytearray(synth_bytes(4, 3 * BS + 5)), dtype=torch.uint8), "b": torch.ones(7)}
     plain = synth_bytes(6, 2 * BS + 1)
-    files = [HostSaveFile.torch_save(ckpt, ctx=fake_crc_backend),
-             HostSaveFile.safetensors(sd, ctx=fake_crc_backend), host_segments_file([plain])]
+    files = [HostDeviceFile.torch_save(ckpt, ctx=fake_device_backend),
+             HostDeviceFile.safetensors(sd, ctx=fake_device_backend), host_segments_file([plain])]
     datas = [saved(ckpt), safetensors_torch.save(sd), plain]
     items = [(f, PurePosixPath(f"/f{i}"), 0o600) for i, f in enumerate(files)]
-    fake_crc_backend.calls.clear()
+    fake_device_backend.calls.clear()
     specs = asyncio.run(blob_utils.device_file_specs2(items))
-    assert [c[0] for c in fake_crc_backend.calls if c[0].startswith("hash_")] == ["hash_segment_parts_device"]
+    assert [c[0] for c in fake_device_backend.calls if c[0].startswith("hash_")] == ["hash_segment_parts_device"]
     for spec, data, (f, remote, _) in zip(specs, datas, items):
         want = asyncio.run(blob_utils.FileUploadSpec2.from_fileobj(io.BytesIO(data), remote, asyncio.Semaphore(1),
                                                                    0o600))
@@ -275,7 +236,7 @@ def test_batch_of_torch_save_safetensors_and_plain_makes_one_call(fake_crc_backe
         assert f.bytes_to_host == 0
 
 
-def test_v2_round_puts_only_missing_blocks_of_a_torch_save_file(fake_crc_backend, monkeypatch):
+def test_v2_round_puts_only_missing_blocks_of_a_torch_save_file(fake_device_backend, monkeypatch):
     BS = 4096
     monkeypatch.setattr(blob_utils, "BLOCK_SIZE", BS)
     ckpt = _adam_state()
@@ -287,7 +248,7 @@ def test_v2_round_puts_only_missing_blocks_of_a_torch_save_file(fake_crc_backend
     async def run():
         async with _volume_server(BS) as (stub, _):
             client = types.SimpleNamespace(stub=stub)
-            f = HostSaveFile.torch_save(ckpt, ctx=fake_crc_backend, bounce_bytes=1000)
+            f = HostDeviceFile.torch_save(ckpt, ctx=fake_device_backend, bounce_bytes=1000)
             async with volume.VolumeUploadContextManager2("vo-t", client) as batch:
                 batch.put_file(io.BytesIO(b"plain"), "/p")
                 batch.put_file(f, "/ckpt/last.pt")
@@ -297,7 +258,7 @@ def test_v2_round_puts_only_missing_blocks_of_a_torch_save_file(fake_crc_backend
             ckpt["big"][7] ^= 0xFF
             image2 = saved(ckpt)
             changed = [i for i in range(nblocks) if image2[i * BS : (i + 1) * BS] != image[i * BS : (i + 1) * BS]]
-            g = HostSaveFile.torch_save(ckpt, ctx=fake_crc_backend)
+            g = HostDeviceFile.torch_save(ckpt, ctx=fake_device_backend)
             before = stub.block_puts
             async with volume.VolumeUploadContextManager2("vo-t", client, force=True) as batch:
                 batch.put_file(g, "/ckpt/last.pt")

@@ -1,7 +1,8 @@
 """tools/device_blocks_bench.py -- volumefs2 block hashing (8 MiB blocks, zero trim + SHA-256) of one large CUDA tensor:
 
-  device   DeviceFile(t).hash_parts(BLOCK_SIZE, SHA256 | TRIM_ZEROS): one b200h_hash_fixed_parts_device call where the
-           tensor lives; only the (trimmed length, SHA-256) table comes to the host
+  device   DeviceFile(t).hash_parts(BLOCK_SIZE, SHA256 | TRIM_ZEROS): one b200h_hash_segment_parts_device call (one
+           segment, every block in place) where the tensor lives; only the (trimmed length, SHA-256) table comes to
+           the host
   host     what a caller had to do before DeviceFile: t.cpu(), then the blocks of that host image the way
            FileUploadSpec2.from_fileobj builds them (b200h_hash_fixed_parts, which stages the bytes back to the GPU)
 

@@ -7,8 +7,8 @@ call to the block table on the host (every arm ends in a synchronisation):
 
   a  segmented     DeviceFile.safetensors(sd) -> FileUploadSpec2 blocks: ONE b200h_hash_segment_parts_device call;
                    the blocks that straddle tensors are gathered into a wave slot, the others hashed in place
-  a0 aligned       the same image bytes in one 16-byte-aligned buffer -> DeviceFile(buf) blocks (b200h_hash_fixed_parts_
-                   device): a against a0 is the cost of in-place parts that start unaligned plus the gather
+  a0 aligned       the same image bytes in one 16-byte-aligned buffer -> DeviceFile(buf) blocks (the same entry with one
+                   segment): a against a0 is the cost of in-place parts that start unaligned plus the gather
   b  cat           torch.cat of the header and every tensor's bytes into one buffer -> DeviceFile(buf) blocks
   c  host          safetensors.torch.save on the host -> FileUploadSpec2.from_fileobj(BytesIO)
   d1 files/call    the tensors as separate files in one v2 batch, one library call per file (from_fileobj each)
