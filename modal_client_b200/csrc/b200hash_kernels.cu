@@ -78,6 +78,12 @@ __device__ __forceinline__ uint32_t addf(uint32_t a, uint32_t b, uint32_t one) {
     asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(one), "r"(b));
     return d;
 }
+// acc + rotl(u, k) as one plain add of a funnel shift: ptxas fuses the two into a single ALU-pipe LEA.HI
+// (acc + ((u:u) << k) >> 32), so the add leaves the FMA pipe without a rotate being added to the ALU pipe.
+template <int K>
+__device__ __forceinline__ uint32_t add_rotl(uint32_t acc, uint32_t u) {
+    return acc + __funnelshift_l(u, u, K);
+}
 __device__ __forceinline__ uint32_t rotr(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
 __device__ __forceinline__ uint32_t rotl(uint32_t x, int n) { return __funnelshift_l(x, x, n); }
 __device__ __forceinline__ uint32_t bswap(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
@@ -122,20 +128,25 @@ __device__ __forceinline__ uint32_t addv(uint32_t a, uint32_t b) {
 // alone on its SMSP issues one instruction per two cycles whatever the pipe, so fewer instructions win).
 #define ADD(x, y) (kPlainAdd ? ((x) + (y)) : addf((x), (y), one))
 #endif
-// B200H_SHAONLY_ROT: in the SHA-256-only instantiation the ALU pipe carries 1040 of the 1640 instructions
-// per block while the FMA pipe idles, so some shifts are moved over as multiplies:
-//   bit 0 / bit 1: the outer rotate of Sigma1 / Sigma0 (Sigma1(e) = rotr6(e ^ rotr5(e) ^ rotr19(e)),
-//                  Sigma0(a) = rotr2(a ^ rotr11(a) ^ rotr20(a))) is a widening multiply x * 2^(32-n) ->
-//                  {x << (32-n), x >> n}; the halves have disjoint bits, so both are simply added into the
-//                  round sum (one SHF less, one IMAD.WIDE + one IMAD more);
-//   bit 2:         the plain shifts of sigma0/sigma1 are IMAD.HI by 2^(32-n) (multiplier in a register so that
-//                  ptxas cannot turn it back into a shift).
-// The fused kernel does not use it: its FMA pipe is already loaded with MD5's adds.
+// The outer rotate of Sigma1 / Sigma0 ends in an add once it is factored out: Sigma1(e) = rotr6(e ^ rotr5(e) ^ rotr19(e)) goes into T1, Sigma0(a) = rotr2(a ^
+// rotr11(a) ^ rotr20(a)) onto Maj.
+// B200H_SHAONLY_ROT, the SHA-256-only instantiation, where the ALU pipe carries 1040 of the 1640 instructions per
+// block while the FMA pipe idles:
+//   bit 0 / bit 1: the outer rotate of Sigma1 / Sigma0 is a widening multiply x * 2^(32-n) -> {x << (32-n), x >> n};
+//                  the halves have disjoint bits, so both are simply added into the round sum (one SHF less, one
+//                  IMAD.WIDE + one IMAD more);
+//   bit 2:         the plain shifts of sigma0/sigma1 are IMAD.HI by 2^(32-n).
+// B200H_FUSED_MIX, the dense fused SHA-256 + MD5 instantiation, where the kernel issues at the rate an SMSP sustains
+// for a mix of ALU-pipe and FMA-pipe instructions, so its time follows the instruction count (DESIGN.md 5.1): a rotate
+// whose result is added becomes one LEA.HI (add_rotl) in place of SHF + IMAD, 1 instruction less, ALU pipe unchanged:
+//   bit 0 / bit 1: Sigma1 / Sigma0 outer rotate with its add (128 per block);
+//   bit 2:         MD5's a = b + rotl(t, s) (64 per block).
+// Multiplies do not pay here: IMAD.HI issues at half the rate of IMAD or SHF on H100 (tools/ubench.cu).
 #ifndef B200H_SHAONLY_ROT
 #define B200H_SHAONLY_ROT 3
 #endif
-#ifndef B200H_FUSED_ROT
-#define B200H_FUSED_ROT 0
+#ifndef B200H_FUSED_MIX
+#define B200H_FUSED_MIX 7
 #endif
 __device__ __forceinline__ void rotw(uint32_t x, uint32_t mul, uint32_t& lo, uint32_t& hi) {
     uint64_t d;
@@ -148,11 +159,14 @@ __device__ __forceinline__ uint32_t mulhi(uint32_t x, uint32_t m) {
     asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(m));
     return d;
 }
-template <int ROT>
+// FUSED: the Sigma rotates through add_rotl (B200H_FUSED_MIX) instead of rotw (B200H_SHAONLY_ROT)
+template <int ROT, bool FUSED>
 __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, uint32_t& d, uint32_t e, uint32_t f,
                                             uint32_t g, uint32_t& h, uint32_t K, uint32_t W, uint32_t one) {
     uint32_t t1 = addf(addf(h, addf(W, K, one), one), lop3<0xCA>(e, f, g), one);
-    if (ROT & 1) {
+    if ((ROT & 1) && FUSED) {
+        t1 = add_rotl<26>(t1, lop3<0x96>(e, rotr(e, 5), rotr(e, 19)));
+    } else if (ROT & 1) {
         uint32_t lo, hi;
         rotw(lop3<0x96>(e, rotr(e, 5), rotr(e, 19)), 1u << 26, lo, hi);
         t1 = addf(addf(t1, lo, one), hi, one);
@@ -160,7 +174,9 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
         t1 = addf(t1, lop3<0x96>(rotr(e, 6), rotr(e, 11), rotr(e, 25)), one);
     }
     uint32_t t2;
-    if (ROT & 2) {
+    if ((ROT & 2) && FUSED) {
+        t2 = add_rotl<30>(lop3<0xE8>(a, b, c), lop3<0x96>(a, rotr(a, 11), rotr(a, 20)));
+    } else if (ROT & 2) {
         uint32_t lo, hi;
         rotw(lop3<0x96>(a, rotr(a, 11), rotr(a, 20)), 1u << 30, lo, hi);
         t2 = addf(addf(lo, hi, one), lop3<0xE8>(a, b, c), one);
@@ -194,10 +210,11 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
         h = ADD(t1, t2);                                                              \
     }
 #endif
-// kShaRot (a constant inside compress<>) is B200H_SHAONLY_ROT for the SHA-only instantiation, else 0
+// kShaRot (a constant inside compress<>) is B200H_SHAONLY_ROT for the dense SHA-only instantiation, bits 0 and 1 of
+// B200H_FUSED_MIX for the dense fused one, else 0
 #define SHA_RND(a, b, c, d, e, f, g, h, K, W)                                           \
     {                                                                                   \
-        if (kShaRot & 3) sha_rnd_rot<kShaRot>(a, b, c, d, e, f, g, h, K, W, one);       \
+        if (kShaRot & 3) sha_rnd_rot<kShaRot, DO_MD5>(a, b, c, d, e, f, g, h, K, W, one); \
         else SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                 \
     }
 #define SHA_SHR3(x) ((kShaRot & 4) ? mulhi((x), m29) : ((x) >> 3))
@@ -208,19 +225,14 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
 #define SHA_SCHED(w, i) \
     (w[(i)&15] = ADD(ADD(ADD(w[(i)&15], w[((i)-7) & 15]), SHA_s0r(w[((i)-15) & 15])), SHA_s1r(w[((i)-2) & 15])))
 
-// Fused kernel: every add of an MD5 step on the FMA pipe (the ALU pipe is saturated by SHA-256's shifts).
-#if defined(B200H_MD5LEA) && B200H_MD5LEA
-// b + rotl(t, s) left to ptxas: it fuses the rotate and the add into one ALU-pipe LEA.HI (one FMA add less per step)
-#define MD5_STEP_FMA(FN, a, b, c, d, xk, s, T)             \
-    {                                                      \
-        a = b + rotl(ADD(ADD(a, ADD(xk, T)), FN(b, c, d)), s); \
+// Fused kernel: the adds of an MD5 step on the FMA pipe; with kMd5Rot (bit 2 of B200H_FUSED_MIX in the dense fused
+// instantiation, else 0) the last one is fused with the rotate into one LEA.HI
+#define MD5_STEP_FMA(FN, a, b, c, d, xk, s, T)                                    \
+    {                                                                             \
+        const uint32_t t_ = ADD(ADD(a, ADD(xk, T)), FN(b, c, d));                 \
+        if (kMd5Rot) a = add_rotl<(s)>(b, t_);                                    \
+        else a = ADD(b, rotl(t_, s));                                             \
     }
-#else
-#define MD5_STEP_FMA(FN, a, b, c, d, xk, s, T)             \
-    {                                                      \
-        a = ADD(b, rotl(ADD(ADD(a, ADD(xk, T)), FN(b, c, d)), s)); \
-    }
-#endif
 // MD5-only kernel: there the FMA pipe is the bottleneck (4 IMAD vs 2 ALU ops per step), so the 3-input sum
 // goes back to the ALU pipe as one IADD3: per step ALU = LOP3 + IADD3 + SHF, FMA = (x+T) and (+b).
 #define MD5_STEP_MIX(FN, a, b, c, d, xk, s, T)             \
@@ -264,11 +276,11 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     constexpr bool kPlainAdd = SPARSE;
     uint32_t w[16];
     uint32_t m14 = x[14], m15 = x[15];
-    // multiplies add instructions: dense instantiations only.  B200H_FUSED_ROT (default 0) is the same knob for the fused
-    // kernel: bit 2 (sigma shifts as IMAD.HI) does not pay there either.
-    constexpr int kShaRot = SPARSE ? 0 : (DO_MD5 ? (B200H_FUSED_ROT) : (B200H_SHAONLY_ROT));
+    // dense instantiations only: the sparse one leaves every add to ptxas, which fuses them itself
+    constexpr int kShaRot = SPARSE ? 0 : (DO_MD5 ? (B200H_FUSED_MIX & 3) : (B200H_SHAONLY_ROT));
+    constexpr bool kMd5Rot = DO_SHA && DO_MD5 && !SPARSE && (B200H_FUSED_MIX & 4);
     const uint32_t m29 = one << 29, m22 = one << 22;  // 2^29, 2^22 as run-time values (bit 2 of kShaRot)
-    (void)m29; (void)m22;
+    (void)m29; (void)m22; (void)kMd5Rot;
     if (DO_SHA) {
 #pragma unroll
         for (int i = 0; i < 16; ++i) w[i] = bswap(x[i]);

@@ -92,6 +92,15 @@ __global__ void k(uint32_t* out, uint32_t one, uint32_t seed, long long* cyc) {
                 else asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));
             }
             if (MODE == 18) asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(fa[i]) : "f"(fb), "f"(fc));      // FFMA alone
+            // acc + rotl(u, 26) on the FMA pipe: multiplier one << 26 (a run-time value), 32-bit accumulator b
+            if (MODE == 21) asm volatile("mad.hi.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one << 26), "r"(b));  // IMAD.HI R,UR,R
+            if (MODE == 22) asm volatile("{ .reg .u32 t; mad.hi.u32 t, %0, %1, %2; mad.lo.u32 %0, %0, %1, t; }"
+                                         : "+r"(a[i]) : "r"(one << 26), "r"(b));                            // IMAD.HI + IMAD
+            if (MODE == 23) {  // alternate LOP3 and IMAD.HI R,UR,R
+                if (i & 1) asm volatile("mad.hi.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one << 26), "r"(b));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+            }
+            if (MODE == 24) asm volatile("mul.hi.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(one << 26));               // IMAD.HI R,UR,RZ
         }
     }
     long long t1 = clock64();
@@ -124,7 +133,7 @@ void run(const char* name, int warps_per_smsp) {
     cudaMemcpy(&c, cyc, 8, cudaMemcpyDeviceToHost);
     float ms;
     cudaEventElapsedTime(&ms, e0, e1);
-    double inst = (double)ITER * ACC * warps_per_smsp;  // warp-instructions per SMSP
+    double inst = (double)ITER * ACC * warps_per_smsp * (MODE == 22 ? 2 : 1);  // warp-instructions per SMSP
     printf("%-28s warps/SMSP=%d  cycles=%lld  IPC/SMSP=%.3f  (%.3f ms)\n", name, warps_per_smsp, c, inst / c, ms);
     cudaFree(out);
     cudaFree(cyc);
@@ -154,6 +163,11 @@ int main() {
         if (w == 4) { run<11>("IMAD.WIDE imm", 4); run<12>("LOP3 + IMAD.WIDE alt", 4); run<13>("2 LOP3 : 1 IMAD", 4); run<14>("1 LOP3 : 2 IMAD", 4); run<15>("IMAD.HI", 4); run<16>("hash mix 7 ALU : 5 IMAD", 4); run<17>("LOP3 + FFMA alt", 4); run<18>("FFMA RRR", 4); }
         if (w == 5) { run<7>("LOP3 + IMAD RRR alt", 5); run<12>("LOP3 + IMAD.WIDE alt", 5); run<13>("2 LOP3 : 1 IMAD", 5); run<16>("hash mix 7 ALU : 5 IMAD", 5); }
         if (w == 8) { run<11>("IMAD.WIDE imm", 8); run<12>("LOP3 + IMAD.WIDE alt", 8); run<13>("2 LOP3 : 1 IMAD", 8); run<14>("1 LOP3 : 2 IMAD", 8); run<15>("IMAD.HI", 8); run<16>("hash mix 7 ALU : 5 IMAD", 8); run<17>("LOP3 + FFMA alt", 8); run<18>("FFMA RRR", 8); }
+    }
+    // acc + rotl(u, k) = mad.lo(u, 2^k, mad.hi(u, 2^k, acc)): the forms alone and against the ALU pipe
+    for (int w : {1, 4, 5, 8}) {
+        run<21>("IMAD.HI R,UR,R (acc)", w); run<24>("IMAD.HI R,UR,RZ", w); run<22>("IMAD.HI + IMAD pair", w);
+        run<23>("LOP3 + IMAD.HI alt", w); run<1>("IMAD R,R,R(one),R", w); run<7>("LOP3 + IMAD RRR alt", w);
     }
     return 0;
 }
