@@ -136,18 +136,30 @@ __device__ __forceinline__ uint32_t addv(uint32_t a, uint32_t b) {
 //                  the halves have disjoint bits, so both are simply added into the round sum (one SHF less, one
 //                  IMAD.WIDE + one IMAD more);
 //   bit 2:         the plain shifts of sigma0/sigma1 are IMAD.HI by 2^(32-n).
-// B200H_FUSED_MIX, the dense fused SHA-256 + MD5 instantiation, where the kernel issues at the rate an SMSP sustains
-// for a mix of ALU-pipe and FMA-pipe instructions, so its time follows the instruction count (DESIGN.md 5.1): a rotate
+// B200H_FUSED_MIX, the dense fused SHA-256 + MD5 instantiation, where the kernel issues at the rate its vector
+// register reads allow, well under both pipes' rates, so fewer instructions win (DESIGN.md 5.1): a rotate
 // whose result is added becomes one LEA.HI (add_rotl) in place of SHF + IMAD, 1 instruction less, ALU pipe unchanged:
 //   bit 0 / bit 1: Sigma1 / Sigma0 outer rotate with its add (128 per block);
 //   bit 2:         MD5's a = b + rotl(t, s) (64 per block).
 // Multiplies do not pay here: IMAD.HI issues at half the rate of IMAD or SHF on H100 (tools/ubench.cu).
+// B200H_FUSED_CONST_ADD, the dense fused instantiation: 1 = the adds of a round constant (SHA-256's W + K, MD5's
+// x + T, 128 per block) are plain adds, which ptxas issues as VIADD R, R, imm; 0 = IMAD R, R, R(one), imm.  Any IMAD
+// with an immediate addend makes ptxas keep `one` in a vector register for every addf, so each of the other 528 adds
+// of a block reads three vector registers; with 1 they read `one` from a uniform register (IMAD R, R, UR, R), which
+// saves a vector register-file read per add (DESIGN.md 5.1).  VIADD stays off the ALU pipe: it issues next to SHF and
+// LOP3 above that pipe's rate (tools/ubench.cu).
 #ifndef B200H_SHAONLY_ROT
 #define B200H_SHAONLY_ROT 3
 #endif
 #ifndef B200H_FUSED_MIX
 #define B200H_FUSED_MIX 7
 #endif
+#ifndef B200H_FUSED_CONST_ADD
+#define B200H_FUSED_CONST_ADD 1
+#endif
+// x + a round constant; kConstAdd (a constant inside compress<>) is B200H_FUSED_CONST_ADD in the dense fused
+// instantiation, else 0
+#define ADDK(x, k) (kConstAdd ? ((x) + (k)) : ADD((x), (k)))
 __device__ __forceinline__ void rotw(uint32_t x, uint32_t mul, uint32_t& lo, uint32_t& hi) {
     uint64_t d;
     asm("mul.wide.u32 %0, %1, %2;" : "=l"(d) : "r"(x), "r"(mul));
@@ -163,7 +175,8 @@ __device__ __forceinline__ uint32_t mulhi(uint32_t x, uint32_t m) {
 template <int ROT, bool FUSED>
 __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, uint32_t& d, uint32_t e, uint32_t f,
                                             uint32_t g, uint32_t& h, uint32_t K, uint32_t W, uint32_t one) {
-    uint32_t t1 = addf(addf(h, addf(W, K, one), one), lop3<0xCA>(e, f, g), one);
+    const uint32_t kw = (FUSED && B200H_FUSED_CONST_ADD) ? W + K : addf(W, K, one);
+    uint32_t t1 = addf(addf(h, kw, one), lop3<0xCA>(e, f, g), one);
     if ((ROT & 1) && FUSED) {
         t1 = add_rotl<26>(t1, lop3<0x96>(e, rotr(e, 5), rotr(e, 19)));
     } else if (ROT & 1) {
@@ -190,21 +203,21 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
 // mode 3: only the last sum of a round (new a = T1 + Sigma0 + Maj) is a 3-input IADD3 on the ALU pipe
 #define SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                         \
     {                                                                                 \
-        uint32_t t1 = ADD(ADD(ADD(h, ADD(W, K)), lop3<0xCA>(e, f, g)), SHA_S1(e));    \
+        uint32_t t1 = ADD(ADD(ADD(h, ADDK(W, K)), lop3<0xCA>(e, f, g)), SHA_S1(e));   \
         d = ADD(d, t1);                                                               \
         h = t1 + SHA_S0(a) + lop3<0xE8>(a, b, c);                                     \
     }
 #elif B200H_ADDMODE == 2
 #define SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                  \
     {                                                                          \
-        uint32_t t1 = ADD(h, ADD(W, K)) + SHA_S1(e) + lop3<0xCA>(e, f, g);     \
+        uint32_t t1 = ADD(h, ADDK(W, K)) + SHA_S1(e) + lop3<0xCA>(e, f, g);    \
         d = ADD(d, t1);                                                        \
         h = t1 + SHA_S0(a) + lop3<0xE8>(a, b, c);                              \
     }
 #else
 #define SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                         \
     {                                                                                 \
-        uint32_t t1 = ADD(ADD(ADD(h, ADD(W, K)), lop3<0xCA>(e, f, g)), SHA_S1(e));    \
+        uint32_t t1 = ADD(ADD(ADD(h, ADDK(W, K)), lop3<0xCA>(e, f, g)), SHA_S1(e));   \
         uint32_t t2 = ADD(SHA_S0(a), lop3<0xE8>(a, b, c));                            \
         d = ADD(d, t1);                                                               \
         h = ADD(t1, t2);                                                              \
@@ -226,10 +239,10 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
     (w[(i)&15] = ADD(ADD(ADD(w[(i)&15], w[((i)-7) & 15]), SHA_s0r(w[((i)-15) & 15])), SHA_s1r(w[((i)-2) & 15])))
 
 // Fused kernel: the adds of an MD5 step on the FMA pipe; with kMd5Rot (bit 2 of B200H_FUSED_MIX in the dense fused
-// instantiation, else 0) the last one is fused with the rotate into one LEA.HI
+// instantiation, else 0) the last one is fused with the rotate into one LEA.HI; x + T is ADDK (VIADD with kConstAdd)
 #define MD5_STEP_FMA(FN, a, b, c, d, xk, s, T)                                    \
     {                                                                             \
-        const uint32_t t_ = ADD(ADD(a, ADD(xk, T)), FN(b, c, d));                 \
+        const uint32_t t_ = ADD(ADD(a, ADDK(xk, T)), FN(b, c, d));                \
         if (kMd5Rot) a = add_rotl<(s)>(b, t_);                                    \
         else a = ADD(b, rotl(t_, s));                                             \
     }
@@ -279,8 +292,9 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     // dense instantiations only: the sparse one leaves every add to ptxas, which fuses them itself
     constexpr int kShaRot = SPARSE ? 0 : (DO_MD5 ? (B200H_FUSED_MIX & 3) : (B200H_SHAONLY_ROT));
     constexpr bool kMd5Rot = DO_SHA && DO_MD5 && !SPARSE && (B200H_FUSED_MIX & 4);
+    constexpr bool kConstAdd = DO_SHA && DO_MD5 && !SPARSE && B200H_FUSED_CONST_ADD;
     const uint32_t m29 = one << 29, m22 = one << 22;  // 2^29, 2^22 as run-time values (bit 2 of kShaRot)
-    (void)m29; (void)m22; (void)kMd5Rot;
+    (void)m29; (void)m22; (void)kMd5Rot; (void)kConstAdd;
     if (DO_SHA) {
 #pragma unroll
         for (int i = 0; i < 16; ++i) w[i] = bswap(x[i]);

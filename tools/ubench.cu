@@ -15,12 +15,24 @@ __global__ void k(uint32_t* out, uint32_t one, uint32_t seed, long long* cyc) {
     uint32_t a[ACC];
 #pragma unroll
     for (int i = 0; i < ACC; ++i) a[i] = seed + threadIdx.x * 7 + i;
+    const uint32_t uone = one;  // stays warp-uniform: ptxas reads it from a uniform register (IMAD R, R, UR, R)
 #ifdef VEC
-    // per-thread operands: ptxas must keep them in vector registers (the hash kernel's operands all are)
-    uint32_t b = (seed ^ 0x9e3779b9u) + threadIdx.x * 0x01000193u, c = seed * 3 + 1 + (threadIdx.x << 7);
+    // per-thread operands: ptxas must keep them in vector registers (the hash kernel's operands all are).  Every
+    // accumulator has its own b and c, so consecutive instructions read distinct registers and the operand reuse cache
+    // cannot serve them, as in the hash kernel (555 of its 4 717 vector source operands per block carry .reuse).
+    uint32_t bv[ACC], cv[ACC];
+#pragma unroll
+    for (int i = 0; i < ACC; ++i) {
+        bv[i] = (seed ^ 0x9e3779b9u) + threadIdx.x * 0x01000193u + i * 0x3c6ef372u;
+        cv[i] = seed * 3 + 1 + (threadIdx.x << 7) + i * 0x7f4a7c15u;
+    }
+#define B(i) bv[i]
+#define C(i) cv[i]
     if (seed == 0x7fffffffu) one += threadIdx.x;  // never true at run time, but keeps `one` in a vector register
 #else
     uint32_t b = seed ^ 0x9e3779b9u, c = seed * 3 + 1;
+#define B(i) b
+#define C(i) c
 #endif
     uint32_t w[ACC];
     float fa[ACC], fb = __uint_as_float(0x3f800001u + (seed & 1)), fc = 1e-9f;
@@ -34,73 +46,100 @@ __global__ void k(uint32_t* out, uint32_t one, uint32_t seed, long long* cyc) {
     for (int it = 0; it < ITER; ++it) {
 #pragma unroll
         for (int i = 0; i < ACC; ++i) {
-            if (MODE == 0) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(b));                          // IADD
-            if (MODE == 1) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(b));         // IMAD R,R,R
-            if (MODE == 2) asm volatile("mad.lo.u32 %0, %0, 3, %1;" : "+r"(a[i]) : "r"(b));                    // IMAD R,imm,R
-            if (MODE == 3) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));       // LOP3
+            if (MODE == 0) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(B(i)));                          // IADD
+            if (MODE == 1) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(B(i)));         // IMAD R,R,R
+            if (MODE == 2) asm volatile("mad.lo.u32 %0, %0, 3, %1;" : "+r"(a[i]) : "r"(B(i)));                    // IMAD R,imm,R
+            if (MODE == 3) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));       // LOP3
             if (MODE == 4) asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));                         // SHF
-            if (MODE == 5) asm volatile("{ .reg .u32 t; add.u32 t, %0, %1; add.u32 %0, t, %2; }" : "+r"(a[i]) : "r"(b), "r"(c)); // IADD3
+            if (MODE == 5) asm volatile("{ .reg .u32 t; add.u32 t, %0, %1; add.u32 %0, t, %2; }" : "+r"(a[i]) : "r"(B(i)), "r"(C(i))); // IADD3
             if (MODE == 6) {  // alternate ALU (LOP3) and IMAD imm
-                if (i & 1) asm volatile("mad.lo.u32 %0, %0, 3, %1;" : "+r"(a[i]) : "r"(b));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (i & 1) asm volatile("mad.lo.u32 %0, %0, 3, %1;" : "+r"(a[i]) : "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 7) {  // alternate ALU (LOP3) and IMAD R,R,R
-                if (i & 1) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(b));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (i & 1) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 8) {  // alternate SHF and IADD (both ALU)
-                if (i & 1) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(b));
+                if (i & 1) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(B(i)));
                 else asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));
             }
-            if (MODE == 9) asm volatile("mad.lo.u32 %0, %0, 1, %1;" : "+r"(a[i]) : "r"(b));                    // what does ptxas do with *1
-            if (MODE == 10) asm volatile("mad.lo.u32 %0, %1, %0, %2;" : "+r"(a[i]) : "r"(one), "r"(b));
+            if (MODE == 9) asm volatile("mad.lo.u32 %0, %0, 1, %1;" : "+r"(a[i]) : "r"(B(i)));                    // what does ptxas do with *1
+            if (MODE == 10) asm volatile("mad.lo.u32 %0, %1, %0, %2;" : "+r"(a[i]) : "r"(one), "r"(B(i)));
             if (MODE == 11) {  // IMAD.WIDE R, R, imm, RZ: rotate by multiply (lo/hi halves kept live by one LOP3 per 4)
                 uint64_t d; asm volatile("mul.wide.u32 %0, %1, 0x4000000;" : "=l"(d) : "r"(a[i]));
                 a[i] = (uint32_t)d; w[i] = (uint32_t)(d >> 32);
             }
             if (MODE == 12) {  // alternate LOP3 and IMAD.WIDE
                 if (i & 1) { uint64_t d; asm volatile("mul.wide.u32 %0, %1, 0x4000000;" : "=l"(d) : "r"(a[i])); a[i] = (uint32_t)d; w[i] = (uint32_t)(d >> 32); }
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 13) {  // 2 ALU : 1 FMA
-                if (i % 3 == 2) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(b));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (i % 3 == 2) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 14) {  // 1 ALU : 2 FMA
-                if (i % 3 != 2) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(b));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (i % 3 != 2) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
-            if (MODE == 15) asm volatile("mul.hi.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(b));                     // IMAD.HI
+            if (MODE == 15) asm volatile("mul.hi.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(B(i)));                     // IMAD.HI
             if (MODE == 16) {  // the hash mix: 7 ALU (4 SHF + 3 LOP3) : 5 IMAD over 12 slots
                 const int j = i % 12;
-                if (j == 1 || j == 3 || j == 6 || j == 8 || j == 10) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(b));
-                else if (j & 1) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (j == 1 || j == 3 || j == 6 || j == 8 || j == 10) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one), "r"(B(i)));
+                else if (j & 1) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
                 else asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));
             }
             if (MODE == 17) {  // FFMA (fma heavy+lite) alternating with LOP3: is the cap an INT-FMA cap or a dispatch cap?
                 if (i & 1) asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(fa[i]) : "f"(fb), "f"(fc));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 19) {  // LOP3 + two-input add (ptxas: VIADD / IMAD.IADD)
-                if (i & 1) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(b));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (i & 1) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 20) {  // the hash mix with two-input adds instead of IMAD
                 const int j = i % 12;
-                if (j == 1 || j == 3 || j == 6 || j == 8 || j == 10) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(b));
-                else if (j & 1) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (j == 1 || j == 3 || j == 6 || j == 8 || j == 10) asm volatile("add.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(B(i)));
+                else if (j & 1) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
                 else asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));
             }
             if (MODE == 18) asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(fa[i]) : "f"(fb), "f"(fc));      // FFMA alone
             // acc + rotl(u, 26) on the FMA pipe: multiplier one << 26 (a run-time value), 32-bit accumulator b
-            if (MODE == 21) asm volatile("mad.hi.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one << 26), "r"(b));  // IMAD.HI R,UR,R
+            if (MODE == 21) asm volatile("mad.hi.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one << 26), "r"(B(i)));  // IMAD.HI R,UR,R
             if (MODE == 22) asm volatile("{ .reg .u32 t; mad.hi.u32 t, %0, %1, %2; mad.lo.u32 %0, %0, %1, t; }"
-                                         : "+r"(a[i]) : "r"(one << 26), "r"(b));                            // IMAD.HI + IMAD
+                                         : "+r"(a[i]) : "r"(one << 26), "r"(B(i)));                            // IMAD.HI + IMAD
             if (MODE == 23) {  // alternate LOP3 and IMAD.HI R,UR,R
-                if (i & 1) asm volatile("mad.hi.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one << 26), "r"(b));
-                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(b), "r"(c));
+                if (i & 1) asm volatile("mad.hi.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(one << 26), "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
             if (MODE == 24) asm volatile("mul.hi.u32 %0, %0, %1;" : "+r"(a[i]) : "r"(one << 26));               // IMAD.HI R,UR,RZ
+            // the fused lane kernel's add forms (B200H_UNIFORM_ONE): x * one + y with `one` in a vector or a uniform
+            // register, and x + constant as VIADD or as IMAD with the constant in the C slot
+            if (MODE == 25) {  // alternate LOP3 and IMAD R,R,UR,R
+                if (i & 1) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(uone), "r"(B(i)));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
+            }
+            if (MODE == 26) {  // alternate LOP3 and VIADD R,R,imm
+                if (i & 1) asm volatile("add.u32 %0, %0, 0x5a827999;" : "+r"(a[i]));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
+            }
+            if (MODE == 27) {  // alternate SHF and VIADD R,R,imm
+                if (i & 1) asm volatile("add.u32 %0, %0, 0x5a827999;" : "+r"(a[i]));
+                else asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));
+            }
+            if (MODE == 28) asm volatile("add.u32 %0, %0, 0x5a827999;" : "+r"(a[i]));                          // VIADD alone
+            if (MODE == 29 || MODE == 30 || MODE == 31) {  // the hash mix, 7 ALU : 5 adds, adds as IMAD R,R,UR,R
+                const int j = i % 12;
+                if (j == 10 && MODE == 30) asm volatile("add.u32 %0, %0, 0x5a827999;" : "+r"(a[i]));  // 1 in 5 a VIADD imm
+                else if (j == 10 && MODE == 31) asm volatile("mad.lo.u32 %0, %0, %1, 0x5a827999;" : "+r"(a[i]) : "r"(one));  // or an IMAD R,R,imm
+                else if (j == 1 || j == 3 || j == 6 || j == 8 || j == 10) asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(uone), "r"(B(i)));
+                else if (j & 1) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
+                else asm volatile("shf.r.wrap.b32 %0, %0, %0, 7;" : "+r"(a[i]));
+            }
+            if (MODE == 32) {  // alternate LOP3 and IMAD R,R,imm (one vector-register multiplier, constant addend)
+                if (i & 1) asm volatile("mad.lo.u32 %0, %0, %1, 0x5a827999;" : "+r"(a[i]) : "r"(one));
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
+            }
         }
     }
     long long t1 = clock64();
@@ -168,6 +207,14 @@ int main() {
     for (int w : {1, 4, 5, 8}) {
         run<21>("IMAD.HI R,UR,R (acc)", w); run<24>("IMAD.HI R,UR,RZ", w); run<22>("IMAD.HI + IMAD pair", w);
         run<23>("LOP3 + IMAD.HI alt", w); run<1>("IMAD R,R,R(one),R", w); run<7>("LOP3 + IMAD RRR alt", w);
+    }
+    // the fused lane kernel's add forms (modes 25-32); it runs 5 warps per SMSP
+    for (int w : {4, 5, 8}) {
+        run<3>("LOP3", w); run<4>("SHF.W", w); run<28>("VIADD imm", w);
+        run<7>("LOP3 + IMAD R,R,R alt", w); run<25>("LOP3 + IMAD R,R,UR,R alt", w); run<32>("LOP3 + IMAD R,R,imm alt", w);
+        run<26>("LOP3 + VIADD imm alt", w); run<27>("SHF + VIADD imm alt", w);
+        run<16>("mix 7:5 IMAD R,R,R", w); run<29>("mix 7:5 IMAD R,R,UR", w); run<30>("mix 7:5 UR, 1/5 VIADD", w);
+        run<31>("mix 7:5 UR, 1/5 IMAD imm", w);
     }
     return 0;
 }
