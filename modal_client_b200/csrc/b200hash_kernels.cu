@@ -437,9 +437,11 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
 
 // ------------------------------------------------------------------------------ lane_hash_kernel
 
-// CTAs per SM the lane kernel is compiled for.  H100 (100 000 x 256 KiB, kernel time): fused SHA-256 + MD5 at 5 CTAs
-// (96 registers, a few bytes of spill) beats 4 CTAs (128 registers, no spill) by 2-3 %; MD5 alone is the same either
-// way; SHA-256 alone gains 5 % at 4 CTAs, so that instantiation gets its own bound.
+// CTAs per SM the lane kernel is compiled for.  H100 (100 000 x 256 KiB, kernel time): SHA-256 alone gains 5 % at 4 CTAs
+// (128 registers) over 5 (96).  The fused SHA-256 + MD5 kernel as it now stands (LEA.HI rotate+adds, uniform `one`)
+// runs 7 % faster at 4 CTAs, where it needs no spill, than at 5 (96 registers, 88 bytes of spill): 36.14 -> 33.70 ms on
+// an H100 80GB HBM3 at a 700 W power limit (DESIGN.md 6).  So every instantiation that computes SHA-256 gets
+// B200H_LANE_MIN_CTAS_SHA; MD5 alone, at 96 registers either way, keeps 5.
 #ifndef B200H_LANE_MIN_CTAS
 #define B200H_LANE_MIN_CTAS 5
 #endif
@@ -492,7 +494,7 @@ __device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
 // bound by its own issue rate (one instruction per two cycles), so the adds are left to ptxas (IADD3 / LEA fusion,
 // ~15 % fewer instructions per block) instead of being spread over the FMA pipe.
 template <bool DO_SHA, bool DO_MD5, bool SPARSE>
-__global__ void __launch_bounds__(kLaneThreads, (DO_SHA && !DO_MD5) ? B200H_LANE_MIN_CTAS_SHA : B200H_LANE_MIN_CTAS)
+__global__ void __launch_bounds__(kLaneThreads, DO_SHA ? B200H_LANE_MIN_CTAS_SHA : B200H_LANE_MIN_CTAS)
 lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ off, const uint64_t* __restrict__ len,
                  uint32_t* __restrict__ ring, uint32_t ring_mask, int* __restrict__ qctl, const int* __restrict__ ctl,
                  uint32_t flags, int lanes_per_warp, uint32_t quantum, uint8_t* __restrict__ sha_out,
@@ -697,9 +699,16 @@ lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ 
                     const uint32_t pieces = (rem < (uint32_t)kBPC ? rem : (uint32_t)kBPC) * 4u + (mis ? 1u : 0u);
                     const uint32_t dst = smem_u32(ring_smem + ((c % kStages) * 32 + lane) * kSlot);
                     const uint8_t* g = src + c * (kBPC * 64);
+                    if (pieces == kBPC * 4) {
+                        // a full, aligned chunk (every chunk of an aligned message but its last): 8 copies at immediate
+                        // offsets from one address pair instead of a predicated address pair per piece
 #pragma unroll
-                    for (uint32_t k = 0; k < kBPC * 4 + 1; ++k)
-                        if (k < pieces) cp_async16(dst + 16 * k, g + 16 * k);
+                        for (uint32_t k = 0; k < kBPC * 4; ++k) cp_async16(dst + 16 * k, g + 16 * k);
+                    } else {
+#pragma unroll
+                        for (uint32_t k = 0; k < kBPC * 4 + 1; ++k)
+                            if (k < pieces) cp_async16(dst + 16 * k, g + 16 * k);
+                    }
                 }
                 cp_async_commit();
             }
@@ -1744,7 +1753,7 @@ int launch_trim(const uint8_t* base, const uint64_t* off, const uint64_t* len, u
 }
 
 
-static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS, B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS};  // [sha+md5, sha, md5]
+static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS};  // [sha+md5, sha, md5]
 
 // most long messages a second, lane-packed launch takes: one wave of lanes at one warp per SMSP
 uint32_t plan_long_cap() {
