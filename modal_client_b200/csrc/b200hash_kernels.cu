@@ -87,6 +87,34 @@ __device__ __forceinline__ uint32_t add_rotl(uint32_t acc, uint32_t u) {
 __device__ __forceinline__ uint32_t rotr(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
 __device__ __forceinline__ uint32_t rotl(uint32_t x, int n) { return __funnelshift_l(x, x, n); }
 __device__ __forceinline__ uint32_t bswap(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
+// rotr by a compile-time amount; no instruction for 0
+template <int N>
+__device__ __forceinline__ uint32_t rotr_c(uint32_t x) {
+    return N == 0 ? x : rotr(x, N);
+}
+
+// lop3 over (a, b, c) with the operands passed in the order PERM names -- 0 (a, b, c), 1 (a, c, b), 2 (b, a, c),
+// 3 (b, c, a), 4 (c, a, b), 5 (c, b, a) -- and the truth table permuted to match, so the result is the same.
+__host__ __device__ constexpr int lop3_src(int perm, int k) {  // which of a (0), b (1), c (2) goes to operand slot k
+    return (perm == 0 ? 0x210 : perm == 1 ? 0x120 : perm == 2 ? 0x201 : perm == 3 ? 0x021 : perm == 4 ? 0x102 : 0x012) >>
+               (4 * k) & 15;
+}
+__host__ __device__ constexpr int lop3_lut(int imm, int perm) {
+    int lut = 0;
+    for (int j = 0; j < 8; ++j) {  // j: the slot values, slot 0 in bit 2 (the 0xF0 operand)
+        int i = 0;
+        for (int k = 0; k < 3; ++k) i |= ((j >> (2 - k)) & 1) << (2 - lop3_src(perm, k));
+        lut |= ((imm >> i) & 1) << j;
+    }
+    return lut;
+}
+template <int IMM, int PERM>
+__device__ __forceinline__ uint32_t lop3p(uint32_t a, uint32_t b, uint32_t c) {
+    constexpr int s0 = lop3_src(PERM, 0), s1 = lop3_src(PERM, 1), s2 = lop3_src(PERM, 2);
+    const uint32_t v[3] = {a, b, c};
+    return lop3<lop3_lut(IMM, PERM)>(v[s0], v[s1], v[s2]);
+}
+static_assert(lop3_lut(0xCA, 0) == 0xCA && lop3_lut(0x96, 5) == 0x96 && lop3_lut(0xCA, 2) == 0xE2, "lop3 permutation");
 
 // ---------------------------------------------------------------------- compression functions
 // SHA-256: FIPS 180-4 section 6.2.2; MD5: RFC 1321 section 3.4.  Boolean functions are single LOP3s:
@@ -157,6 +185,40 @@ __device__ __forceinline__ uint32_t addv(uint32_t a, uint32_t b) {
 #ifndef B200H_FUSED_CONST_ADD
 #define B200H_FUSED_CONST_ADD 1
 #endif
+// Equivalent forms of the dense fused body.  Each gives the same digests and the same ALU-pipe instructions; they
+// change which registers the instructions read and how ptxas schedules and allocates them (DESIGN.md 5.1):
+//   B200H_FUSED_S1_OUT (6, 11 or 25) / B200H_FUSED_S0_OUT (2, 13 or 22): the rotate of Sigma1 / Sigma0 that is taken
+//       outside the xor3 and fused with its add into LEA.HI, e.g. Sigma1 = rotr6(e ^ rotr5 e ^ rotr19 e) =
+//       rotr11(rotr27 e ^ e ^ rotr14 e) = rotr25(rotr13 e ^ rotr18 e ^ e);
+//   B200H_FUSED_LOP_SHA / B200H_FUSED_LOP_MD5 (0..5): the operand order of every LOP3 of SHA-256 (Ch, Maj, the Sigma
+//       and sigma xor3s) / MD5 (F, G, H, I), with its truth table permuted to match (lop3p);
+//   B200H_FUSED_SCHED (1, 4 or 8): message schedule words expanded ahead of the rounds that use them (4: the four of
+//       each quad of rounds, 8: the next eight every second quad, 1: each word just before its round);
+//   B200H_FUSED_MD5_FIRST (with B200H_ILV 4): 1 = each quad's four MD5 steps ahead of its four SHA-256 rounds in
+//       source order (what B200H_ILV=40 does for every instantiation), 0 = after them.
+// The defaults (LOP3 order 3 = (b, c, a), MD5 first, 3 CTAs per SM in B200H_LANE_MIN_CTAS_FUSED) were picked from
+// measured builds: 3.1 % less lane-kernel time than the forms before (tools/lane_sass_score.py, DESIGN.md 5.1, 6).
+#ifndef B200H_FUSED_S1_OUT
+#define B200H_FUSED_S1_OUT 6
+#endif
+#ifndef B200H_FUSED_S0_OUT
+#define B200H_FUSED_S0_OUT 2
+#endif
+#ifndef B200H_FUSED_LOP_SHA
+#define B200H_FUSED_LOP_SHA 3
+#endif
+#ifndef B200H_FUSED_LOP_MD5
+#define B200H_FUSED_LOP_MD5 0
+#endif
+#ifndef B200H_FUSED_SCHED
+#define B200H_FUSED_SCHED 4
+#endif
+#ifndef B200H_FUSED_MD5_FIRST
+#define B200H_FUSED_MD5_FIRST 1
+#endif
+static_assert(B200H_FUSED_S1_OUT == 6 || B200H_FUSED_S1_OUT == 11 || B200H_FUSED_S1_OUT == 25, "B200H_FUSED_S1_OUT");
+static_assert(B200H_FUSED_S0_OUT == 2 || B200H_FUSED_S0_OUT == 13 || B200H_FUSED_S0_OUT == 22, "B200H_FUSED_S0_OUT");
+static_assert(B200H_FUSED_SCHED == 1 || B200H_FUSED_SCHED == 4 || B200H_FUSED_SCHED == 8, "B200H_FUSED_SCHED");
 // x + a round constant; kConstAdd (a constant inside compress<>) is B200H_FUSED_CONST_ADD in the dense fused
 // instantiation, else 0
 #define ADDK(x, k) (kConstAdd ? ((x) + (k)) : ADD((x), (k)))
@@ -171,14 +233,17 @@ __device__ __forceinline__ uint32_t mulhi(uint32_t x, uint32_t m) {
     asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(m));
     return d;
 }
-// FUSED: the Sigma rotates through add_rotl (B200H_FUSED_MIX) instead of rotw (B200H_SHAONLY_ROT)
-template <int ROT, bool FUSED>
+// FUSED: the Sigma rotates through add_rotl (B200H_FUSED_MIX) instead of rotw (B200H_SHAONLY_ROT), outer rotates
+// B200H_FUSED_S1_OUT / B200H_FUSED_S0_OUT, LOP3 operand order LOP (0 unless FUSED)
+template <int ROT, bool FUSED, int LOP>
 __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, uint32_t& d, uint32_t e, uint32_t f,
                                             uint32_t g, uint32_t& h, uint32_t K, uint32_t W, uint32_t one) {
+    constexpr int R1 = B200H_FUSED_S1_OUT, R0 = B200H_FUSED_S0_OUT;
     const uint32_t kw = (FUSED && B200H_FUSED_CONST_ADD) ? W + K : addf(W, K, one);
-    uint32_t t1 = addf(addf(h, kw, one), lop3<0xCA>(e, f, g), one);
+    uint32_t t1 = addf(addf(h, kw, one), lop3p<0xCA, LOP>(e, f, g), one);
     if ((ROT & 1) && FUSED) {
-        t1 = add_rotl<26>(t1, lop3<0x96>(e, rotr(e, 5), rotr(e, 19)));
+        t1 = add_rotl<32 - R1>(t1, lop3p<0x96, LOP>(rotr_c<(38 - R1) % 32>(e), rotr_c<(43 - R1) % 32>(e),
+                                                    rotr_c<(57 - R1) % 32>(e)));
     } else if (ROT & 1) {
         uint32_t lo, hi;
         rotw(lop3<0x96>(e, rotr(e, 5), rotr(e, 19)), 1u << 26, lo, hi);
@@ -188,7 +253,9 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
     }
     uint32_t t2;
     if ((ROT & 2) && FUSED) {
-        t2 = add_rotl<30>(lop3<0xE8>(a, b, c), lop3<0x96>(a, rotr(a, 11), rotr(a, 20)));
+        t2 = add_rotl<32 - R0>(lop3p<0xE8, LOP>(a, b, c), lop3p<0x96, LOP>(rotr_c<(34 - R0) % 32>(a),
+                                                                             rotr_c<(45 - R0) % 32>(a),
+                                                                             rotr_c<(54 - R0) % 32>(a)));
     } else if (ROT & 2) {
         uint32_t lo, hi;
         rotw(lop3<0x96>(a, rotr(a, 11), rotr(a, 20)), 1u << 30, lo, hi);
@@ -224,16 +291,16 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
     }
 #endif
 // kShaRot (a constant inside compress<>) is B200H_SHAONLY_ROT for the dense SHA-only instantiation, bits 0 and 1 of
-// B200H_FUSED_MIX for the dense fused one, else 0
-#define SHA_RND(a, b, c, d, e, f, g, h, K, W)                                           \
-    {                                                                                   \
-        if (kShaRot & 3) sha_rnd_rot<kShaRot, DO_MD5>(a, b, c, d, e, f, g, h, K, W, one); \
-        else SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                 \
+// B200H_FUSED_MIX for the dense fused one, else 0; kLopSha is B200H_FUSED_LOP_SHA in the dense fused one, else 0
+#define SHA_RND(a, b, c, d, e, f, g, h, K, W)                                                       \
+    {                                                                                               \
+        if (kShaRot & 3) sha_rnd_rot<kShaRot, DO_MD5, kLopSha>(a, b, c, d, e, f, g, h, K, W, one); \
+        else SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                             \
     }
 #define SHA_SHR3(x) ((kShaRot & 4) ? mulhi((x), m29) : ((x) >> 3))
 #define SHA_SHR10(x) ((kShaRot & 4) ? mulhi((x), m22) : ((x) >> 10))
-#define SHA_s0r(x) lop3<0x96>(rotr(x, 7), rotr(x, 18), SHA_SHR3(x))
-#define SHA_s1r(x) lop3<0x96>(rotr(x, 17), rotr(x, 19), SHA_SHR10(x))
+#define SHA_s0r(x) lop3p<0x96, kLopSha>(rotr(x, 7), rotr(x, 18), SHA_SHR3(x))
+#define SHA_s1r(x) lop3p<0x96, kLopSha>(rotr(x, 17), rotr(x, 19), SHA_SHR10(x))
 // message schedule in place: w[i&15] becomes W[i] for i >= 16
 #define SHA_SCHED(w, i) \
     (w[(i)&15] = ADD(ADD(ADD(w[(i)&15], w[((i)-7) & 15]), SHA_s0r(w[((i)-15) & 15])), SHA_s1r(w[((i)-2) & 15])))
@@ -255,10 +322,10 @@ __device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, 
     }
 #define MD5_STEP(FN, a, b, c, d, xk, s, T)                 \
     if (DO_SHA) MD5_STEP_FMA(FN, a, b, c, d, xk, s, T) else MD5_STEP_MIX(FN, a, b, c, d, xk, s, T)
-#define MD5_F(b, c, d) lop3<0xCA>(b, c, d)
-#define MD5_G(b, c, d) lop3<0xE4>(b, c, d)
-#define MD5_H(b, c, d) lop3<0x96>(b, c, d)
-#define MD5_I(b, c, d) lop3<0x39>(b, c, d)
+#define MD5_F(b, c, d) lop3p<0xCA, kLopMd5>(b, c, d)
+#define MD5_G(b, c, d) lop3p<0xE4, kLopMd5>(b, c, d)
+#define MD5_H(b, c, d) lop3p<0x96, kLopMd5>(b, c, d)
+#define MD5_I(b, c, d) lop3p<0x39, kLopMd5>(b, c, d)
 
 #ifndef B200H_ROLLED
 #define B200H_ROLLED 0
@@ -293,6 +360,9 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     constexpr int kShaRot = SPARSE ? 0 : (DO_MD5 ? (B200H_FUSED_MIX & 3) : (B200H_SHAONLY_ROT));
     constexpr bool kMd5Rot = DO_SHA && DO_MD5 && !SPARSE && (B200H_FUSED_MIX & 4);
     constexpr bool kConstAdd = DO_SHA && DO_MD5 && !SPARSE && B200H_FUSED_CONST_ADD;
+    constexpr bool kFusedForm = DO_SHA && DO_MD5 && !SPARSE;  // the B200H_FUSED_* body forms apply
+    constexpr int kLopSha = kFusedForm ? B200H_FUSED_LOP_SHA : 0, kLopMd5 = kFusedForm ? B200H_FUSED_LOP_MD5 : 0;
+    constexpr int kSchedAhead = kFusedForm ? B200H_FUSED_SCHED : 4;
     const uint32_t m29 = one << 29, m22 = one << 22;  // 2^29, 2^22 as run-time values (bit 2 of kShaRot)
     (void)m29; (void)m22; (void)kMd5Rot; (void)kConstAdd;
     if (DO_SHA) {
@@ -310,25 +380,35 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     uint32_t a = hs[0], b = hs[1], c = hs[2], d = hs[3], e = hs[4], f = hs[5], g = hs[6], h = hs[7];
     uint32_t A = hm[0], B = hm[1], C = hm[2], D = hm[3];
 
-#define SHA4(i, k0, k1, k2, k3)                                 \
-    if (DO_SHA) {                                               \
-        if ((i) >= 16) {                                        \
-            SHA_SCHED(w, (i));                                  \
-            SHA_SCHED(w, (i) + 1);                              \
-            SHA_SCHED(w, (i) + 2);                              \
-            SHA_SCHED(w, (i) + 3);                              \
-        }                                                       \
-        if (((i)&7) == 0) {                                     \
-            SHA_RND(a, b, c, d, e, f, g, h, k0, w[(i)&15]);    \
-            SHA_RND(h, a, b, c, d, e, f, g, k1, w[((i) + 1) & 15]); \
-            SHA_RND(g, h, a, b, c, d, e, f, k2, w[((i) + 2) & 15]); \
-            SHA_RND(f, g, h, a, b, c, d, e, k3, w[((i) + 3) & 15]); \
-        } else {                                                \
-            SHA_RND(e, f, g, h, a, b, c, d, k0, w[(i)&15]);    \
-            SHA_RND(d, e, f, g, h, a, b, c, k1, w[((i) + 1) & 15]); \
-            SHA_RND(c, d, e, f, g, h, a, b, k2, w[((i) + 2) & 15]); \
-            SHA_RND(b, c, d, e, f, g, h, a, k3, w[((i) + 3) & 15]); \
-        }                                                       \
+    // kSchedAhead (B200H_FUSED_SCHED): W[i] is expanded in the quad's preamble (4), eight at a time (8) or in SCHED1
+    // just before its round (1)
+#define SCHED1(i) \
+    if (kSchedAhead == 1 && (i) >= 16) SHA_SCHED(w, (i));
+#define SHA4(i, k0, k1, k2, k3)                                                 \
+    if (DO_SHA) {                                                               \
+        if ((i) >= 16 && (kSchedAhead == 4 || (kSchedAhead == 8 && ((i)&7) == 0))) { \
+            SHA_SCHED(w, (i));                                                  \
+            SHA_SCHED(w, (i) + 1);                                              \
+            SHA_SCHED(w, (i) + 2);                                              \
+            SHA_SCHED(w, (i) + 3);                                              \
+        }                                                                       \
+        if ((i) >= 16 && kSchedAhead == 8 && ((i)&7) == 0) {                    \
+            SHA_SCHED(w, (i) + 4);                                              \
+            SHA_SCHED(w, (i) + 5);                                              \
+            SHA_SCHED(w, (i) + 6);                                              \
+            SHA_SCHED(w, (i) + 7);                                              \
+        }                                                                       \
+        if (((i)&7) == 0) {                                                     \
+            SCHED1(i) SHA_RND(a, b, c, d, e, f, g, h, k0, w[(i)&15]);           \
+            SCHED1((i) + 1) SHA_RND(h, a, b, c, d, e, f, g, k1, w[((i) + 1) & 15]); \
+            SCHED1((i) + 2) SHA_RND(g, h, a, b, c, d, e, f, k2, w[((i) + 2) & 15]); \
+            SCHED1((i) + 3) SHA_RND(f, g, h, a, b, c, d, e, k3, w[((i) + 3) & 15]); \
+        } else {                                                                \
+            SCHED1(i) SHA_RND(e, f, g, h, a, b, c, d, k0, w[(i)&15]);           \
+            SCHED1((i) + 1) SHA_RND(d, e, f, g, h, a, b, c, k1, w[((i) + 1) & 15]); \
+            SCHED1((i) + 2) SHA_RND(c, d, e, f, g, h, a, b, k2, w[((i) + 2) & 15]); \
+            SCHED1((i) + 3) SHA_RND(b, c, d, e, f, g, h, a, k3, w[((i) + 3) & 15]); \
+        }                                                                       \
     }
 #define MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
     if (DO_MD5) {                                               \
@@ -359,8 +439,12 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
         else MD5_STEP(FN, B, C, D, A, xk, s, T)               \
     }
 #if B200H_ILV == 4
-#define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
-    SHA4(i, k0, k1, k2, k3) MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3)
+#define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3)      \
+    if (kFusedForm && B200H_FUSED_MD5_FIRST) {                                         \
+        MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) SHA4(i, k0, k1, k2, k3) \
+    } else {                                                                           \
+        SHA4(i, k0, k1, k2, k3) MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
+    }
 #elif B200H_ILV == 40  // MD5 steps ahead of the SHA rounds of the same quad
 #define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
     MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) SHA4(i, k0, k1, k2, k3)
@@ -420,6 +504,7 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     QUAD(56, 0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u, MD5_I, x[8], m15, x[6], x[13], 6, 10, 15, 21, 0x6fa87e4fu, 0xfe2ce6e0u, 0xa3014314u, 0x4e0811a1u)
     QUAD(60, 0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u, MD5_I, x[4], x[11], x[2], x[9], 6, 10, 15, 21, 0xf7537e82u, 0xbd3af235u, 0x2ad7d2bbu, 0xeb86d391u)
 #endif
+#undef SCHED1
 #undef SHA4
 #undef MD4
 #undef SHA1
@@ -440,13 +525,20 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
 // CTAs per SM the lane kernel is compiled for.  H100 (100 000 x 256 KiB, kernel time): SHA-256 alone gains 5 % at 4 CTAs
 // (128 registers) over 5 (96).  The fused SHA-256 + MD5 kernel as it now stands (LEA.HI rotate+adds, uniform `one`)
 // runs 7 % faster at 4 CTAs, where it needs no spill, than at 5 (96 registers, 88 bytes of spill): 36.14 -> 33.70 ms on
-// an H100 80GB HBM3 at a 700 W power limit (DESIGN.md 6).  So every instantiation that computes SHA-256 gets
-// B200H_LANE_MIN_CTAS_SHA; MD5 alone, at 96 registers either way, keeps 5.
+// an H100 80GB HBM3 at a 700 W power limit (DESIGN.md 6).  So the instantiations that compute SHA-256 get
+// B200H_LANE_MIN_CTAS_SHA, except the dense fused one, which has gone on to 3 (B200H_LANE_MIN_CTAS_FUSED below); MD5
+// alone, at 96 registers either way, keeps 5.
 #ifndef B200H_LANE_MIN_CTAS
 #define B200H_LANE_MIN_CTAS 5
 #endif
 #ifndef B200H_LANE_MIN_CTAS_SHA
 #define B200H_LANE_MIN_CTAS_SHA 4
+#endif
+// The dense fused instantiation on its own: at 3 CTAs (up to 168 registers; ptxas takes 158) its body reads fewer
+// vector registers and it ran 2.2 % faster than at 4 (128 registers) on an H100 at 700 W, and 3.1 % faster with the
+// B200H_FUSED_* defaults (DESIGN.md 6).  The SHA-256-only and sparse ones stay at B200H_LANE_MIN_CTAS_SHA.
+#ifndef B200H_LANE_MIN_CTAS_FUSED
+#define B200H_LANE_MIN_CTAS_FUSED 3
 #endif
 constexpr int kLaneThreads = 128;  // 4 warps; every warp runs an independent TMA/mbarrier ring
 constexpr int kLaneWarps = kLaneThreads / 32;
@@ -494,7 +586,8 @@ __device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
 // bound by its own issue rate (one instruction per two cycles), so the adds are left to ptxas (IADD3 / LEA fusion,
 // ~15 % fewer instructions per block) instead of being spread over the FMA pipe.
 template <bool DO_SHA, bool DO_MD5, bool SPARSE>
-__global__ void __launch_bounds__(kLaneThreads, DO_SHA ? B200H_LANE_MIN_CTAS_SHA : B200H_LANE_MIN_CTAS)
+__global__ void __launch_bounds__(kLaneThreads, DO_SHA ? (DO_MD5 && !SPARSE ? B200H_LANE_MIN_CTAS_FUSED : B200H_LANE_MIN_CTAS_SHA)
+                                                        : B200H_LANE_MIN_CTAS)
 lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ off, const uint64_t* __restrict__ len,
                  uint32_t* __restrict__ ring, uint32_t ring_mask, int* __restrict__ qctl, const int* __restrict__ ctl,
                  uint32_t flags, int lanes_per_warp, uint32_t quantum, uint8_t* __restrict__ sha_out,
@@ -1753,7 +1846,8 @@ int launch_trim(const uint8_t* base, const uint64_t* off, const uint64_t* len, u
 }
 
 
-static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS};  // [sha+md5, sha, md5]
+// [sha+md5, sha, md5]; configure_kernels() replaces them with the occupancy the compiled kernels reach
+static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS_FUSED, B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS};
 
 // most long messages a second, lane-packed launch takes: one wave of lanes at one warp per SMSP
 uint32_t plan_long_cap() {

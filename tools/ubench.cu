@@ -140,6 +140,24 @@ __global__ void k(uint32_t* out, uint32_t one, uint32_t seed, long long* cyc) {
                 if (i & 1) asm volatile("mad.lo.u32 %0, %0, %1, 0x5a827999;" : "+r"(a[i]) : "r"(one));
                 else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
             }
+            // the read costs tools/lane_sass_score.py assumes (modes 33-37, 40); mode 4 is SHF.W with hi == lo.  Register banks
+            // cannot be set from PTX: ptxas allocates (and splits 64-bit pairs) freely, so no mode pins a LOP3's sources to one bank
+            if (MODE == 33) asm volatile("shf.r.wrap.b32 %0, %0, %1, 7;" : "+r"(a[i]) : "r"(B(i)));            // SHF.W lo != hi
+            // acc + rotl: ptxas fuses a plain add of a funnel shift into LEA.HI d, lo, acc, hi (as add_rotl does)
+            if (MODE == 34) a[i] = B(i) + __funnelshift_l(a[i], a[i], 5);                                     // LEA.HI (u, u)
+            if (MODE == 35) a[i] = B(i) + __funnelshift_l(C(i), a[i], 5);                                     // LEA.HI (u, v)
+            if (MODE == 36) {  // alternate LOP3 and LEA.HI (u, u): at most 0.5 if LEA.HI is on the ALU pipe
+                if (i & 1) a[i] = B(i) + __funnelshift_l(a[i], a[i], 5);
+                else asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
+            }
+            if (MODE == 37) {  // alternate IMAD R,R,UR,R and LEA.HI (u, u)
+                if (i & 1) a[i] = B(i) + __funnelshift_l(a[i], a[i], 5);
+                else asm volatile("mad.lo.u32 %0, %0, %1, %2;" : "+r"(a[i]) : "r"(uone), "r"(B(i)));
+            }
+            if (MODE == 40) {  // LOP3 alone, 8 per accumulator and loop trip: the loop's own instructions count 8x less
+#pragma unroll
+                for (int r = 0; r < 8; ++r) asm volatile("lop3.b32 %0, %0, %1, %2, 0x96;" : "+r"(a[i]) : "r"(B(i)), "r"(C(i)));
+            }
         }
     }
     long long t1 = clock64();
@@ -172,13 +190,26 @@ void run(const char* name, int warps_per_smsp) {
     cudaMemcpy(&c, cyc, 8, cudaMemcpyDeviceToHost);
     float ms;
     cudaEventElapsedTime(&ms, e0, e1);
-    double inst = (double)ITER * ACC * warps_per_smsp * (MODE == 22 ? 2 : 1);  // warp-instructions per SMSP
+    double inst = (double)ITER * ACC * warps_per_smsp * (MODE == 22 ? 2 : MODE == 40 ? 8 : 1);  // warp-instructions per SMSP
     printf("%-28s warps/SMSP=%d  cycles=%lld  IPC/SMSP=%.3f  (%.3f ms)\n", name, warps_per_smsp, c, inst / c, ms);
     cudaFree(out);
     cudaFree(cyc);
 }
 
-int main() {
+static void read_modes() {
+    // the read costs of the fused lane kernel's body (modes 33-37, 40); it runs 4 warps per SMSP, 3 at 3 CTAs per SM
+    for (int w : {3, 4}) {
+        run<4>("SHF.W hi == lo", w); run<33>("SHF.W hi != lo", w);
+        run<34>("LEA.HI (u, u)", w); run<35>("LEA.HI (u, v)", w);
+        run<36>("LOP3 + LEA.HI alt", w); run<37>("IMAD R,R,UR,R + LEA.HI alt", w);
+        run<3>("LOP3", w); run<40>("LOP3 x8 per loop trip", w);
+    }
+}
+
+int main(int argc, char** argv) {
+    (void)argv;
+    read_modes();
+    if (argc > 1) return 0;  // `ubench reads`: only the read-cost modes
     // one warp per SMSP: what a single instruction stream with plenty of ILP can issue
     run<0>("IADD R,R,R", 1); run<1>("IMAD R,R,R(one),R", 1); run<3>("LOP3", 1); run<4>("SHF.W", 1);
     run<6>("LOP3 + IMAD imm alt", 1); run<8>("SHF + IADD alt", 1);
