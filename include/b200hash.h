@@ -183,6 +183,33 @@ int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, u
  * (torch/serialization.py _save -> PyTorchStreamWriter::writeRecord), for a checkpoint that lives in HBM. */
 int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, uint32_t* d_crc_out, void* cuda_stream);
 
+/* len bytes at offset `offset` of file `file` of a segmented batch. */
+typedef struct b200h_file_range {
+    uint64_t file, offset, len;
+} b200h_file_range;
+
+/* Copy byte ranges of files that live in device memory as many buffers into page-locked HOST memory: range i lands at
+ * h_dst + dst_offsets[i].  The files are described exactly as for b200h_hash_segment_parts_device (segs,
+ * file_first_seg: host arrays, file-major).  A range may lie inside one segment or cross any number of them, empty
+ * ones included; len == 0 copies nothing.  `ranges` and `dst_offsets` are host arrays.
+ * h_dst is what b200h_host_alloc returns (16-byte aligned).  The caller owns its layout: every dst_offsets[i] must be a
+ * multiple of 16 and the destinations must lie inside h_dst_bytes without overlapping; no packing rule is imposed.
+ * Every argument is checked before any work is enqueued, B200H_E_INVALID otherwise: the rules of the segment-parts
+ * entry for segs / file_first_seg (every non-empty segment's first and last byte device memory on ctx's device),
+ * file < nfiles, offset + len within the file, h_dst page-locked host memory the context's device can reach
+ * (cudaPointerGetAttributes), destination offsets aligned, in bounds and disjoint.
+ * ONE kernel launch (stage_ranges_kernel) per call whatever the number of ranges and segments, none when every range
+ * is empty.  The kernel stores straight into h_dst, and every store is a full aligned 16-byte word whatever the phase
+ * of the source bytes, except the bytes behind a range's last whole word; bytes of h_dst outside the destinations are
+ * not written.  The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream): its tables live in a
+ * stream-ordered allocation as b200h_crc32_device's do, so it never synchronises; h_dst holds the bytes once the work
+ * enqueued on the stream has completed (cudaStreamSynchronize, or an event recorded after the call).
+ * Replaces: the per-chunk reads of _put_missing_blocks (py/modal/volume.py:1500-1574) for a file that lives in HBM,
+ * which the reference would have in host memory already. */
+int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                              uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* h_dst,
+                              uint64_t h_dst_bytes, const uint64_t* dst_offsets, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

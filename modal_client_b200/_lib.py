@@ -34,7 +34,7 @@ ABI_SYMBOLS = (
     "b200h_last_outlier_count", "b200h_hash_batch_device_hl", "b200h_combine_stats", "b200h_plan_sync_count",
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
-    "b200h_crc32_device",
+    "b200h_crc32_device", "b200h_copy_ranges_to_host",
 )
 
 
@@ -43,7 +43,8 @@ class B200HashError(RuntimeError):
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    srcs = [os.path.join(CSRC, f) for f in ("b200hash_kernels.cu", "b200hash_dedupe.cu", "b200hash_crc32.cu", "b200hash_api.cu",
+    srcs = [os.path.join(CSRC, f) for f in ("b200hash_kernels.cu", "b200hash_dedupe.cu", "b200hash_crc32.cu", "b200hash_stage.cu",
+                                            "b200hash_api.cu",
                                             "b200blob_host.cpp", "b200pack_copy.cpp", "b200hash_kernels.cuh", "b200pack_team.h")]
     srcs += [os.path.join(os.path.dirname(_PKG), "include", h) for h in ("b200hash.h", "b200blob.h")]
     stale = not os.path.exists(LIB_PATH) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
@@ -109,6 +110,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_segment_parts_preview.restype = i32
         L.b200h_crc32_device.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_crc32_device.restype = i32
+        L.b200h_copy_ranges_to_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
+        L.b200h_copy_ranges_to_host.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -429,6 +432,23 @@ class Context:
         rc = self._L.b200h_crc32_device(self._h, _np_ptr(ranges) if len(ranges) else None, len(ranges), d_out or None,
                                         stream or None)
         self._check(rc, "b200h_crc32_device")
+
+    def copy_ranges_to_host(self, seg_ptrs, seg_lens, file_first_seg, ranges, dst: np.ndarray, dst_offsets,
+                            stream: int = 0) -> None:
+        """Copy byte ranges of files made of device buffers (described as for ``hash_segment_parts_device``) into
+        ``dst``, a uint8 array over page-locked memory from ``host_alloc``: range i = ``(file, offset, len)`` lands at
+        ``dst[dst_offsets[i]:]`` (offsets multiples of 16, destinations disjoint).  One kernel launch, only enqueued on
+        ``stream``: ``dst`` holds the bytes once that stream's work has completed."""
+        segs = _segments(seg_ptrs, seg_lens)
+        ffs, nfiles = _segment_args(file_first_seg)
+        rg = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 3)
+        offs = np.ascontiguousarray(dst_offsets, dtype=np.uint64)
+        if offs.shape != (len(rg),):
+            raise ValueError("dst_offsets needs one entry per range")
+        rc = self._L.b200h_copy_ranges_to_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs), nfiles,
+                                               _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(dst.ctypes.data),
+                                               dst.size, _np_ptr(offs) if len(rg) else None, stream or None)
+        self._check(rc, "b200h_copy_ranges_to_host")
 
     # -- files: stat + read + hash entirely inside the library (native reader threads, no mmap / Python I/O)
     @staticmethod

@@ -167,6 +167,46 @@ class BytesIOSegmentPayload(Payload):
             self.progress_report_cb(advance=len(chunk))
 
 
+class MemorySegmentPayload(BytesPayload):
+    """Body of one PUT whose bytes already lie in host memory (a ``memoryview`` into a staging buffer): sent from
+    where they are, ``chunk_size`` bytes per write with the progress reports and the ``reset_on_error`` behaviour of
+    ``BytesIOSegmentPayload``, without reading, copying or hashing anything."""
+
+    def __init__(self, data: memoryview, chunk_size: int = DEFAULT_SEGMENT_CHUNK_SIZE,
+                 progress_report_cb: Callable | None = None):
+        super().__init__(data)
+        self.chunk_size = chunk_size
+        self.progress_report_cb = progress_report_cb if progress_report_cb is not None else _ignore_progress
+        self.num_bytes_read = 0
+
+    @contextlib.contextmanager
+    def reset_on_error(self, subtract_progress: bool = False):
+        try:
+            yield
+        except Exception as failed:
+            sent, self.num_bytes_read = self.num_bytes_read, 0
+            try:
+                if subtract_progress:
+                    self.progress_report_cb(advance=-sent)
+                else:
+                    self.progress_report_cb(reset=True)
+            except Exception as cb_exc:
+                raise cb_exc from failed
+            raise
+        self.num_bytes_read = 0
+
+    async def write(self, writer: AbstractStreamWriter):
+        await self.write_with_length(writer, None)  # aiohttp < 3.12 enters here
+
+    async def write_with_length(self, writer: AbstractStreamWriter, content_length: int | None):
+        limit = len(self._value) if content_length is None else min(len(self._value), content_length)
+        while self.num_bytes_read < limit:
+            chunk = self._value[self.num_bytes_read : min(limit, self.num_bytes_read + self.chunk_size)]
+            await writer.write(chunk)
+            self.num_bytes_read += len(chunk)
+            self.progress_report_cb(advance=len(chunk))
+
+
 class KnownBytesBody:
     """An in-memory blob on its way to a single-part PUT together with the MD5 the GPU batch already produced for it.
     The map pump creates one per blobified input (10^5 per map), so this is a two-slot record; the aiohttp payload

@@ -1384,6 +1384,107 @@ int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, 
     return 0;
 }
 
+int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                              uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* h_dst,
+                              uint64_t h_dst_bytes, const uint64_t* dst_offsets, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_ranges_to_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
+    if (!file_first_seg) return fail(ctx, B200H_E_INVALID, "file_first_seg must not be NULL (it has nfiles + 1 entries)");
+    if (file_first_seg[0] != 0) return fail(ctx, B200H_E_INVALID, "file_first_seg[0] must be 0");
+    if (file_first_seg[nfiles] != nsegs) return fail(ctx, B200H_E_INVALID, "file_first_seg[nfiles] must equal nsegs");
+    for (uint64_t f = 0; f < nfiles; ++f)
+        if (file_first_seg[f + 1] < file_first_seg[f]) return fail(ctx, B200H_E_INVALID, "file_first_seg must not decrease");
+    // seg_start[s]: offset of segment s in its file; file_size[f]
+    std::vector<uint64_t> seg_start(nsegs), file_size(nfiles, 0);
+    for (uint64_t f = 0; f < nfiles; ++f)
+        for (uint64_t s = file_first_seg[f]; s < file_first_seg[f + 1]; ++s) {
+            if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
+            if (file_size[f] + segs[s].len < file_size[f]) return fail(ctx, B200H_E_INVALID, "a file is larger than 2^64 - 1 bytes");
+            seg_start[s] = file_size[f];
+            file_size[f] += segs[s].len;
+        }
+    if (nranges && (!ranges || !dst_offsets)) return fail(ctx, B200H_E_INVALID, "ranges and dst_offsets must not be NULL");
+    if (nranges && !h_dst) return fail(ctx, B200H_E_INVALID, "h_dst must not be NULL");
+    if ((uintptr_t)h_dst & 15u) return fail(ctx, B200H_E_INVALID, "h_dst must be 16-byte aligned");
+    std::vector<uint64_t> order;  // the non-empty ranges, by destination
+    for (uint64_t i = 0; i < nranges; ++i) {
+        const b200h_file_range& r = ranges[i];
+        const std::string name = "range " + std::to_string(i);
+        if (r.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
+        if (r.offset > file_size[r.file] || r.len > file_size[r.file] - r.offset)
+            return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
+        if (dst_offsets[i] & 15u) return fail(ctx, B200H_E_INVALID, name + ": its destination offset is not a multiple of 16");
+        if (dst_offsets[i] > h_dst_bytes || r.len > h_dst_bytes - dst_offsets[i])
+            return fail(ctx, B200H_E_INVALID, name + ": its destination reaches past h_dst_bytes");
+        if (r.len) order.push_back(i);
+    }
+    std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return dst_offsets[a] < dst_offsets[b]; });
+    for (size_t k = 1; k < order.size(); ++k)
+        if (dst_offsets[order[k - 1]] + ranges[order[k - 1]].len > dst_offsets[order[k]])
+            return fail(ctx, B200H_E_INVALID, "the destinations of ranges " + std::to_string(order[k - 1]) + " and " +
+                                                  std::to_string(order[k]) + " overlap");
+    if (nranges == 0) return 0;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    // the destination must be page-locked host memory the device can store to (pageable memory would fault the kernel)
+    void* d_dst = nullptr;
+    for (const uint8_t* q : {(const uint8_t*)h_dst, (const uint8_t*)h_dst + (h_dst_bytes ? h_dst_bytes - 1 : 0)}) {
+        cudaPointerAttributes at;
+        const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess && at.type == cudaMemoryTypeHost &&
+                        cudaHostGetDevicePointer(&d_dst, h_dst, 0) == cudaSuccess && d_dst;
+        cudaGetLastError();
+        if (!ok)
+            return fail(ctx, B200H_E_INVALID,
+                        "h_dst is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
+    }
+    for (uint64_t s = 0; s < nsegs; ++s)
+        if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
+            return fail(ctx, B200H_E_INVALID,
+                        "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
+    if (order.empty()) return 0;
+
+    // pieces (range x segment, in destination order within a range) and the tiles that draw from them
+    std::vector<StagePiece> pieces;
+    std::vector<StageTile> tiles;
+    for (uint64_t i = 0; i < nranges; ++i) {
+        const b200h_file_range& r = ranges[i];
+        if (!r.len) continue;
+        const uint64_t a = file_first_seg[r.file], b = file_first_seg[r.file + 1];
+        // the last segment of the file that starts at or before the range's first byte and is not empty
+        uint64_t s = std::upper_bound(seg_start.begin() + a, seg_start.begin() + b, r.offset) - seg_start.begin() - 1;
+        const size_t first = pieces.size();
+        for (uint64_t done = 0; done < r.len; ++s) {
+            const uint64_t in = r.offset + done - seg_start[s];
+            if (in >= segs[s].len) continue;  // an empty segment
+            const uint64_t n = std::min(segs[s].len - in, r.len - done);
+            pieces.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in, dst_offsets[i] + done, n});
+            done += n;
+        }
+        size_t p = first;
+        for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
+            const uint64_t n = std::min(kStageTileBytes, r.len - o), d = dst_offsets[i] + o;
+            while (pieces[p].dst + pieces[p].len <= d) ++p;
+            size_t q = p;
+            while (q + 1 < pieces.size() && pieces[q + 1].dst < d + n) ++q;
+            tiles.push_back({d, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
+        }
+    }
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    // stream-ordered allocation, as b200h_crc32_device: no synchronisation, no scratch shared with other streams' calls
+    const size_t tile_bytes = tiles.size() * sizeof(StageTile), bytes = tile_bytes + pieces.size() * sizeof(StagePiece);
+    void* d_table = nullptr;
+    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
+    StageTile* d_tiles = (StageTile*)d_table;
+    StagePiece* d_pieces = (StagePiece*)((uint8_t*)d_table + tile_bytes);
+    CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tile_bytes, cudaMemcpyHostToDevice, st));
+    CU_TRY(ctx, cudaMemcpyAsync(d_pieces, pieces.data(), bytes - tile_bytes, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_dst, st);
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaFreeAsync(d_table, st));
+    return 0;
+}
+
 // ---------------------------------------------------------------------------------------------- files
 
 int b200h_stat_files(b200h_ctx* ctx, const char* const* paths, uint64_t n, uint64_t* sizes_out, uint32_t* modes_out) {

@@ -104,6 +104,22 @@ int launch_crc32(const CrcRange* ranges, const uint64_t* first, uint64_t n, uint
 // (host arithmetic on CRC values; no data involved)
 uint32_t crc32_length_term(uint64_t len);
 
+// Ranges of segmented device files copied to one destination buffer (b200hash_stage.cu).  A piece is the part of a
+// range that lies in one segment (len > 0); the pieces of a range are listed in destination order and cover its
+// destination without gaps.  A tile is up to kStageTileBytes of one range's destination, starting at a multiple of 16;
+// it draws from pieces [first_piece, first_piece + npieces), the first of which holds the tile's first byte.
+struct StagePiece {
+    uint64_t src, dst, len;  // device address; byte offset in the destination buffer
+};
+struct StageTile {
+    uint64_t dst;  // byte offset in the destination buffer
+    uint32_t len, npieces;
+    uint64_t first_piece;
+};
+constexpr uint64_t kStageTileBytes = 64 << 10;
+// Every tile's copy, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the device can store to.
+int launch_stage_ranges(const StageTile* tiles, uint64_t ntiles, const StagePiece* pieces, void* dst, cudaStream_t st);
+
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)
 cudaError_t configure_kernels();  // one-time cudaFuncSetAttribute calls for the current device

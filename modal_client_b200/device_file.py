@@ -18,6 +18,11 @@ image is never assembled, neither in host memory nor in HBM.
 so host memory never has to hold the tensors.  ``bytes_to_host`` counts what has crossed.  The readers ``reopen()``
 hands out share the tensors, the bounce buffer and that counter.  The tensors must not change while an upload reads
 them.
+
+``stage_ranges(files, ranges, dst, dst_offsets)`` is the bulk route off the device: any byte ranges of any number of
+device files into a page-locked buffer with ONE ``b200h_copy_ranges_to_host`` call, after which the tensors are not
+needed for those bytes.  The volumefs2 uploader uses it for the missing blocks when it is given
+``device_staging_bytes``.
 """
 from __future__ import annotations
 
@@ -86,6 +91,14 @@ class _TensorBytes:
         """Order this source's stream after everything ``other``'s stream holds."""
         if other.stream_handle != self.stream_handle:
             self.stream.wait_stream(other.stream)
+
+    def _mark(self):
+        """-> a callable that blocks until everything queued on this source's stream so far has completed."""
+        import torch
+
+        event = torch.cuda.Event()
+        event.record(self.stream)
+        return event.synchronize
 
     @classmethod
     def _to_device(cls, data: bytes, ctx):
@@ -197,6 +210,58 @@ def hash_parts_many(files: list["DeviceFile"], part_len: int, flags: int = _lib.
     digested by ONE ``b200h_hash_segment_parts_device`` call on the first file's stream, which is ordered after every
     file's stream.  -> (sha uint8[n,32] | None, md5 uint8[n,16] | None, trimmed uint64[n])."""
     return _hash_sources([f._src for f in files], ctx or get_context(), part_len, flags)
+
+
+class Staged:
+    """Ranges of device files on their way into a page-locked host buffer (``stage_ranges``)."""
+
+    def __init__(self, dst: np.ndarray, spans: list[tuple[int, int]], done):
+        self._dst, self._spans, self._done = dst, spans, done
+
+    def wait(self) -> None:
+        """Blocks until the copy has completed (call it through ``asyncio.to_thread`` from a coroutine).  From then on
+        the files' tensors are not needed for these ranges."""
+        if self._done is not None:
+            self._done()
+            self._done = None
+
+    def view(self, i: int) -> memoryview:
+        """The bytes of range ``i`` where they are in the destination buffer (no copy); valid after ``wait()``."""
+        at, n = self._spans[i]
+        return memoryview(self._dst[at : at + n])
+
+
+def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets, ctx=None) -> Staged:
+    """Copy ``ranges`` -- ``(index into files, offset, length)`` each -- of device files into ``dst``, a uint8 array
+    over page-locked memory from ``ctx.host_alloc``; range i lands at ``dst[dst_offsets[i]:]`` (offsets multiples of
+    16, destinations disjoint; the layout is the caller's).  ONE ``b200h_copy_ranges_to_host`` call (one kernel launch)
+    whatever the files are made of, enqueued on the first file's stream, which is ordered after every file's stream.
+    Returns at once; ``wait()`` on the result blocks until the bytes are in ``dst``.  Every file's ``bytes_to_host``
+    grows by the bytes of its ranges."""
+    ctx = ctx or get_context()
+    sources = [f._src for f in files]
+    ranges = [(int(f), int(o), int(n)) for f, o, n in ranges]
+    offsets = [int(o) for o in dst_offsets]
+    if len(offsets) != len(ranges):
+        raise ValueError("dst_offsets needs one entry per range")
+    if not sources:
+        if ranges:
+            raise ValueError("ranges without files")
+        return Staged(dst, [], None)
+    lead = sources[0]
+    ptrs, lens, first = [], [], [0]
+    for src in sources:
+        lead._after(src)
+        ptrs += [s.data_ptr() if s.numel() else 0 for s in src.segments]
+        lens += [s.numel() for s in src.segments]
+        first.append(len(lens))
+    with lead._on_stream():
+        ctx.copy_ranges_to_host(ptrs, lens, first, ranges, dst, offsets, lead.stream_handle)
+        done = lead._mark()
+    for f, _, n in ranges:
+        with sources[f].lock:
+            sources[f].bytes_to_host += n
+    return Staged(dst, [(at, n) for at, (_, _, n) in zip(offsets, ranges)], done)
 
 
 # ------------------------------------------------------------------------------------------ safetensors
@@ -681,4 +746,4 @@ class DeviceFile(io.RawIOBase):
         return f"<DeviceFile {self._src.nbytes} bytes in {len(segs)} segments on {segs[0].device}>"
 
 
-__all__ = ["DeviceFile", "BOUNCE_BYTES", "hash_parts_many", "safetensors_layout"]
+__all__ = ["DeviceFile", "BOUNCE_BYTES", "Staged", "hash_parts_many", "safetensors_layout", "stage_ranges"]

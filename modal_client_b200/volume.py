@@ -10,7 +10,9 @@ batch for the whole tree -- before the first RPC goes out.  File objects (``Byte
 per-object spec builders.  A ``DeviceFile`` (the bytes of a CUDA tensor) is hashed in GPU memory by the volumefs2
 uploader -- all of a batch's ``DeviceFile``s, safetensors images of whole state dicts included, in one device call
 (``blob_utils.device_file_specs2``) -- and only the trimmed bytes of the blocks the server is missing are copied to the
-host; the volumefs1 uploader reads it like any other stream.
+host; the volumefs1 uploader reads it like any other stream.  Given ``device_staging_bytes`` of page-locked host memory,
+the volumefs2 uploader copies those blocks off the device in waves of one ``stage_ranges`` call each and PUTs them from
+there, so the tensors are free again (``device_released``) after the last copy instead of after the last PUT.
 """
 from __future__ import annotations
 
@@ -29,7 +31,7 @@ from . import _wire, blob_utils
 from ._logging import logger
 from .async_utils import bounded_map, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
-from .device_file import DeviceFile
+from .device_file import DeviceFile, stage_ranges
 from .exception import ExecutionError
 from .http_utils import ClientSessionRegistry
 
@@ -166,12 +168,26 @@ class VolumeUploadContextManager2(_BatchBase):
     """volumefs2 batch upload: all 8 MiB blocks of all queued files form one GPU batch (trim scan + SHA-256)."""
 
     def __init__(self, volume_id: str, client, progress_cb=None, force: bool = False,
-                 hash_concurrency: int | None = None, put_concurrency: int = 128):
+                 hash_concurrency: int | None = None, put_concurrency: int = 128,
+                 device_staging_bytes: int | None = None):
+        """``device_staging_bytes``: page-locked host memory the batch may take (``ctx.host_alloc``, from the first
+        missing-block answer until the batch ends) to stage the missing blocks of its ``DeviceFile``s: they are copied
+        off the device in waves of at most half that many bytes, one device call per wave, and PUT from host memory,
+        wave k + 1 being copied while wave k's PUTs run.  ``device_released`` is set once the last wave's copy has
+        completed: from then on the batch never reads the tensors again, so they may change while the PUTs drain.  It
+        must hold two blocks.  ``None`` (the default) takes no such memory: every block is read through its file's
+        bounce buffer while it is PUT, and the tensors must not change until the batch has ended."""
         super().__init__(volume_id, client, progress_cb, force)
         # the reference hashes blocks under a semaphore of ``hash_concurrency`` = cpu_count executor threads
         # (volume.py:1358,1383); here every block of every file is one GPU batch, so the knob is accepted and unused
         self._hash_concurrency = hash_concurrency
         self._put_concurrency = put_concurrency
+        if device_staging_bytes is not None and device_staging_bytes < 2 * blob_utils.BLOCK_SIZE:
+            raise ValueError(f"device_staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), "
+                             f"got {device_staging_bytes}")
+        self._device_staging_bytes = device_staging_bytes
+        self._device_files: dict[int, DeviceFile] = {}  # index into the batch's specs -> the file behind it
+        self.device_released = asyncio.Event()  # the batch no longer reads its DeviceFiles' tensors
 
     async def __aexit__(self, exc_type, exc_val, exc_tb):
         if exc_val:
@@ -182,12 +198,24 @@ class VolumeUploadContextManager2(_BatchBase):
         one_at_a_time = asyncio.Semaphore(1)
         for fp, remote, mode in self._fileobjs:
             if isinstance(fp, DeviceFile):
+                self._device_files[len(specs)] = fp
                 specs.append(next(device_specs))
             else:
                 specs.append(await FileUploadSpec2.from_fileobj(fp, remote, one_at_a_time, mode))
         await self._put_file_specs(specs)
 
     async def _put_file_specs(self, file_specs: list[FileUploadSpec2]):
+        staging = None
+        if self._device_staging_bytes is not None:
+            staging = _DeviceStaging(self._device_files, self._device_staging_bytes, self.device_released)
+        try:
+            await self._put_rounds(file_specs, staging)
+        finally:
+            if staging is not None:
+                staging.close()
+            self.device_released.set()  # at the latest when the batch ends, however it ends
+
+    async def _put_rounds(self, file_specs: list[FileUploadSpec2], staging: "_DeviceStaging | None"):
         put_responses: dict[bytes, bytes] = {}
         B = _wire.VolumePutFiles2Request
         for _attempt in range(2):  # once to learn the missing blocks, once more with every put_response
@@ -204,24 +232,77 @@ class VolumeUploadContextManager2(_BatchBase):
                 if type(exc).__name__ == "AlreadyExistsError":
                     raise FileExistsError(str(exc))
                 raise
+            if staging is not None:
+                if not any(mb.file_index in staging.files for mb in response.missing_blocks):
+                    self.device_released.set()
+                elif self.device_released.is_set():
+                    # the tensors were given back after the first round: there is nothing left to read
+                    raise RuntimeError("Did not succeed at uploading all files despite supplying all missing blocks")
             if not response.missing_blocks:
                 break
             await _put_missing_blocks(file_specs, response.missing_blocks, put_responses, self._put_concurrency,
-                                      self._progress_cb)
+                                      self._progress_cb, staging)
         else:
             raise RuntimeError("Did not succeed at uploading all files despite supplying all missing blocks")
         self._progress_cb(complete=True)
 
 
+class _DeviceStaging:
+    """The page-locked buffer a volumefs2 batch stages its DeviceFiles' missing blocks through: two halves, a wave of
+    blocks each (every block at a multiple of 128 bytes, its trimmed length)."""
+
+    ALIGN = 128
+
+    def __init__(self, files: dict[int, DeviceFile], nbytes: int, released: asyncio.Event):
+        self.files, self.released = files, released
+        self.half = nbytes // 2 // self.ALIGN * self.ALIGN
+        self._ctx, self._buf = None, None
+
+    def buffer(self) -> np.ndarray:
+        if self._buf is None:
+            self._ctx = blob_utils.get_context()
+            self._buf = self._ctx.host_alloc(2 * self.half)
+        return self._buf
+
+    def waves(self, file_specs, missing) -> list[list[tuple[Any, int, int]]]:
+        """``missing`` (blocks of device files) cut greedily, in order, into waves that fit one half:
+        [(missing block, offset in the half, trimmed length), ...] per wave."""
+        waves, used = [], 0
+        for mb in missing:
+            block = file_specs[mb.file_index].blocks[mb.block_index]
+            n = block.end - block.start
+            if not waves or used + n > self.half:
+                waves.append([])
+                used = 0
+            waves[-1].append((mb, used, n))
+            used += -(-n // self.ALIGN) * self.ALIGN
+        return waves
+
+    def stage(self, file_specs, wave, half: int):
+        """Enqueue one wave's copy into half ``half``: one ``stage_ranges`` call."""
+        order = sorted({mb.file_index for mb, _, _ in wave})
+        slot = {f: i for i, f in enumerate(order)}
+        ranges = [(slot[mb.file_index], file_specs[mb.file_index].blocks[mb.block_index].start, n) for mb, _, n in wave]
+        return stage_ranges([self.files[f] for f in order], ranges, self.buffer(),
+                            [half * self.half + at for _, at, _ in wave], ctx=self._ctx)
+
+    def close(self):
+        if self._buf is not None:
+            self._ctx.host_free(self._buf)
+            self._buf = None
+
+
 async def _put_missing_blocks(file_specs, missing_blocks, put_responses: dict[bytes, bytes], put_concurrency: int,
-                              progress_cb: Callable[..., Any]):
+                              progress_cb: Callable[..., Any], staging: _DeviceStaging | None = None):
     """PUT each block the server reported missing (only the zero-trimmed bytes travel) and remember the
-    server's put_response per block digest (py/modal/volume.py:1500-1574)."""
-    from .bytes_io_segment_payload import BytesIOSegmentPayload
+    server's put_response per block digest (py/modal/volume.py:1500-1574).  With ``staging``, the blocks of its device
+    files are first copied to its buffer, a wave per device call, and sent from there; everything else about the round
+    is the same."""
+    from .bytes_io_segment_payload import BytesIOSegmentPayload, MemorySegmentPayload
 
     pending: dict[str, tuple[Any, set[int]]] = {}
 
-    async def put_one(mb) -> tuple[bytes, bytes]:
+    async def put_one(mb, staged_bytes: memoryview | None = None) -> tuple[bytes, bytes]:
         spec = file_specs[mb.file_index]
         block = spec.blocks[mb.block_index]
         if spec.path not in pending:
@@ -238,11 +319,14 @@ async def _put_missing_blocks(file_specs, missing_blocks, put_responses: dict[by
                         raise ExecutionError(f"block PUT failed with status {resp.status}: {await resp.text()}")
                     return await resp.content.read()
 
-        with spec.source() as fp:
-            # the block digest is already known (GPU batch): no re-hash while sending
-            payload = BytesIOSegmentPayload(fp, block.start, block.end - block.start, chunk_size=256 * 1024,
-                                            progress_report_cb=report, md5_digest=b"\0" * 16)
-            data = await attempt(payload)
+        if staged_bytes is not None:  # the block is in host memory already: sent from there, retries included
+            data = await attempt(MemorySegmentPayload(staged_bytes, chunk_size=256 * 1024, progress_report_cb=report))
+        else:
+            with spec.source() as fp:
+                # the block digest is already known (GPU batch): no re-hash while sending
+                payload = BytesIOSegmentPayload(fp, block.start, block.end - block.start, chunk_size=256 * 1024,
+                                                progress_report_cb=report, md5_digest=b"\0" * 16)
+                data = await attempt(payload)
         waiting.discard(mb.block_index)
         if not waiting:
             report(complete=True)
@@ -257,8 +341,42 @@ async def _put_missing_blocks(file_specs, missing_blocks, put_responses: dict[by
                              np.uint8).reshape(len(missing), 32)
         first, _ = await asyncio.to_thread(blob_utils.get_context().dedupe, keys)
         missing = [mb for i, mb in enumerate(missing) if first[i] == i]
-    for digest, resp in await bounded_map(missing, put_one, concurrency=put_concurrency):
-        put_responses[digest] = resp
+    if staging is None:
+        for digest, resp in await bounded_map(missing, put_one, concurrency=put_concurrency):
+            put_responses[digest] = resp
+        return
+
+    slots = asyncio.Semaphore(put_concurrency)  # one bound for the staged and the unstaged PUTs of the round
+
+    async def put_limited(item) -> tuple[bytes, bytes]:
+        async with slots:
+            return await put_one(*item)
+
+    def start(items):
+        return asyncio.ensure_future(bounded_map(items, put_limited, concurrency=put_concurrency))
+
+    waves = staging.waves(file_specs, [mb for mb in missing if mb.file_index in staging.files])
+    running = [start([(mb,) for mb in missing if mb.file_index not in staging.files])]
+    if not waves:  # every missing device block has the content of an ordinary file's block that is sent instead
+        staging.released.set()
+    in_half: list[Any] = [None, None]  # the PUTs that still send from each half
+    try:
+        for k, wave in enumerate(waves):
+            if in_half[k & 1] is not None:
+                await in_half[k & 1]  # the half is free once every PUT out of it has its put_response
+            staged = staging.stage(file_specs, wave, k & 1)
+            await asyncio.to_thread(staged.wait)
+            if k == len(waves) - 1:
+                staging.released.set()
+            in_half[k & 1] = start([(mb, staged.view(i)) for i, (mb, _, _) in enumerate(wave)])
+            running.append(in_half[k & 1])
+        for task in running:
+            for digest, resp in await task:
+                put_responses[digest] = resp
+    finally:
+        for task in running:
+            task.cancel()
+        await asyncio.gather(*running, return_exceptions=True)
 
 
 # ---------------------------------------------------------------------------------- the reference's names
@@ -279,11 +397,15 @@ class _AbstractVolumeUploadContextManager:
     def put_directory(self, local_path, remote_path, recursive=True): ...
 
     @staticmethod
-    def resolve(version, object_id: str, client, progress_cb: Callable[..., Any] | None = None, force: bool = False):
+    def resolve(version, object_id: str, client, progress_cb: Callable[..., Any] | None = None, force: bool = False,
+                device_staging_bytes: int | None = None):
+        """``device_staging_bytes`` goes to the volumefs2 manager only: volumefs1 needs whole-object digests and reads
+        device files through the host anyway."""
         if version in (None, VOLUME_FS_VERSION_UNSPECIFIED, VOLUME_FS_VERSION_V1):
             return VolumeUploadContextManager(object_id, client, progress_cb=progress_cb, force=force)
         if version == VOLUME_FS_VERSION_V2:
-            return VolumeUploadContextManager2(object_id, client, progress_cb=progress_cb, force=force)
+            return VolumeUploadContextManager2(object_id, client, progress_cb=progress_cb, force=force,
+                                               device_staging_bytes=device_staging_bytes)
         raise RuntimeError(f"unsupported volume version: {version}")
 
 

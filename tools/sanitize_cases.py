@@ -6,6 +6,9 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
   trim kernels probe + wide scan (atomicMax across CTAs, work counter), blank and half-blank blocks
   dedupe       hash-table insert/resolve with CAS
   streams      absorb/digest on a private CUDA stream
+  stage        ranges of segmented device files into page-locked host memory: every source phase, segments that start
+               at the first and end at the last byte of their allocation (the aligned-hull loads), ranges across tiny
+               and empty segments, partial last words
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -83,5 +86,31 @@ assert s.digests() == (hashlib.sha256(data).digest(), hashlib.md5(data).digest()
 s.close()
 c2.close()
 print("stream ok", flush=True)
+
+# 6. stage_ranges_kernel: segments cut out of exact-size allocations at every phase, ranges with odd edges
+import torch
+
+pool = [torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda") for n in (70_001, 4097, 33, 1, 300_007)]
+segs = [pool[0], pool[1][5:], pool[2][:-3], pool[3], pool[1][:0], pool[4][9:]] + [pool[4][i * 7 : i * 7 + 1 + i % 9] for i in range(64)]
+segs += [pool[0][ph : 5000 + 2 * ph] for ph in range(16)]
+image = np.concatenate([t.cpu().numpy() for t in segs])
+ranges = [(0, 0, image.size), (0, 3, image.size - 8), (0, image.size - 1, 1), (0, 7, 0)]
+ranges += [(0, 70_001 - 9 + a, 4097 + 40 + a) for a in range(16)]
+offsets, at = [], 128
+for _, _, n in ranges:
+    offsets.append(at)
+    at += -(-n // 128) * 128 + 128
+dst = ctx.host_alloc(at)
+dst[:] = 0xC3
+ctx.copy_ranges_to_host([t.data_ptr() if t.numel() else 0 for t in segs], [t.numel() for t in segs], [0, len(segs)], ranges,
+                        dst, offsets, 1)
+torch.cuda.synchronize()
+clean = np.ones(at, bool)
+for (_, off, n), o in zip(ranges, offsets):
+    assert np.array_equal(dst[o : o + n], image[off : off + n]), (off, n)
+    clean[o : o + n] = False
+assert (dst[clean] == 0xC3).all()
+ctx.host_free(dst)
+print("stage ranges ok", flush=True)
 ctx.close()
 print("ALL OK")
