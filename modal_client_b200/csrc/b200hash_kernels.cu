@@ -87,284 +87,139 @@ __device__ __forceinline__ uint32_t add_rotl(uint32_t acc, uint32_t u) {
 __device__ __forceinline__ uint32_t rotr(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
 __device__ __forceinline__ uint32_t rotl(uint32_t x, int n) { return __funnelshift_l(x, x, n); }
 __device__ __forceinline__ uint32_t bswap(uint32_t x) { return __byte_perm(x, 0, 0x0123); }
-// rotr by a compile-time amount; no instruction for 0
-template <int N>
-__device__ __forceinline__ uint32_t rotr_c(uint32_t x) {
-    return N == 0 ? x : rotr(x, N);
-}
-
-// lop3 over (a, b, c) with the operands passed in the order PERM names -- 0 (a, b, c), 1 (a, c, b), 2 (b, a, c),
-// 3 (b, c, a), 4 (c, a, b), 5 (c, b, a) -- and the truth table permuted to match, so the result is the same.
-__host__ __device__ constexpr int lop3_src(int perm, int k) {  // which of a (0), b (1), c (2) goes to operand slot k
-    return (perm == 0 ? 0x210 : perm == 1 ? 0x120 : perm == 2 ? 0x201 : perm == 3 ? 0x021 : perm == 4 ? 0x102 : 0x012) >>
-               (4 * k) & 15;
-}
-__host__ __device__ constexpr int lop3_lut(int imm, int perm) {
-    int lut = 0;
-    for (int j = 0; j < 8; ++j) {  // j: the slot values, slot 0 in bit 2 (the 0xF0 operand)
-        int i = 0;
-        for (int k = 0; k < 3; ++k) i |= ((j >> (2 - k)) & 1) << (2 - lop3_src(perm, k));
-        lut |= ((imm >> i) & 1) << j;
-    }
-    return lut;
-}
-template <int IMM, int PERM>
-__device__ __forceinline__ uint32_t lop3p(uint32_t a, uint32_t b, uint32_t c) {
-    constexpr int s0 = lop3_src(PERM, 0), s1 = lop3_src(PERM, 1), s2 = lop3_src(PERM, 2);
-    const uint32_t v[3] = {a, b, c};
-    return lop3<lop3_lut(IMM, PERM)>(v[s0], v[s1], v[s2]);
-}
-static_assert(lop3_lut(0xCA, 0) == 0xCA && lop3_lut(0x96, 5) == 0x96 && lop3_lut(0xCA, 2) == 0xE2, "lop3 permutation");
 
 // ---------------------------------------------------------------------- compression functions
 // SHA-256: FIPS 180-4 section 6.2.2; MD5: RFC 1321 section 3.4.  Boolean functions are single LOP3s:
-//   Ch(e,f,g)=e?f:g (0xCA)  Maj (0xE8)  xor3 (0x96)  MD5 F=b?c:d (0xCA)  G=d?b:c (0xE4)  I=c^(b|~d) (0x39)
+//   Ch(e,f,g)=e?f:g (0xCA)  Maj (0xE8)  xor3 (0x96)  MD5 F=b?c:d (0xCA)  G=d?b:c (0xE4)  H=b^c^d (0x96)  I=c^(b|~d) (0x39)
 
 #define SHA_S0(x) lop3<0x96>(rotr(x, 2), rotr(x, 13), rotr(x, 22))
 #define SHA_S1(x) lop3<0x96>(rotr(x, 6), rotr(x, 11), rotr(x, 25))
 #define SHA_s0(x) lop3<0x96>(rotr(x, 7), rotr(x, 18), (x) >> 3)
 #define SHA_s1(x) lop3<0x96>(rotr(x, 17), rotr(x, 19), (x) >> 10)
+constexpr int kMd5F = 0xCA, kMd5G = 0xE4, kMd5H = 0x96, kMd5I = 0x39;
 
-// one SHA round on rotating register names; KW = K[i] + W[i]
-// B200H_ADDMODE selects where the additions run: 0 = plain C (ptxas picks IADD3 on the ALU pipe),
-// 1 = every add as IMAD on the FMA pipe, 2 = hybrid: the two 3-input sums of a SHA round stay IADD3
-// (one ALU slot each, shortest critical path), everything else moves to the FMA pipe.
-#ifndef B200H_ADDMODE
-#define B200H_ADDMODE 1
-#endif
-#if B200H_ADDMODE == 0
-#define ADD(x, y) ((x) + (y))
-#elif B200H_ADDMODE == 4
-// mode 4: single two-input PTX adds (ptxas: VIADD / IADD3 as it sees fit, no forced multiply)
-__device__ __forceinline__ uint32_t add2(uint32_t a, uint32_t b) {
-    uint32_t d;
-    asm volatile("add.u32 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-    return d;
+// lop3<IMM>(a, b, c) issued with its operands in the order (b, c, a), the truth table permuted to match
+__host__ __device__ constexpr int lut_bca(int imm) {
+    int lut = 0;
+    for (int j = 0; j < 8; ++j) lut |= ((imm >> (((j & 1) << 2) | (j >> 1))) & 1) << j;
+    return lut;
 }
-#define ADD(x, y) add2((x), (y))
-#elif B200H_ADDMODE == 5
-// mode 5: scalar video add (experiment: does ptxas keep it as a two-input VIADD?)
-__device__ __forceinline__ uint32_t addv(uint32_t a, uint32_t b) {
-    uint32_t d;
-    asm("vadd.u32.u32.u32 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-    return d;
+static_assert(lut_bca(0xCA) == 0xE4 && lut_bca(0xE8) == 0xE8 && lut_bca(0x96) == 0x96, "lop3 operand order");
+template <int IMM>
+__device__ __forceinline__ uint32_t lop3_bca(uint32_t a, uint32_t b, uint32_t c) {
+    return lop3<lut_bca(IMM)>(b, c, a);
 }
-#define ADD(x, y) addv((x), (y))
-#else
-// kPlainAdd (a constant where ADD is expanded): false = the add is issued as IMAD on the FMA pipe (dense batches:
-// the ALU pipe is the bottleneck); true = plain add, ptxas fuses pairs into IADD3 / LEA (sparse batches: a warp
-// alone on its SMSP issues one instruction per two cycles whatever the pipe, so fewer instructions win).
-#define ADD(x, y) (kPlainAdd ? ((x) + (y)) : addf((x), (y), one))
-#endif
-// The outer rotate of Sigma1 / Sigma0 ends in an add once it is factored out: Sigma1(e) = rotr6(e ^ rotr5(e) ^ rotr19(e)) goes into T1, Sigma0(a) = rotr2(a ^
-// rotr11(a) ^ rotr20(a)) onto Maj.
-// B200H_SHAONLY_ROT, the SHA-256-only instantiation, where the ALU pipe carries 1040 of the 1640 instructions per
-// block while the FMA pipe idles:
-//   bit 0 / bit 1: the outer rotate of Sigma1 / Sigma0 is a widening multiply x * 2^(32-n) -> {x << (32-n), x >> n};
-//                  the halves have disjoint bits, so both are simply added into the round sum (one SHF less, one
-//                  IMAD.WIDE + one IMAD more);
-//   bit 2:         the plain shifts of sigma0/sigma1 are IMAD.HI by 2^(32-n).
-// B200H_FUSED_MIX, the dense fused SHA-256 + MD5 instantiation, where the kernel issues at the rate its vector
-// register reads allow, well under both pipes' rates, so fewer instructions win (DESIGN.md 5.1): a rotate
-// whose result is added becomes one LEA.HI (add_rotl) in place of SHF + IMAD, 1 instruction less, ALU pipe unchanged:
-//   bit 0 / bit 1: Sigma1 / Sigma0 outer rotate with its add (128 per block);
-//   bit 2:         MD5's a = b + rotl(t, s) (64 per block).
-// Multiplies do not pay here: IMAD.HI issues at half the rate of IMAD or SHF on H100 (tools/ubench.cu).
-// B200H_FUSED_CONST_ADD, the dense fused instantiation: 1 = the adds of a round constant (SHA-256's W + K, MD5's
-// x + T, 128 per block) are plain adds, which ptxas issues as VIADD R, R, imm; 0 = IMAD R, R, R(one), imm.  Any IMAD
-// with an immediate addend makes ptxas keep `one` in a vector register for every addf, so each of the other 528 adds
-// of a block reads three vector registers; with 1 they read `one` from a uniform register (IMAD R, R, UR, R), which
-// saves a vector register-file read per add (DESIGN.md 5.1).  VIADD stays off the ALU pipe: it issues next to SHF and
-// LOP3 above that pipe's rate (tools/ubench.cu).
-#ifndef B200H_SHAONLY_ROT
-#define B200H_SHAONLY_ROT 3
-#endif
-#ifndef B200H_FUSED_MIX
-#define B200H_FUSED_MIX 7
-#endif
-#ifndef B200H_FUSED_CONST_ADD
-#define B200H_FUSED_CONST_ADD 1
-#endif
-// Equivalent forms of the dense fused body.  Each gives the same digests and the same ALU-pipe instructions; they
-// change which registers the instructions read and how ptxas schedules and allocates them (DESIGN.md 5.1):
-//   B200H_FUSED_S1_OUT (6, 11 or 25) / B200H_FUSED_S0_OUT (2, 13 or 22): the rotate of Sigma1 / Sigma0 that is taken
-//       outside the xor3 and fused with its add into LEA.HI, e.g. Sigma1 = rotr6(e ^ rotr5 e ^ rotr19 e) =
-//       rotr11(rotr27 e ^ e ^ rotr14 e) = rotr25(rotr13 e ^ rotr18 e ^ e);
-//   B200H_FUSED_LOP_SHA / B200H_FUSED_LOP_MD5 (0..5): the operand order of every LOP3 of SHA-256 (Ch, Maj, the Sigma
-//       and sigma xor3s) / MD5 (F, G, H, I), with its truth table permuted to match (lop3p);
-//   B200H_FUSED_SCHED (1, 4 or 8): message schedule words expanded ahead of the rounds that use them (4: the four of
-//       each quad of rounds, 8: the next eight every second quad, 1: each word just before its round);
-//   B200H_FUSED_MD5_FIRST (with B200H_ILV 4): 1 = each quad's four MD5 steps ahead of its four SHA-256 rounds in
-//       source order (what B200H_ILV=40 does for every instantiation), 0 = after them.
-// The defaults (LOP3 order 3 = (b, c, a), MD5 first, 3 CTAs per SM in B200H_LANE_MIN_CTAS_FUSED) were picked from
-// measured builds: 3.1 % less lane-kernel time than the forms before (tools/lane_sass_score.py, DESIGN.md 5.1, 6).
-#ifndef B200H_FUSED_S1_OUT
-#define B200H_FUSED_S1_OUT 6
-#endif
-#ifndef B200H_FUSED_S0_OUT
-#define B200H_FUSED_S0_OUT 2
-#endif
-#ifndef B200H_FUSED_LOP_SHA
-#define B200H_FUSED_LOP_SHA 3
-#endif
-#ifndef B200H_FUSED_LOP_MD5
-#define B200H_FUSED_LOP_MD5 0
-#endif
-#ifndef B200H_FUSED_SCHED
-#define B200H_FUSED_SCHED 4
-#endif
-#ifndef B200H_FUSED_MD5_FIRST
-#define B200H_FUSED_MD5_FIRST 1
-#endif
-static_assert(B200H_FUSED_S1_OUT == 6 || B200H_FUSED_S1_OUT == 11 || B200H_FUSED_S1_OUT == 25, "B200H_FUSED_S1_OUT");
-static_assert(B200H_FUSED_S0_OUT == 2 || B200H_FUSED_S0_OUT == 13 || B200H_FUSED_S0_OUT == 22, "B200H_FUSED_S0_OUT");
-static_assert(B200H_FUSED_SCHED == 1 || B200H_FUSED_SCHED == 4 || B200H_FUSED_SCHED == 8, "B200H_FUSED_SCHED");
-// x + a round constant; kConstAdd (a constant inside compress<>) is B200H_FUSED_CONST_ADD in the dense fused
-// instantiation, else 0
-#define ADDK(x, k) (kConstAdd ? ((x) + (k)) : ADD((x), (k)))
 __device__ __forceinline__ void rotw(uint32_t x, uint32_t mul, uint32_t& lo, uint32_t& hi) {
     uint64_t d;
     asm("mul.wide.u32 %0, %1, %2;" : "=l"(d) : "r"(x), "r"(mul));
     lo = (uint32_t)d;
     hi = (uint32_t)(d >> 32);
 }
-__device__ __forceinline__ uint32_t mulhi(uint32_t x, uint32_t m) {
-    uint32_t d;
-    asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(m));
-    return d;
-}
-// FUSED: the Sigma rotates through add_rotl (B200H_FUSED_MIX) instead of rotw (B200H_SHAONLY_ROT), outer rotates
-// B200H_FUSED_S1_OUT / B200H_FUSED_S0_OUT, LOP3 operand order LOP (0 unless FUSED)
-template <int ROT, bool FUSED, int LOP>
-__device__ __forceinline__ void sha_rnd_rot(uint32_t a, uint32_t b, uint32_t c, uint32_t& d, uint32_t e, uint32_t f,
-                                            uint32_t g, uint32_t& h, uint32_t K, uint32_t W, uint32_t one) {
-    constexpr int R1 = B200H_FUSED_S1_OUT, R0 = B200H_FUSED_S0_OUT;
-    const uint32_t kw = (FUSED && B200H_FUSED_CONST_ADD) ? W + K : addf(W, K, one);
-    uint32_t t1 = addf(addf(h, kw, one), lop3p<0xCA, LOP>(e, f, g), one);
-    if ((ROT & 1) && FUSED) {
-        t1 = add_rotl<32 - R1>(t1, lop3p<0x96, LOP>(rotr_c<(38 - R1) % 32>(e), rotr_c<(43 - R1) % 32>(e),
-                                                    rotr_c<(57 - R1) % 32>(e)));
-    } else if (ROT & 1) {
+
+// The forms of the lane kernel's compression body, one per kind of batch; compress<> picks one per instantiation.
+// Dense batches put many warps on every SMSP, and the ALU pipe, which SHF/LOP3/PRMT already load, sets the pace: their
+// adds run as IMAD on the FMA pipe (addf).  Sparse batches (<= 4 warps per SM) leave every warp alone on its SMSP, where
+// it issues one instruction per two cycles whatever the pipe: their adds are plain C, which ptxas fuses into IADD3 / LEA
+// (~15 % fewer instructions per block).
+enum class Body {
+    kDenseFused,  // SHA-256 + MD5, dense
+    kDenseSha,    // SHA-256 alone, dense
+    kMd5,         // MD5 alone, dense or not
+    kSparse,      // SHA-256 + MD5 or SHA-256 alone, sparse
+};
+
+// One SHA-256 round on rotating register names: d += T1, h = T1 + T2.
+template <Body B>
+__device__ __forceinline__ void sha_round(uint32_t a, uint32_t b, uint32_t c, uint32_t& d, uint32_t e, uint32_t f,
+                                          uint32_t g, uint32_t& h, uint32_t K, uint32_t W, uint32_t one) {
+    if constexpr (B == Body::kDenseFused) {
+        // This kernel issues at the rate its vector register reads allow, well under both pipes' rates, so fewer
+        // instructions win (DESIGN.md 5.1).  Factored out, the outer rotate of Sigma1 / Sigma0 ends in an add --
+        // Sigma1(e) = rotr6(e ^ rotr5 e ^ rotr19 e) goes into T1, Sigma0(a) = rotr2(a ^ rotr11 a ^ rotr20 a) onto Maj --
+        // and each such pair is one LEA.HI (add_rotl) in place of SHF + IMAD: 1 instruction less, ALU pipe unchanged.
+        // Multiplies do not pay here: IMAD.HI issues at half the rate of IMAD or SHF on H100 (tools/ubench.cu).
+        // W + K is a plain add, which ptxas issues as VIADD R, R, imm.  Any IMAD with an immediate addend makes ptxas keep
+        // `one` in a vector register for every addf, so each of the other 528 adds of a block would read three vector
+        // registers; this way they read `one` from a uniform register (IMAD R, R, UR, R).  VIADD stays off the ALU pipe:
+        // it issues next to SHF and LOP3 above that pipe's rate (tools/ubench.cu).
+        // Every LOP3 of SHA-256 (here and in sha_sched) takes its operands in the order (b, c, a).  With 3 CTAs per SM
+        // and the MD5 steps ahead of the SHA-256 rounds (compress), that made the lane kernel 3.1 % faster than order
+        // (a, b, c) at 4 CTAs, H100 at 700 W (tools/lane_sass_score.py, DESIGN.md 5.1, 6).
+        uint32_t t1 = addf(addf(h, W + K, one), lop3_bca<0xCA>(e, f, g), one);
+        t1 = add_rotl<26>(t1, lop3_bca<0x96>(e, rotr(e, 5), rotr(e, 19)));
+        const uint32_t t2 = add_rotl<30>(lop3_bca<0xE8>(a, b, c), lop3_bca<0x96>(a, rotr(a, 11), rotr(a, 20)));
+        d = addf(d, t1, one);
+        h = addf(t1, t2, one);
+    } else if constexpr (B == Body::kDenseSha) {
+        // Without MD5 the ALU pipe carries 1040 of the 1640 instructions per block while the FMA pipe idles, so the
+        // outer rotate of Sigma1 / Sigma0 is a widening multiply x * 2^(32-n) -> {x << (32-n), x >> n}; the halves have
+        // disjoint bits, so both are simply added into the round sum (one SHF less, one IMAD.WIDE + one IMAD more).
+        uint32_t t1 = addf(addf(h, addf(W, K, one), one), lop3<0xCA>(e, f, g), one);
         uint32_t lo, hi;
         rotw(lop3<0x96>(e, rotr(e, 5), rotr(e, 19)), 1u << 26, lo, hi);
         t1 = addf(addf(t1, lo, one), hi, one);
-    } else {
-        t1 = addf(t1, lop3<0x96>(rotr(e, 6), rotr(e, 11), rotr(e, 25)), one);
-    }
-    uint32_t t2;
-    if ((ROT & 2) && FUSED) {
-        t2 = add_rotl<32 - R0>(lop3p<0xE8, LOP>(a, b, c), lop3p<0x96, LOP>(rotr_c<(34 - R0) % 32>(a),
-                                                                             rotr_c<(45 - R0) % 32>(a),
-                                                                             rotr_c<(54 - R0) % 32>(a)));
-    } else if (ROT & 2) {
-        uint32_t lo, hi;
         rotw(lop3<0x96>(a, rotr(a, 11), rotr(a, 20)), 1u << 30, lo, hi);
-        t2 = addf(addf(lo, hi, one), lop3<0xE8>(a, b, c), one);
+        const uint32_t t2 = addf(addf(lo, hi, one), lop3<0xE8>(a, b, c), one);
+        d = addf(d, t1, one);
+        h = addf(t1, t2, one);
     } else {
-        t2 = addf(lop3<0x96>(rotr(a, 2), rotr(a, 13), rotr(a, 22)), lop3<0xE8>(a, b, c), one);
+        static_assert(B == Body::kSparse, "no SHA-256 round in this body");
+        const uint32_t t1 = h + (W + K) + lop3<0xCA>(e, f, g) + SHA_S1(e);
+        const uint32_t t2 = SHA_S0(a) + lop3<0xE8>(a, b, c);
+        d = d + t1;
+        h = t1 + t2;
     }
-    d = addf(d, t1, one);
-    h = addf(t1, t2, one);
 }
-#if B200H_ADDMODE == 3
-// mode 3: only the last sum of a round (new a = T1 + Sigma0 + Maj) is a 3-input IADD3 on the ALU pipe
-#define SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                         \
-    {                                                                                 \
-        uint32_t t1 = ADD(ADD(ADD(h, ADDK(W, K)), lop3<0xCA>(e, f, g)), SHA_S1(e));   \
-        d = ADD(d, t1);                                                               \
-        h = t1 + SHA_S0(a) + lop3<0xE8>(a, b, c);                                     \
-    }
-#elif B200H_ADDMODE == 2
-#define SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                  \
-    {                                                                          \
-        uint32_t t1 = ADD(h, ADDK(W, K)) + SHA_S1(e) + lop3<0xCA>(e, f, g);    \
-        d = ADD(d, t1);                                                        \
-        h = t1 + SHA_S0(a) + lop3<0xE8>(a, b, c);                              \
-    }
-#else
-#define SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                         \
-    {                                                                                 \
-        uint32_t t1 = ADD(ADD(ADD(h, ADDK(W, K)), lop3<0xCA>(e, f, g)), SHA_S1(e));   \
-        uint32_t t2 = ADD(SHA_S0(a), lop3<0xE8>(a, b, c));                            \
-        d = ADD(d, t1);                                                               \
-        h = ADD(t1, t2);                                                              \
-    }
-#endif
-// kShaRot (a constant inside compress<>) is B200H_SHAONLY_ROT for the dense SHA-only instantiation, bits 0 and 1 of
-// B200H_FUSED_MIX for the dense fused one, else 0; kLopSha is B200H_FUSED_LOP_SHA in the dense fused one, else 0
-#define SHA_RND(a, b, c, d, e, f, g, h, K, W)                                                       \
-    {                                                                                               \
-        if (kShaRot & 3) sha_rnd_rot<kShaRot, DO_MD5, kLopSha>(a, b, c, d, e, f, g, h, K, W, one); \
-        else SHA_RND_BASE(a, b, c, d, e, f, g, h, K, W)                                             \
-    }
-#define SHA_SHR3(x) ((kShaRot & 4) ? mulhi((x), m29) : ((x) >> 3))
-#define SHA_SHR10(x) ((kShaRot & 4) ? mulhi((x), m22) : ((x) >> 10))
-#define SHA_s0r(x) lop3p<0x96, kLopSha>(rotr(x, 7), rotr(x, 18), SHA_SHR3(x))
-#define SHA_s1r(x) lop3p<0x96, kLopSha>(rotr(x, 17), rotr(x, 19), SHA_SHR10(x))
-// message schedule in place: w[i&15] becomes W[i] for i >= 16
-#define SHA_SCHED(w, i) \
-    (w[(i)&15] = ADD(ADD(ADD(w[(i)&15], w[((i)-7) & 15]), SHA_s0r(w[((i)-15) & 15])), SHA_s1r(w[((i)-2) & 15])))
 
-// Fused kernel: the adds of an MD5 step on the FMA pipe; with kMd5Rot (bit 2 of B200H_FUSED_MIX in the dense fused
-// instantiation, else 0) the last one is fused with the rotate into one LEA.HI; x + T is ADDK (VIADD with kConstAdd)
-#define MD5_STEP_FMA(FN, a, b, c, d, xk, s, T)                                    \
-    {                                                                             \
-        const uint32_t t_ = ADD(ADD(a, ADDK(xk, T)), FN(b, c, d));                \
-        if (kMd5Rot) a = add_rotl<(s)>(b, t_);                                    \
-        else a = ADD(b, rotl(t_, s));                                             \
-    }
-// MD5-only kernel: there the FMA pipe is the bottleneck (4 IMAD vs 2 ALU ops per step), so the 3-input sum
-// goes back to the ALU pipe as one IADD3: per step ALU = LOP3 + IADD3 + SHF, FMA = (x+T) and (+b).
-#define MD5_STEP_MIX(FN, a, b, c, d, xk, s, T)             \
-    {                                                      \
-        const uint32_t xt_ = ADD(xk, T);                   \
-        a = ADD(b, rotl(a + FN(b, c, d) + xt_, s));        \
-    }
-#define MD5_STEP(FN, a, b, c, d, xk, s, T)                 \
-    if (DO_SHA) MD5_STEP_FMA(FN, a, b, c, d, xk, s, T) else MD5_STEP_MIX(FN, a, b, c, d, xk, s, T)
-#define MD5_F(b, c, d) lop3p<0xCA, kLopMd5>(b, c, d)
-#define MD5_G(b, c, d) lop3p<0xE4, kLopMd5>(b, c, d)
-#define MD5_H(b, c, d) lop3p<0x96, kLopMd5>(b, c, d)
-#define MD5_I(b, c, d) lop3p<0x39, kLopMd5>(b, c, d)
+// Message schedule in place: w[i & 15] becomes W[i] for i >= 16, with the adds and LOP3 operand order of sha_round.
+// W[i-16], W[i-7], W[i-15], W[i-2] are read in the order they are added: another order changes the SASS ptxas emits.
+template <Body B>
+__device__ __forceinline__ void sha_sched(uint32_t (&w)[16], int i, uint32_t one) {
+    const uint32_t w16 = w[i & 15], w7 = w[(i - 7) & 15], w15 = w[(i - 15) & 15], w2 = w[(i - 2) & 15];
+    if constexpr (B == Body::kDenseFused)
+        w[i & 15] = addf(addf(addf(w16, w7, one), lop3_bca<0x96>(rotr(w15, 7), rotr(w15, 18), w15 >> 3), one),
+                         lop3_bca<0x96>(rotr(w2, 17), rotr(w2, 19), w2 >> 10), one);
+    else if constexpr (B == Body::kDenseSha)
+        w[i & 15] = addf(addf(addf(w16, w7, one), SHA_s0(w15), one), SHA_s1(w2), one);
+    else
+        w[i & 15] = w16 + w7 + SHA_s0(w15) + SHA_s1(w2);
+}
 
-#ifndef B200H_ROLLED
-#define B200H_ROLLED 0
-#endif
-#ifndef B200H_ILV
-#define B200H_ILV 4
-#endif
-#ifndef B200H_PAIR_GATHER
-#define B200H_PAIR_GATHER 1
-#endif
-#ifndef B200H_OCTET_GATHER
-#define B200H_OCTET_GATHER 1
-#endif
-// SHA-256 round constants for rounds 16..63 (used by the rolled variant)
-__constant__ uint32_t kShaK[48] = {
-    0xe49b69c1u, 0xefbe4786u, 0x0fc19dc6u, 0x240ca1ccu, 0x2de92c6fu, 0x4a7484aau, 0x5cb0a9dcu, 0x76f988dau,
-    0x983e5152u, 0xa831c66du, 0xb00327c8u, 0xbf597fc7u, 0xc6e00bf3u, 0xd5a79147u, 0x06ca6351u, 0x14292967u,
-    0x27b70a85u, 0x2e1b2138u, 0x4d2c6dfcu, 0x53380d13u, 0x650a7354u, 0x766a0abbu, 0x81c2c92eu, 0x92722c85u,
-    0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u,
-    0x19a4c116u, 0x1e376c08u, 0x2748774cu, 0x34b0bcb5u, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u,
-    0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u, 0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u};
+// One MD5 step: a = b + rotl(a + FN(b, c, d) + x[k] + T, S).
+template <Body B, int FN, int S>
+__device__ __forceinline__ void md5_step(uint32_t& a, uint32_t b, uint32_t c, uint32_t d, uint32_t xk, uint32_t T,
+                                         uint32_t one) {
+    if constexpr (B == Body::kDenseFused) {
+        // as in sha_round: the last add fused with the rotate into one LEA.HI (64 per block), x + T a VIADD
+        const uint32_t t = addf(addf(a, xk + T, one), lop3<FN>(b, c, d), one);
+        a = add_rotl<S>(b, t);
+    } else if constexpr (B == Body::kMd5) {
+        // MD5 alone: the FMA pipe is the bottleneck (4 IMAD vs 2 ALU ops per step), so the 3-input sum goes back to
+        // the ALU pipe as one IADD3: per step ALU = LOP3 + IADD3 + SHF, FMA = (x + T) and (+ b).
+        const uint32_t xt = addf(xk, T, one);
+        a = addf(b, rotl(a + lop3<FN>(b, c, d) + xt, S), one);
+    } else {
+        static_assert(B == Body::kSparse, "no MD5 step in this body");
+        a = b + rotl(a + (xk + T) + lop3<FN>(b, c, d), S);
+    }
+}
 
 // The two hashes are independent dependency chains over the same 16 words, so their rounds are
 // interleaved at source level (4 SHA rounds : 4 MD5 steps) to give every warp two chains of ILP.
 template <bool DO_SHA, bool DO_MD5, bool SPARSE = false>
 __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], const uint32_t (&x)[16],
                                          bool is_last, uint32_t bits_lo, uint32_t bits_hi, uint32_t one) {
-    constexpr bool kPlainAdd = SPARSE;
+    //   instantiation <DO_SHA, DO_MD5, SPARSE>   SHA-256 round         MD5 step                   quad order
+    //   dense fused    <1, 1, 0>  kDenseFused    LEA.HI Sigma rotates  LEA.HI rotate-add          MD5 first
+    //   dense SHA-256  <1, 0, 0>  kDenseSha      IMAD.WIDE rotates     -                          -
+    //   MD5 only       <0, 1, 0>  kMd5           -                     IADD3 sum, IMAD x+T and +b -
+    //   sparse fused   <1, 1, 1>  kSparse        plain adds            plain adds                 SHA-256 first
+    //   sparse SHA-256 <1, 0, 1>  kSparse        plain adds            -                          -
+    // Every body expands the four schedule words of a quad of SHA-256 rounds ahead of its first round.
+    static_assert(DO_SHA || !SPARSE, "MD5 alone has no sparse body");
+    constexpr Body kBody = SPARSE ? Body::kSparse : !DO_SHA ? Body::kMd5 : DO_MD5 ? Body::kDenseFused : Body::kDenseSha;
     uint32_t w[16];
     uint32_t m14 = x[14], m15 = x[15];
-    // dense instantiations only: the sparse one leaves every add to ptxas, which fuses them itself
-    constexpr int kShaRot = SPARSE ? 0 : (DO_MD5 ? (B200H_FUSED_MIX & 3) : (B200H_SHAONLY_ROT));
-    constexpr bool kMd5Rot = DO_SHA && DO_MD5 && !SPARSE && (B200H_FUSED_MIX & 4);
-    constexpr bool kConstAdd = DO_SHA && DO_MD5 && !SPARSE && B200H_FUSED_CONST_ADD;
-    constexpr bool kFusedForm = DO_SHA && DO_MD5 && !SPARSE;  // the B200H_FUSED_* body forms apply
-    constexpr int kLopSha = kFusedForm ? B200H_FUSED_LOP_SHA : 0, kLopMd5 = kFusedForm ? B200H_FUSED_LOP_MD5 : 0;
-    constexpr int kSchedAhead = kFusedForm ? B200H_FUSED_SCHED : 4;
-    const uint32_t m29 = one << 29, m22 = one << 22;  // 2^29, 2^22 as run-time values (bit 2 of kShaRot)
-    (void)m29; (void)m22; (void)kMd5Rot; (void)kConstAdd;
     if (DO_SHA) {
 #pragma unroll
         for (int i = 0; i < 16; ++i) w[i] = bswap(x[i]);
@@ -380,135 +235,58 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
     uint32_t a = hs[0], b = hs[1], c = hs[2], d = hs[3], e = hs[4], f = hs[5], g = hs[6], h = hs[7];
     uint32_t A = hm[0], B = hm[1], C = hm[2], D = hm[3];
 
-    // kSchedAhead (B200H_FUSED_SCHED): W[i] is expanded in the quad's preamble (4), eight at a time (8) or in SCHED1
-    // just before its round (1)
-#define SCHED1(i) \
-    if (kSchedAhead == 1 && (i) >= 16) SHA_SCHED(w, (i));
-#define SHA4(i, k0, k1, k2, k3)                                                 \
-    if (DO_SHA) {                                                               \
-        if ((i) >= 16 && (kSchedAhead == 4 || (kSchedAhead == 8 && ((i)&7) == 0))) { \
-            SHA_SCHED(w, (i));                                                  \
-            SHA_SCHED(w, (i) + 1);                                              \
-            SHA_SCHED(w, (i) + 2);                                              \
-            SHA_SCHED(w, (i) + 3);                                              \
-        }                                                                       \
-        if ((i) >= 16 && kSchedAhead == 8 && ((i)&7) == 0) {                    \
-            SHA_SCHED(w, (i) + 4);                                              \
-            SHA_SCHED(w, (i) + 5);                                              \
-            SHA_SCHED(w, (i) + 6);                                              \
-            SHA_SCHED(w, (i) + 7);                                              \
-        }                                                                       \
-        if (((i)&7) == 0) {                                                     \
-            SCHED1(i) SHA_RND(a, b, c, d, e, f, g, h, k0, w[(i)&15]);           \
-            SCHED1((i) + 1) SHA_RND(h, a, b, c, d, e, f, g, k1, w[((i) + 1) & 15]); \
-            SCHED1((i) + 2) SHA_RND(g, h, a, b, c, d, e, f, k2, w[((i) + 2) & 15]); \
-            SCHED1((i) + 3) SHA_RND(f, g, h, a, b, c, d, e, k3, w[((i) + 3) & 15]); \
-        } else {                                                                \
-            SCHED1(i) SHA_RND(e, f, g, h, a, b, c, d, k0, w[(i)&15]);           \
-            SCHED1((i) + 1) SHA_RND(d, e, f, g, h, a, b, c, k1, w[((i) + 1) & 15]); \
-            SCHED1((i) + 2) SHA_RND(c, d, e, f, g, h, a, b, k2, w[((i) + 2) & 15]); \
-            SCHED1((i) + 3) SHA_RND(b, c, d, e, f, g, h, a, k3, w[((i) + 3) & 15]); \
-        }                                                                       \
+#define SHA4(i, k0, k1, k2, k3)                                               \
+    if constexpr (DO_SHA) {                                                   \
+        if ((i) >= 16) {                                                      \
+            sha_sched<kBody>(w, (i), one);                                    \
+            sha_sched<kBody>(w, (i) + 1, one);                                \
+            sha_sched<kBody>(w, (i) + 2, one);                                \
+            sha_sched<kBody>(w, (i) + 3, one);                                \
+        }                                                                     \
+        if (((i)&7) == 0) {                                                   \
+            sha_round<kBody>(a, b, c, d, e, f, g, h, k0, w[(i)&15], one);     \
+            sha_round<kBody>(h, a, b, c, d, e, f, g, k1, w[((i) + 1) & 15], one); \
+            sha_round<kBody>(g, h, a, b, c, d, e, f, k2, w[((i) + 2) & 15], one); \
+            sha_round<kBody>(f, g, h, a, b, c, d, e, k3, w[((i) + 3) & 15], one); \
+        } else {                                                              \
+            sha_round<kBody>(e, f, g, h, a, b, c, d, k0, w[(i)&15], one);     \
+            sha_round<kBody>(d, e, f, g, h, a, b, c, k1, w[((i) + 1) & 15], one); \
+            sha_round<kBody>(c, d, e, f, g, h, a, b, k2, w[((i) + 2) & 15], one); \
+            sha_round<kBody>(b, c, d, e, f, g, h, a, k3, w[((i) + 3) & 15], one); \
+        }                                                                     \
     }
 #define MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
-    if (DO_MD5) {                                               \
-        MD5_STEP(FN, A, B, C, D, x0, s0, t0);                   \
-        MD5_STEP(FN, D, A, B, C, x1, s1, t1);                   \
-        MD5_STEP(FN, C, D, A, B, x2, s2, t2);                   \
-        MD5_STEP(FN, B, C, D, A, x3, s3, t3);                   \
+    if constexpr (DO_MD5) {                                     \
+        md5_step<kBody, FN, s0>(A, B, C, D, x0, t0, one);       \
+        md5_step<kBody, FN, s1>(D, A, B, C, x1, t1, one);       \
+        md5_step<kBody, FN, s2>(C, D, A, B, x2, t2, one);       \
+        md5_step<kBody, FN, s3>(B, C, D, A, x3, t3, one);       \
     }
-
-    // B200H_ILV: interleave granularity of the two chains in source order (4 = 4 SHA rounds : 4 MD5 steps).
-#define SHA1(i, K)                                                                   \
-    if (DO_SHA) {                                                                    \
-        if ((i) >= 16) SHA_SCHED(w, (i));                                            \
-        if (((i)&7) == 0) SHA_RND(a, b, c, d, e, f, g, h, K, w[(i)&15])              \
-        else if (((i)&7) == 1) SHA_RND(h, a, b, c, d, e, f, g, K, w[(i)&15])         \
-        else if (((i)&7) == 2) SHA_RND(g, h, a, b, c, d, e, f, K, w[(i)&15])         \
-        else if (((i)&7) == 3) SHA_RND(f, g, h, a, b, c, d, e, K, w[(i)&15])         \
-        else if (((i)&7) == 4) SHA_RND(e, f, g, h, a, b, c, d, K, w[(i)&15])         \
-        else if (((i)&7) == 5) SHA_RND(d, e, f, g, h, a, b, c, K, w[(i)&15])         \
-        else if (((i)&7) == 6) SHA_RND(c, d, e, f, g, h, a, b, K, w[(i)&15])         \
-        else SHA_RND(b, c, d, e, f, g, h, a, K, w[(i)&15])                           \
-    }
-#define MD1(j, FN, xk, s, T)                                  \
-    if (DO_MD5) {                                             \
-        if ((j) == 0) MD5_STEP(FN, A, B, C, D, xk, s, T)      \
-        else if ((j) == 1) MD5_STEP(FN, D, A, B, C, xk, s, T) \
-        else if ((j) == 2) MD5_STEP(FN, C, D, A, B, xk, s, T) \
-        else MD5_STEP(FN, B, C, D, A, xk, s, T)               \
-    }
-#if B200H_ILV == 4
 #define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3)      \
-    if (kFusedForm && B200H_FUSED_MD5_FIRST) {                                         \
+    if constexpr (kBody == Body::kDenseFused) {                                        \
         MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) SHA4(i, k0, k1, k2, k3) \
     } else {                                                                           \
         SHA4(i, k0, k1, k2, k3) MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
     }
-#elif B200H_ILV == 40  // MD5 steps ahead of the SHA rounds of the same quad
-#define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
-    MD4(FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) SHA4(i, k0, k1, k2, k3)
-#elif B200H_ILV == 2
-#define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
-    SHA1(i, k0) SHA1((i) + 1, k1) MD1(0, FN, x0, s0, t0) MD1(1, FN, x1, s1, t1)     \
-    SHA1((i) + 2, k2) SHA1((i) + 3, k3) MD1(2, FN, x2, s2, t2) MD1(3, FN, x3, s3, t3)
-#else
-#define QUAD(i, k0, k1, k2, k3, FN, x0, x1, x2, x3, s0, s1, s2, s3, t0, t1, t2, t3) \
-    SHA1(i, k0) MD1(0, FN, x0, s0, t0) SHA1((i) + 1, k1) MD1(1, FN, x1, s1, t1)     \
-    SHA1((i) + 2, k2) MD1(2, FN, x2, s2, t2) SHA1((i) + 3, k3) MD1(3, FN, x3, s3, t3)
-#endif
 
-    QUAD(0, 0x428a2f98u, 0x71374491u, 0xb5c0fbcfu, 0xe9b5dba5u, MD5_F, x[0], x[1], x[2], x[3], 7, 12, 17, 22, 0xd76aa478u, 0xe8c7b756u, 0x242070dbu, 0xc1bdceeeu)
-    QUAD(4, 0x3956c25bu, 0x59f111f1u, 0x923f82a4u, 0xab1c5ed5u, MD5_F, x[4], x[5], x[6], x[7], 7, 12, 17, 22, 0xf57c0fafu, 0x4787c62au, 0xa8304613u, 0xfd469501u)
-    QUAD(8, 0xd807aa98u, 0x12835b01u, 0x243185beu, 0x550c7dc3u, MD5_F, x[8], x[9], x[10], x[11], 7, 12, 17, 22, 0x698098d8u, 0x8b44f7afu, 0xffff5bb1u, 0x895cd7beu)
-    QUAD(12, 0x72be5d74u, 0x80deb1feu, 0x9bdc06a7u, 0xc19bf174u, MD5_F, x[12], x[13], m14, m15, 7, 12, 17, 22, 0x6b901122u, 0xfd987193u, 0xa679438eu, 0x49b40821u)
-#if B200H_ROLLED
-    // Rounds 16..63 as three trips through one copy of the 16-round body (round constants from constant
-    // memory), MD5 rounds 2..4 selected per trip: halves the instruction footprint of the hot loop, which
-    // otherwise streams ~36 KB of code per block through the instruction caches.
-#pragma unroll 1
-    for (int it = 0; it < 3; ++it) {
-        const uint32_t* kk = kShaK + 16 * it;
-        SHA4(16, kk[0], kk[1], kk[2], kk[3])
-        SHA4(20, kk[4], kk[5], kk[6], kk[7])
-        SHA4(24, kk[8], kk[9], kk[10], kk[11])
-        SHA4(28, kk[12], kk[13], kk[14], kk[15])
-        if (it == 0) {
-            MD4(MD5_G, x[1], x[6], x[11], x[0], 5, 9, 14, 20, 0xf61e2562u, 0xc040b340u, 0x265e5a51u, 0xe9b6c7aau)
-            MD4(MD5_G, x[5], x[10], m15, x[4], 5, 9, 14, 20, 0xd62f105du, 0x02441453u, 0xd8a1e681u, 0xe7d3fbc8u)
-            MD4(MD5_G, x[9], m14, x[3], x[8], 5, 9, 14, 20, 0x21e1cde6u, 0xc33707d6u, 0xf4d50d87u, 0x455a14edu)
-            MD4(MD5_G, x[13], x[2], x[7], x[12], 5, 9, 14, 20, 0xa9e3e905u, 0xfcefa3f8u, 0x676f02d9u, 0x8d2a4c8au)
-        } else if (it == 1) {
-            MD4(MD5_H, x[5], x[8], x[11], m14, 4, 11, 16, 23, 0xfffa3942u, 0x8771f681u, 0x6d9d6122u, 0xfde5380cu)
-            MD4(MD5_H, x[1], x[4], x[7], x[10], 4, 11, 16, 23, 0xa4beea44u, 0x4bdecfa9u, 0xf6bb4b60u, 0xbebfbc70u)
-            MD4(MD5_H, x[13], x[0], x[3], x[6], 4, 11, 16, 23, 0x289b7ec6u, 0xeaa127fau, 0xd4ef3085u, 0x04881d05u)
-            MD4(MD5_H, x[9], x[12], m15, x[2], 4, 11, 16, 23, 0xd9d4d039u, 0xe6db99e5u, 0x1fa27cf8u, 0xc4ac5665u)
-        } else {
-            MD4(MD5_I, x[0], x[7], m14, x[5], 6, 10, 15, 21, 0xf4292244u, 0x432aff97u, 0xab9423a7u, 0xfc93a039u)
-            MD4(MD5_I, x[12], x[3], x[10], x[1], 6, 10, 15, 21, 0x655b59c3u, 0x8f0ccc92u, 0xffeff47du, 0x85845dd1u)
-            MD4(MD5_I, x[8], m15, x[6], x[13], 6, 10, 15, 21, 0x6fa87e4fu, 0xfe2ce6e0u, 0xa3014314u, 0x4e0811a1u)
-            MD4(MD5_I, x[4], x[11], x[2], x[9], 6, 10, 15, 21, 0xf7537e82u, 0xbd3af235u, 0x2ad7d2bbu, 0xeb86d391u)
-        }
-    }
-#else
-    QUAD(16, 0xe49b69c1u, 0xefbe4786u, 0x0fc19dc6u, 0x240ca1ccu, MD5_G, x[1], x[6], x[11], x[0], 5, 9, 14, 20, 0xf61e2562u, 0xc040b340u, 0x265e5a51u, 0xe9b6c7aau)
-    QUAD(20, 0x2de92c6fu, 0x4a7484aau, 0x5cb0a9dcu, 0x76f988dau, MD5_G, x[5], x[10], m15, x[4], 5, 9, 14, 20, 0xd62f105du, 0x02441453u, 0xd8a1e681u, 0xe7d3fbc8u)
-    QUAD(24, 0x983e5152u, 0xa831c66du, 0xb00327c8u, 0xbf597fc7u, MD5_G, x[9], m14, x[3], x[8], 5, 9, 14, 20, 0x21e1cde6u, 0xc33707d6u, 0xf4d50d87u, 0x455a14edu)
-    QUAD(28, 0xc6e00bf3u, 0xd5a79147u, 0x06ca6351u, 0x14292967u, MD5_G, x[13], x[2], x[7], x[12], 5, 9, 14, 20, 0xa9e3e905u, 0xfcefa3f8u, 0x676f02d9u, 0x8d2a4c8au)
-    QUAD(32, 0x27b70a85u, 0x2e1b2138u, 0x4d2c6dfcu, 0x53380d13u, MD5_H, x[5], x[8], x[11], m14, 4, 11, 16, 23, 0xfffa3942u, 0x8771f681u, 0x6d9d6122u, 0xfde5380cu)
-    QUAD(36, 0x650a7354u, 0x766a0abbu, 0x81c2c92eu, 0x92722c85u, MD5_H, x[1], x[4], x[7], x[10], 4, 11, 16, 23, 0xa4beea44u, 0x4bdecfa9u, 0xf6bb4b60u, 0xbebfbc70u)
-    QUAD(40, 0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, MD5_H, x[13], x[0], x[3], x[6], 4, 11, 16, 23, 0x289b7ec6u, 0xeaa127fau, 0xd4ef3085u, 0x04881d05u)
-    QUAD(44, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u, MD5_H, x[9], x[12], m15, x[2], 4, 11, 16, 23, 0xd9d4d039u, 0xe6db99e5u, 0x1fa27cf8u, 0xc4ac5665u)
-    QUAD(48, 0x19a4c116u, 0x1e376c08u, 0x2748774cu, 0x34b0bcb5u, MD5_I, x[0], x[7], m14, x[5], 6, 10, 15, 21, 0xf4292244u, 0x432aff97u, 0xab9423a7u, 0xfc93a039u)
-    QUAD(52, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u, MD5_I, x[12], x[3], x[10], x[1], 6, 10, 15, 21, 0x655b59c3u, 0x8f0ccc92u, 0xffeff47du, 0x85845dd1u)
-    QUAD(56, 0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u, MD5_I, x[8], m15, x[6], x[13], 6, 10, 15, 21, 0x6fa87e4fu, 0xfe2ce6e0u, 0xa3014314u, 0x4e0811a1u)
-    QUAD(60, 0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u, MD5_I, x[4], x[11], x[2], x[9], 6, 10, 15, 21, 0xf7537e82u, 0xbd3af235u, 0x2ad7d2bbu, 0xeb86d391u)
-#endif
-#undef SCHED1
+    QUAD(0, 0x428a2f98u, 0x71374491u, 0xb5c0fbcfu, 0xe9b5dba5u, kMd5F, x[0], x[1], x[2], x[3], 7, 12, 17, 22, 0xd76aa478u, 0xe8c7b756u, 0x242070dbu, 0xc1bdceeeu)
+    QUAD(4, 0x3956c25bu, 0x59f111f1u, 0x923f82a4u, 0xab1c5ed5u, kMd5F, x[4], x[5], x[6], x[7], 7, 12, 17, 22, 0xf57c0fafu, 0x4787c62au, 0xa8304613u, 0xfd469501u)
+    QUAD(8, 0xd807aa98u, 0x12835b01u, 0x243185beu, 0x550c7dc3u, kMd5F, x[8], x[9], x[10], x[11], 7, 12, 17, 22, 0x698098d8u, 0x8b44f7afu, 0xffff5bb1u, 0x895cd7beu)
+    QUAD(12, 0x72be5d74u, 0x80deb1feu, 0x9bdc06a7u, 0xc19bf174u, kMd5F, x[12], x[13], m14, m15, 7, 12, 17, 22, 0x6b901122u, 0xfd987193u, 0xa679438eu, 0x49b40821u)
+    QUAD(16, 0xe49b69c1u, 0xefbe4786u, 0x0fc19dc6u, 0x240ca1ccu, kMd5G, x[1], x[6], x[11], x[0], 5, 9, 14, 20, 0xf61e2562u, 0xc040b340u, 0x265e5a51u, 0xe9b6c7aau)
+    QUAD(20, 0x2de92c6fu, 0x4a7484aau, 0x5cb0a9dcu, 0x76f988dau, kMd5G, x[5], x[10], m15, x[4], 5, 9, 14, 20, 0xd62f105du, 0x02441453u, 0xd8a1e681u, 0xe7d3fbc8u)
+    QUAD(24, 0x983e5152u, 0xa831c66du, 0xb00327c8u, 0xbf597fc7u, kMd5G, x[9], m14, x[3], x[8], 5, 9, 14, 20, 0x21e1cde6u, 0xc33707d6u, 0xf4d50d87u, 0x455a14edu)
+    QUAD(28, 0xc6e00bf3u, 0xd5a79147u, 0x06ca6351u, 0x14292967u, kMd5G, x[13], x[2], x[7], x[12], 5, 9, 14, 20, 0xa9e3e905u, 0xfcefa3f8u, 0x676f02d9u, 0x8d2a4c8au)
+    QUAD(32, 0x27b70a85u, 0x2e1b2138u, 0x4d2c6dfcu, 0x53380d13u, kMd5H, x[5], x[8], x[11], m14, 4, 11, 16, 23, 0xfffa3942u, 0x8771f681u, 0x6d9d6122u, 0xfde5380cu)
+    QUAD(36, 0x650a7354u, 0x766a0abbu, 0x81c2c92eu, 0x92722c85u, kMd5H, x[1], x[4], x[7], x[10], 4, 11, 16, 23, 0xa4beea44u, 0x4bdecfa9u, 0xf6bb4b60u, 0xbebfbc70u)
+    QUAD(40, 0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, kMd5H, x[13], x[0], x[3], x[6], 4, 11, 16, 23, 0x289b7ec6u, 0xeaa127fau, 0xd4ef3085u, 0x04881d05u)
+    QUAD(44, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u, kMd5H, x[9], x[12], m15, x[2], 4, 11, 16, 23, 0xd9d4d039u, 0xe6db99e5u, 0x1fa27cf8u, 0xc4ac5665u)
+    QUAD(48, 0x19a4c116u, 0x1e376c08u, 0x2748774cu, 0x34b0bcb5u, kMd5I, x[0], x[7], m14, x[5], 6, 10, 15, 21, 0xf4292244u, 0x432aff97u, 0xab9423a7u, 0xfc93a039u)
+    QUAD(52, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u, kMd5I, x[12], x[3], x[10], x[1], 6, 10, 15, 21, 0x655b59c3u, 0x8f0ccc92u, 0xffeff47du, 0x85845dd1u)
+    QUAD(56, 0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u, kMd5I, x[8], m15, x[6], x[13], 6, 10, 15, 21, 0x6fa87e4fu, 0xfe2ce6e0u, 0xa3014314u, 0x4e0811a1u)
+    QUAD(60, 0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u, kMd5I, x[4], x[11], x[2], x[9], 6, 10, 15, 21, 0xf7537e82u, 0xbd3af235u, 0x2ad7d2bbu, 0xeb86d391u)
 #undef SHA4
 #undef MD4
-#undef SHA1
-#undef MD1
 #undef QUAD
 
     if (DO_SHA) {
@@ -522,24 +300,17 @@ __device__ __forceinline__ void compress(uint32_t (&hs)[8], uint32_t (&hm)[4], c
 
 // ------------------------------------------------------------------------------ lane_hash_kernel
 
-// CTAs per SM the lane kernel is compiled for.  H100 (100 000 x 256 KiB, kernel time): SHA-256 alone gains 5 % at 4 CTAs
-// (128 registers) over 5 (96).  The fused SHA-256 + MD5 kernel as it now stands (LEA.HI rotate+adds, uniform `one`)
-// runs 7 % faster at 4 CTAs, where it needs no spill, than at 5 (96 registers, 88 bytes of spill): 36.14 -> 33.70 ms on
-// an H100 80GB HBM3 at a 700 W power limit (DESIGN.md 6).  So the instantiations that compute SHA-256 get
-// B200H_LANE_MIN_CTAS_SHA, except the dense fused one, which has gone on to 3 (B200H_LANE_MIN_CTAS_FUSED below); MD5
-// alone, at 96 registers either way, keeps 5.
-#ifndef B200H_LANE_MIN_CTAS
-#define B200H_LANE_MIN_CTAS 5
-#endif
-#ifndef B200H_LANE_MIN_CTAS_SHA
-#define B200H_LANE_MIN_CTAS_SHA 4
-#endif
-// The dense fused instantiation on its own: at 3 CTAs (up to 168 registers; ptxas takes 158) its body reads fewer
-// vector registers and it ran 2.2 % faster than at 4 (128 registers) on an H100 at 700 W, and 3.1 % faster with the
-// B200H_FUSED_* defaults (DESIGN.md 6).  The SHA-256-only and sparse ones stay at B200H_LANE_MIN_CTAS_SHA.
-#ifndef B200H_LANE_MIN_CTAS_FUSED
-#define B200H_LANE_MIN_CTAS_FUSED 3
-#endif
+// CTAs per SM each lane-kernel instantiation is compiled for.  H100 (100 000 x 256 KiB, kernel time): SHA-256 alone
+// gains 5 % at 4 CTAs (128 registers) over 5 (96).  The fused SHA-256 + MD5 kernel with LEA.HI rotate+adds and a uniform
+// `one` runs 7 % faster at 4 CTAs, where it needs no spill, than at 5 (96 registers, 88 bytes of spill): 36.14 -> 33.70
+// ms on an H100 80GB HBM3 at a 700 W power limit (DESIGN.md 6).  So the instantiations that compute SHA-256 get 4,
+// except the dense fused one: at 3 CTAs (up to 168 registers; ptxas takes 158) its body reads fewer vector registers and
+// it ran 2.2 % faster than at 4 (128 registers) on an H100 at 700 W, and 3.1 % faster with its LOP3 operand order and
+// MD5-first quads (sha_round, DESIGN.md 6).  MD5 alone, at 96 registers either way, keeps 5.
+template <bool DO_SHA, bool DO_MD5, bool SPARSE>
+__host__ __device__ constexpr int lane_ctas_per_sm() {
+    return !DO_SHA ? 5 : (DO_MD5 && !SPARSE) ? 3 : 4;
+}
 constexpr int kLaneThreads = 128;  // 4 warps; every warp runs an independent TMA/mbarrier ring
 constexpr int kLaneWarps = kLaneThreads / 32;
 constexpr int kBPC = 2;     // 64-byte blocks per chunk (one bulk copy)
@@ -586,8 +357,7 @@ __device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
 // bound by its own issue rate (one instruction per two cycles), so the adds are left to ptxas (IADD3 / LEA fusion,
 // ~15 % fewer instructions per block) instead of being spread over the FMA pipe.
 template <bool DO_SHA, bool DO_MD5, bool SPARSE>
-__global__ void __launch_bounds__(kLaneThreads, DO_SHA ? (DO_MD5 && !SPARSE ? B200H_LANE_MIN_CTAS_FUSED : B200H_LANE_MIN_CTAS_SHA)
-                                                        : B200H_LANE_MIN_CTAS)
+__global__ void __launch_bounds__(kLaneThreads, lane_ctas_per_sm<DO_SHA, DO_MD5, SPARSE>())
 lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ off, const uint64_t* __restrict__ len,
                  uint32_t* __restrict__ ring, uint32_t ring_mask, int* __restrict__ qctl, const int* __restrict__ ctl,
                  uint32_t flags, int lanes_per_warp, uint32_t quantum, uint8_t* __restrict__ sha_out,
@@ -597,8 +367,8 @@ lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ 
     const int wib = threadIdx.x >> 5;
     const uint32_t lt_mask = (1u << lane) - 1u;
     uint8_t* ring_smem = smem + wib * kWarpSmem;
-    constexpr bool kOctetGather = (B200H_OCTET_GATHER != 0) && !DO_SHA && kBPC == 2;
-    constexpr bool kPairGather = (B200H_PAIR_GATHER != 0) && !(DO_SHA && DO_MD5) && !kOctetGather;
+    constexpr bool kOctetGather = !DO_SHA && kBPC == 2;
+    constexpr bool kPairGather = !(DO_SHA && DO_MD5) && !kOctetGather;
     const bool final = !(flags & F_NO_FINAL);
     const bool lane_on = lane < lanes_per_warp;
     if (flags & F_YIELD_CHAIN_SMS) {
@@ -966,18 +736,11 @@ __device__ __forceinline__ void load_block_words(const uint8_t* blk, uint32_t to
 // One SHA-256 round for the chain warp.  A lone warp issues at most one instruction every two cycles whatever
 // the pipe, so what counts here is the instruction count: the two three-input sums are IADD3s (14 instructions
 // per round instead of 16 with two-input IMAD adds: 2 049 -> 1 769 cycles per block, tools/chainbench.cu).
-#define CH_RND_FMA(a, b, c, d, e, f, g, h, WK)                                        \
-    {                                                                                 \
-        uint32_t t1 = ADD(ADD(ADD(h, WK), lop3<0xCA>(e, f, g)), SHA_S1(e));           \
-        uint32_t t2 = ADD(SHA_S0(a), lop3<0xE8>(a, b, c));                            \
-        d = ADD(d, t1);                                                               \
-        h = ADD(t1, t2);                                                              \
-    }
 #define CH_RND(a, b, c, d, e, f, g, h, WK)                                            \
     {                                                                                 \
-        const uint32_t hwk = ADD(h, WK);                                              \
+        const uint32_t hwk = addf(h, WK, one);                                        \
         const uint32_t t1 = hwk + lop3<0xCA>(e, f, g) + SHA_S1(e);                    \
-        d = ADD(d, t1);                                                               \
+        d = addf(d, t1, one);                                                         \
         h = t1 + SHA_S0(a) + lop3<0xE8>(a, b, c);                                     \
     }
 
@@ -1084,7 +847,6 @@ chain_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__
                   const uint32_t* __restrict__ chain_list, const int* __restrict__ qctl, uint32_t flags,
                   uint8_t* __restrict__ sha_out, uint8_t* __restrict__ md5_out, ChainState* __restrict__ st,
                   int resume, uint32_t one) {
-    constexpr bool kPlainAdd = false;  // ADD() inside CH_RND: the one off-path sum stays an IMAD
     const uint32_t n_chain = (uint32_t)qctl[3];
     if (blockIdx.x >= n_chain) return;  // entry e lives in CTA e % gridDim.x: this CTA has none
     if (threadIdx.x == 0) {  // tell lane CTAs that this SM is taken (F_YIELD_CHAIN_SMS), then that this CTA is resident
@@ -1847,7 +1609,8 @@ int launch_trim(const uint8_t* base, const uint64_t* off, const uint64_t* len, u
 
 
 // [sha+md5, sha, md5]; configure_kernels() replaces them with the occupancy the compiled kernels reach
-static int g_lane_ctas_per_sm[3] = {B200H_LANE_MIN_CTAS_FUSED, B200H_LANE_MIN_CTAS_SHA, B200H_LANE_MIN_CTAS};
+static int g_lane_ctas_per_sm[3] = {lane_ctas_per_sm<true, true, false>(), lane_ctas_per_sm<true, false, false>(),
+                                    lane_ctas_per_sm<false, true, false>()};
 
 // most long messages a second, lane-packed launch takes: one wave of lanes at one warp per SMSP
 uint32_t plan_long_cap() {

@@ -17,7 +17,7 @@ from modal_client_b200 import _lib
 
 FUSED_DENSE = "_ZN5b200h16lane_hash_kernelILb1ELb1ELb0E"
 # per 64-byte block with CUDA 12.9: 545 SHF + 416 LOP3 + 192 LEA.HI + 16 PRMT on the ALU pipe, 671 IMAD on the FMA
-# pipe, 10 others.  Each LEA.HI is a rotate fused with its add (B200H_FUSED_MIX): without them the body is 2 042.
+# pipe, 10 others.  Each LEA.HI is a rotate fused with its add (add_rotl): without them the body is 2 042.
 BODY_MAX = 1850
 ALU_MAX = 1169
 

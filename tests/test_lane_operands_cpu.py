@@ -4,7 +4,7 @@ Every add of that body but the round-constant ones is `addf` = IMAD x, one, y.  
 vector registers issues slower next to the ALU-pipe LOP3s and SHFs than one that reads `one` from a uniform register
 (tools/ubench.cu modes 7 and 25, DESIGN.md 5.1).  ptxas keeps `one` in a uniform register only while no IMAD of the
 kernel has an immediate addend, so the 128 round-constant adds (SHA-256's W + K, MD5's x + T) are plain adds, which it
-issues as VIADD (B200H_FUSED_CONST_ADD).  A toolkit or a source change that puts `one` back in a vector register, or
+issues as VIADD (sha_round / md5_step).  A toolkit or a source change that puts `one` back in a vector register, or
 turns those adds into ALU-pipe IADD3s, costs throughput without failing any digest test; this catches both."""
 import re
 from collections import Counter

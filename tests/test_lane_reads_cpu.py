@@ -17,8 +17,8 @@ from tests.test_lane_mix_cpu import FUSED_DENSE, _block_body, _kernel_sass, _opc
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
 from lane_sass_score import score_body  # noqa: E402
 
-# per 64-byte block, the body as built by default: 3 854 vector reads at 3 CTAs per SM with the B200H_FUSED_* defaults;
-# the form before (4 CTAs, 128 registers) read 3 882 and ran 3.1 % slower (DESIGN.md 5.1)
+# per 64-byte block, the body as built: 3 854 vector reads at 3 CTAs per SM with SHA-256's LOP3 operands in the order
+# (b, c, a) and MD5 steps first; the form before (4 CTAs, 128 registers) read 3 882 and ran 3.1 % slower (DESIGN.md 5.1)
 VREADS_MAX = 3860
 ALU = 1169  # 545 SHF + 416 LOP3 + 192 LEA.HI + 16 PRMT
 LEA_HI = 192

@@ -9,6 +9,13 @@
 namespace b200h {
 
 // round variants for the lone-warp chain: fewer instructions matter more than pipe placement at 0.5 instr/clk
+#define CH_RND_FMA(a, b, c, d, e, f, g, h, WK)                                                        \
+    {                                                                                                 \
+        const uint32_t t1 = addf(addf(addf(h, WK, one), lop3<0xCA>(e, f, g), one), SHA_S1(e), one);   \
+        const uint32_t t2 = addf(SHA_S0(a), lop3<0xE8>(a, b, c), one);                                \
+        d = addf(d, t1, one);                                                                         \
+        h = addf(t1, t2, one);                                                                        \
+    }
 #define CH_RND_PLAIN(a, b, c, d, e, f, g, h, WK)                                      \
     {                                                                                 \
         const uint32_t t1 = h + WK + lop3<0xCA>(e, f, g) + SHA_S1(e);                 \
@@ -17,10 +24,10 @@ namespace b200h {
     }
 #define CH_RND_DPRE(a, b, c, d, e, f, g, h, WK)                                       \
     {                                                                                 \
-        const uint32_t hwk = ADD(h, WK);                                              \
-        const uint32_t dh = ADD(d, hwk);                                              \
+        const uint32_t hwk = addf(h, WK, one);                                        \
+        const uint32_t dh = addf(d, hwk, one);                                        \
         const uint32_t cs = lop3<0xCA>(e, f, g) + SHA_S1(e);                          \
-        d = ADD(dh, cs);                                                              \
+        d = addf(dh, cs, one);                                                        \
         h = hwk + cs + SHA_S0(a) + lop3<0xE8>(a, b, c);                               \
     }
 
@@ -52,7 +59,6 @@ __global__ void __launch_bounds__(128) chain_bench(uint32_t* out, long long* cyc
     __shared__ __align__(16) uint32_t rows[32][68];  // 32 blocks of 64 W+K words (or 16 message words), padded
     for (int i = threadIdx.x; i < 32 * 68; i += blockDim.x) (&rows[0][0])[i] = seed * 2654435761u + i * 40503u;
     __syncthreads();
-    constexpr bool kPlainAdd = false;  // ADD() inside the CH_RND variants
     uint32_t hs[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
     uint32_t hm[4] = {0x67452301u, 0xefcdab89u, 0x98badcfeu, 0x10325476u};
     const long long t0 = clock64();

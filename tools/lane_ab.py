@@ -4,7 +4,8 @@ usage: python tools/lane_ab.py --variant NAME=SPEC [--variant NAME=SPEC ...] [--
                                [--build-dir DIR] [--build-only] [--json FILE]
 
 A SPEC is either a path to a built libb200hash.so (e.g. a build of another commit) or a list of -D defines (possibly
-empty) that the library is built with from this tree's sources, e.g. `default=` and `mix16=-DB200H_FUSED_MIX=16`.
+empty) that the library is built with from this tree's sources, e.g. `head=` and `parent=/tmp/parent/libb200hash.so`,
+or `trial=-DTRIAL_FORM` for a form under study put behind an `#if` in the source.
 Every build goes to --build-dir (default: a temporary directory), never into the tree, and is loaded through B200H_LIB.
 Rounds alternate the variants (the order flips every round, so a drift of the card's clock over the call does not
 favour one of them).  Each result line gives the median and min-max next to the card's name, power limit, median SM
@@ -25,8 +26,8 @@ from concurrent.futures import ThreadPoolExecutor
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "modal_client_b200", "csrc")
-SRCS = ["b200hash_kernels.cu", "b200hash_dedupe.cu", "b200hash_crc32.cu", "b200hash_api.cu", "b200blob_host.cpp",
-        "b200pack_copy.cpp"]
+SRCS = ["b200hash_kernels.cu", "b200hash_dedupe.cu", "b200hash_crc32.cu", "b200hash_stage.cu", "b200hash_api.cu",
+        "b200blob_host.cpp", "b200pack_copy.cpp"]  # the sources of modal_client_b200/csrc/Makefile
 NVFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC,-Wall,-mavx2",
            "-Xptxas", "-v"]  # the flags of modal_client_b200/csrc/Makefile
 FLAG_NAMES = {3: "sha256+md5", 1: "sha256", 2: "md5"}

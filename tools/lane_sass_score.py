@@ -1,10 +1,12 @@
 """tools/lane_sass_score.py -- rank equivalent forms of the dense fused lane kernel's block body from their SASS (CPU only).
 
-usage: python tools/lane_sass_score.py [--variant NAME=SPEC ...] [--build-dir DIR] [--jobs 4] [--json FILE]
+usage: python tools/lane_sass_score.py --variant NAME=SPEC [--variant NAME=SPEC ...] [--build-dir DIR] [--jobs 4]
+                                      [--json FILE]
 
-Every variant is a list of -D defines built from this tree's sources with the flags of tools/lane_ab.py (default: the
-B200H_FUSED_* / B200H_ILV / B200H_LANE_MIN_CTAS_FUSED grid below).  For each it prints, for the per-block body of
-lane_hash_kernel<true,true,false> (the block extraction of tests/test_lane_mix_cpu.py):
+A SPEC is what tools/lane_ab.py takes: a path to a built libb200hash.so (e.g. a build of another commit, or of this tree
+with the form under study edited in) or a list of -D defines (possibly empty) built from this tree's sources with
+lane_ab.py's flags.  For each variant it prints, for the per-block body of lane_hash_kernel<true,true,false> (the block
+extraction of tests/test_lane_mix_cpu.py):
   body     instructions in the body;  alu: SHF + LOP3 + LEA + PRMT (the ALU pipe);  lea: LEA.HI;  imad / viadd;
   regs     registers and spill bytes (stores + loads) of the kernel, from ptxas -v;  local: LDL/STL in the body;
   vreads   vector-register source reads: every R operand of an instruction (memory addresses included) except RZ,
@@ -34,19 +36,6 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 from lane_ab import build  # noqa: E402  (same sources and flags as the timed builds)
 from tests.test_lane_mix_cpu import _INSN, FUSED_DENSE, _block_body, _cuobjdump, _opcode  # noqa: E402
 
-GRID = {
-    "default": "",
-    **{f"s1o{a}_s0o{b}": f"-DB200H_FUSED_S1_OUT={a} -DB200H_FUSED_S0_OUT={b}"
-       for a in (6, 11, 25) for b in (2, 13, 22) if (a, b) != (6, 2)},
-    **{f"lopsha{p}": f"-DB200H_FUSED_LOP_SHA={p}" for p in range(1, 6)},
-    **{f"lopmd5{p}": f"-DB200H_FUSED_LOP_MD5={p}" for p in range(1, 6)},
-    "sched1": "-DB200H_FUSED_SCHED=1",
-    "sched8": "-DB200H_FUSED_SCHED=8",
-    "ilv40": "-DB200H_ILV=40",
-    "ilv2": "-DB200H_ILV=2",
-    "ilv1": "-DB200H_ILV=1",
-    "ctas3": "-DB200H_LANE_MIN_CTAS_FUSED=3",
-}
 _REG = re.compile(r"^-?\|?R(\d+)\|?(\.reuse)?")
 _MEMREG = re.compile(r"\bR(\d+)\b")
 
@@ -103,8 +92,13 @@ def score_body(body: list) -> dict:
     }
 
 
-def ptxas_info(log: str) -> dict:
-    """registers and spill bytes of the dense fused kernel, from the build's ptxas -v output."""
+def ptxas_info(lib: str) -> dict:
+    """registers and spill bytes of the dense fused kernel, from the ptxas -v output of lib's build: build.log next to
+    lib (a lane_ab.py build) or in the csrc/ beside it (the Makefile's)."""
+    d = os.path.dirname(lib)
+    log = next((p for p in (os.path.join(d, "build.log"), os.path.join(d, "csrc", "build.log")) if os.path.exists(p)), None)
+    if log is None:
+        raise SystemExit(f"no build.log for {lib}")
     lines = open(log).read().splitlines()
     for i, ln in enumerate(lines):
         if "Function properties for " + FUSED_DENSE in ln:
@@ -116,21 +110,21 @@ def ptxas_info(log: str) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-    ap.add_argument("--variant", action="append", metavar="NAME=SPEC", help="default: the built-in grid")
+    ap.add_argument("--variant", action="append", metavar="NAME=SPEC", required=True)
     ap.add_argument("--build-dir", default=None)
     ap.add_argument("--jobs", type=int, default=4)
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     if _cuobjdump() is None:
         raise SystemExit("cuobjdump not found")
-    variants = dict(v.split("=", 1) for v in args.variant) if args.variant else GRID
+    variants = dict(v.split("=", 1) for v in args.variant)
     build_dir = os.path.abspath(args.build_dir or tempfile.mkdtemp(prefix="lane_score_"))
     with ThreadPoolExecutor(max_workers=args.jobs) as ex:
         libs = dict(zip(variants, ex.map(lambda kv: build(kv[0], kv[1], build_dir), variants.items())))
     rows = {}
     for name, lib in libs.items():
         rows[name] = {**score_body(_block_body(fused_sass(lib))),
-                      **ptxas_info(os.path.join(os.path.dirname(lib), "build.log"))}
+                      **ptxas_info(lib)}
     cols = ["body", "alu", "lea", "imad", "viadd", "regs", "spill", "local", "vreads", "vdist", "bank3"]
     print("bank = register index mod 2 is an assumption (see the module docstring)")
     print(f"{'variant':>14} " + " ".join(f"{c:>6}" for c in cols) + "  defines")
