@@ -210,6 +210,26 @@ int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_
                               uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* h_dst,
                               uint64_t h_dst_bytes, const uint64_t* dst_offsets, void* cuda_stream);
 
+/* The inverse of b200h_copy_ranges_to_host: the bytes at h_src + src_offsets[i] are written to range i of files that
+ * live in device memory as many buffers, described as there (segs, file_first_seg, b200h_file_range; host arrays).
+ * h_src is what b200h_host_alloc returns (16-byte aligned); every src_offsets[i] must be a multiple of 16 and every
+ * source must lie inside h_src_bytes (sources may overlap).
+ * Every argument is checked before any work is enqueued, B200H_E_INVALID otherwise: the rules of the to-host entry for
+ * segs / file_first_seg / ranges, h_src page-locked host memory the context's device can reach
+ * (cudaPointerGetAttributes), source offsets aligned and in bounds, and no device byte written by two ranges (checked on
+ * the resolved device addresses: two files, or two segments of one file, may share a tensor).
+ * ONE kernel launch (load_ranges_kernel) per call whatever the number of ranges and segments, none when every range is
+ * empty.  The kernel reads h_src straight over PCIe, every source byte once, in aligned 16-byte loads that stay inside
+ * the 16-byte hull of the sources; device stores are full aligned 16-byte words except at the edges of a segment's part
+ * of a range and at one word per 64 KiB of source.  Device bytes of the segments outside every range are not written.
+ * The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream), as the to-host entry does: h_src must
+ * stay unchanged, and the device bytes are there, once the work enqueued on the stream has completed.
+ * Replaces: _read_file_into_fileobj (py/modal/volume.py:923-1000) writing a downloaded file into host memory, from
+ * which a checkpoint would then be copied to the device tensor by tensor. */
+int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, const void* h_src,
+                                uint64_t h_src_bytes, const uint64_t* src_offsets, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

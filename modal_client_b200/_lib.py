@@ -34,7 +34,7 @@ ABI_SYMBOLS = (
     "b200h_last_outlier_count", "b200h_hash_batch_device_hl", "b200h_combine_stats", "b200h_plan_sync_count",
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
-    "b200h_crc32_device", "b200h_copy_ranges_to_host",
+    "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host",
 )
 
 
@@ -112,6 +112,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_crc32_device.restype = i32
         L.b200h_copy_ranges_to_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
         L.b200h_copy_ranges_to_host.restype = i32
+        L.b200h_copy_ranges_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
+        L.b200h_copy_ranges_from_host.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -449,6 +451,24 @@ class Context:
                                                _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(dst.ctypes.data),
                                                dst.size, _np_ptr(offs) if len(rg) else None, stream or None)
         self._check(rc, "b200h_copy_ranges_to_host")
+
+    def copy_ranges_from_host(self, seg_ptrs, seg_lens, file_first_seg, ranges, src: np.ndarray, src_offsets,
+                              stream: int = 0) -> None:
+        """The inverse of ``copy_ranges_to_host``: ``src[src_offsets[i]:]`` (``src`` a uint8 array over page-locked
+        memory from ``host_alloc``, offsets multiples of 16) is written to range i = ``(file, offset, len)`` of files
+        made of device buffers; no device byte may belong to two ranges.  One kernel launch, only enqueued on
+        ``stream``: ``src`` must stay unchanged until that stream's work has completed."""
+        segs = _segments(seg_ptrs, seg_lens)
+        ffs, nfiles = _segment_args(file_first_seg)
+        rg = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 3)
+        offs = np.ascontiguousarray(src_offsets, dtype=np.uint64)
+        if offs.shape != (len(rg),):
+            raise ValueError("src_offsets needs one entry per range")
+        rc = self._L.b200h_copy_ranges_from_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
+                                                 nfiles, _np_ptr(rg) if len(rg) else None, len(rg),
+                                                 ctypes.c_void_p(src.ctypes.data), src.size,
+                                                 _np_ptr(offs) if len(rg) else None, stream or None)
+        self._check(rc, "b200h_copy_ranges_from_host")
 
     # -- files: stat + read + hash entirely inside the library (native reader threads, no mmap / Python I/O)
     @staticmethod

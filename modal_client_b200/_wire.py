@@ -129,6 +129,18 @@ except Exception:
 
 
 try:  # pragma: no cover
+    from modal_proto.api_pb2 import VolumeGetFile2Request  # type: ignore
+except Exception:
+
+    @dataclasses.dataclass
+    class VolumeGetFile2Request:  # type: ignore[no-redef]  (api.proto:3840-3845)
+        volume_id: str = ""
+        path: str = ""
+        start: int = 0
+        len: int = 0  # 0: to the end of the file
+
+
+try:  # pragma: no cover
     from modal_proto.api_pb2 import SharedVolumeGetFileRequest, SharedVolumePutFileRequest  # type: ignore
 except Exception:
 

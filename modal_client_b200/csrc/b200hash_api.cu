@@ -1384,20 +1384,18 @@ int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, 
     return 0;
 }
 
-int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
-                              uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* h_dst,
-                              uint64_t h_dst_bytes, const uint64_t* dst_offsets, void* cuda_stream) {
-    if (!ctx) return B200H_E_INVALID;
-    B200H_RANGE("b200h_copy_ranges_to_host");
-    std::lock_guard<std::mutex> lk(ctx->mu);
+// The file table of the range-copy entries (segs / file_first_seg as for b200h_hash_segment_parts_device), checked;
+// seg_start[s] = offset of segment s in its file, file_size[f].
+static int segment_files(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                         uint64_t nfiles, std::vector<uint64_t>& seg_start, std::vector<uint64_t>& file_size) {
     if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
     if (!file_first_seg) return fail(ctx, B200H_E_INVALID, "file_first_seg must not be NULL (it has nfiles + 1 entries)");
     if (file_first_seg[0] != 0) return fail(ctx, B200H_E_INVALID, "file_first_seg[0] must be 0");
     if (file_first_seg[nfiles] != nsegs) return fail(ctx, B200H_E_INVALID, "file_first_seg[nfiles] must equal nsegs");
     for (uint64_t f = 0; f < nfiles; ++f)
         if (file_first_seg[f + 1] < file_first_seg[f]) return fail(ctx, B200H_E_INVALID, "file_first_seg must not decrease");
-    // seg_start[s]: offset of segment s in its file; file_size[f]
-    std::vector<uint64_t> seg_start(nsegs), file_size(nfiles, 0);
+    seg_start.assign(nsegs, 0);
+    file_size.assign(nfiles, 0);
     for (uint64_t f = 0; f < nfiles; ++f)
         for (uint64_t s = file_first_seg[f]; s < file_first_seg[f + 1]; ++s) {
             if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
@@ -1405,6 +1403,48 @@ int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_
             seg_start[s] = file_size[f];
             file_size[f] += segs[s].len;
         }
+    return 0;
+}
+
+// The device's address of [h, h + bytes), or NULL unless it is page-locked host memory ctx's device can reach
+// (pageable memory would fault the kernels).  Needs cudaSetDevice(ctx->device).
+static void* pinned_device_pointer(b200h_ctx* ctx, const void* h, uint64_t bytes) {
+    void* d = nullptr;
+    for (const uint8_t* q : {(const uint8_t*)h, (const uint8_t*)h + (bytes ? bytes - 1 : 0)}) {
+        cudaPointerAttributes at;
+        const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess && at.type == cudaMemoryTypeHost &&
+                        cudaHostGetDevicePointer(&d, const_cast<void*>(h), 0) == cudaSuccess && d;
+        cudaGetLastError();
+        if (!ok) return nullptr;
+    }
+    return d;
+}
+
+// Calls piece(device address, offset in the host buffer, n) for every part of range r that lies in one segment, in
+// file order (the range lands at / comes from host offset `at`; r.len > 0 and within its file).
+static void range_pieces(const b200h_segment* segs, const std::vector<uint64_t>& seg_start, const uint64_t* file_first_seg,
+                         const b200h_file_range& r, uint64_t at,
+                         const std::function<void(uint64_t, uint64_t, uint64_t)>& piece) {
+    const uint64_t a = file_first_seg[r.file], b = file_first_seg[r.file + 1];
+    // the last segment of the file that starts at or before the range's first byte and is not empty
+    uint64_t s = std::upper_bound(seg_start.begin() + a, seg_start.begin() + b, r.offset) - seg_start.begin() - 1;
+    for (uint64_t done = 0; done < r.len; ++s) {
+        const uint64_t in = r.offset + done - seg_start[s];
+        if (in >= segs[s].len) continue;  // an empty segment
+        const uint64_t n = std::min(segs[s].len - in, r.len - done);
+        piece((uint64_t)(uintptr_t)segs[s].d_ptr + in, at + done, n);
+        done += n;
+    }
+}
+
+int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                              uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* h_dst,
+                              uint64_t h_dst_bytes, const uint64_t* dst_offsets, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_ranges_to_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    std::vector<uint64_t> seg_start, file_size;
+    if (int rc = segment_files(ctx, segs, nsegs, file_first_seg, nfiles, seg_start, file_size)) return rc;
     if (nranges && (!ranges || !dst_offsets)) return fail(ctx, B200H_E_INVALID, "ranges and dst_offsets must not be NULL");
     if (nranges && !h_dst) return fail(ctx, B200H_E_INVALID, "h_dst must not be NULL");
     if ((uintptr_t)h_dst & 15u) return fail(ctx, B200H_E_INVALID, "h_dst must be 16-byte aligned");
@@ -1428,16 +1468,10 @@ int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     if (nranges == 0) return 0;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     // the destination must be page-locked host memory the device can store to (pageable memory would fault the kernel)
-    void* d_dst = nullptr;
-    for (const uint8_t* q : {(const uint8_t*)h_dst, (const uint8_t*)h_dst + (h_dst_bytes ? h_dst_bytes - 1 : 0)}) {
-        cudaPointerAttributes at;
-        const bool ok = cudaPointerGetAttributes(&at, q) == cudaSuccess && at.type == cudaMemoryTypeHost &&
-                        cudaHostGetDevicePointer(&d_dst, h_dst, 0) == cudaSuccess && d_dst;
-        cudaGetLastError();
-        if (!ok)
-            return fail(ctx, B200H_E_INVALID,
-                        "h_dst is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
-    }
+    void* d_dst = pinned_device_pointer(ctx, h_dst, h_dst_bytes);
+    if (!d_dst)
+        return fail(ctx, B200H_E_INVALID,
+                    "h_dst is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
     for (uint64_t s = 0; s < nsegs; ++s)
         if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
             return fail(ctx, B200H_E_INVALID,
@@ -1450,17 +1484,9 @@ int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     for (uint64_t i = 0; i < nranges; ++i) {
         const b200h_file_range& r = ranges[i];
         if (!r.len) continue;
-        const uint64_t a = file_first_seg[r.file], b = file_first_seg[r.file + 1];
-        // the last segment of the file that starts at or before the range's first byte and is not empty
-        uint64_t s = std::upper_bound(seg_start.begin() + a, seg_start.begin() + b, r.offset) - seg_start.begin() - 1;
         const size_t first = pieces.size();
-        for (uint64_t done = 0; done < r.len; ++s) {
-            const uint64_t in = r.offset + done - seg_start[s];
-            if (in >= segs[s].len) continue;  // an empty segment
-            const uint64_t n = std::min(segs[s].len - in, r.len - done);
-            pieces.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in, dst_offsets[i] + done, n});
-            done += n;
-        }
+        range_pieces(segs, seg_start, file_first_seg, r, dst_offsets[i],
+                     [&](uint64_t dev, uint64_t host, uint64_t n) { pieces.push_back({dev, host, n}); });
         size_t p = first;
         for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
             const uint64_t n = std::min(kStageTileBytes, r.len - o), d = dst_offsets[i] + o;
@@ -1480,6 +1506,85 @@ int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tile_bytes, cudaMemcpyHostToDevice, st));
     CU_TRY(ctx, cudaMemcpyAsync(d_pieces, pieces.data(), bytes - tile_bytes, cudaMemcpyHostToDevice, st));
     ctx->launches += launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_dst, st);
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaFreeAsync(d_table, st));
+    return 0;
+}
+
+int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, const void* h_src,
+                                uint64_t h_src_bytes, const uint64_t* src_offsets, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_ranges_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    std::vector<uint64_t> seg_start, file_size;
+    if (int rc = segment_files(ctx, segs, nsegs, file_first_seg, nfiles, seg_start, file_size)) return rc;
+    if (nranges && (!ranges || !src_offsets)) return fail(ctx, B200H_E_INVALID, "ranges and src_offsets must not be NULL");
+    if (nranges && !h_src) return fail(ctx, B200H_E_INVALID, "h_src must not be NULL");
+    if ((uintptr_t)h_src & 15u) return fail(ctx, B200H_E_INVALID, "h_src must be 16-byte aligned");
+    uint64_t nonempty = 0;
+    for (uint64_t i = 0; i < nranges; ++i) {
+        const b200h_file_range& r = ranges[i];
+        const std::string name = "range " + std::to_string(i);
+        if (r.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
+        if (r.offset > file_size[r.file] || r.len > file_size[r.file] - r.offset)
+            return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
+        if (src_offsets[i] & 15u) return fail(ctx, B200H_E_INVALID, name + ": its source offset is not a multiple of 16");
+        if (src_offsets[i] > h_src_bytes || r.len > h_src_bytes - src_offsets[i])
+            return fail(ctx, B200H_E_INVALID, name + ": its source reaches past h_src_bytes");
+        nonempty += r.len != 0;
+    }
+    if (nranges == 0) return 0;
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    const void* d_src = pinned_device_pointer(ctx, h_src, h_src_bytes);
+    if (!d_src)
+        return fail(ctx, B200H_E_INVALID,
+                    "h_src is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
+    for (uint64_t s = 0; s < nsegs; ++s)
+        if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
+            return fail(ctx, B200H_E_INVALID,
+                        "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
+    if (!nonempty) return 0;
+
+    // pieces (range x segment, in source order within a range) and the tiles that read through them
+    std::vector<LoadPiece> pieces;
+    std::vector<LoadTile> tiles;
+    std::vector<uint64_t> range_of;  // per piece: the range it belongs to (for the overlap message)
+    for (uint64_t i = 0; i < nranges; ++i) {
+        const b200h_file_range& r = ranges[i];
+        if (!r.len) continue;
+        const size_t first = pieces.size();
+        range_pieces(segs, seg_start, file_first_seg, r, src_offsets[i], [&](uint64_t dev, uint64_t host, uint64_t n) {
+            pieces.push_back({host, dev, n});
+            range_of.push_back(i);
+        });
+        size_t p = first;
+        for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
+            const uint64_t n = std::min(kStageTileBytes, r.len - o), at = src_offsets[i] + o;
+            while (pieces[p].src + pieces[p].len <= at) ++p;
+            size_t q = p;
+            while (q + 1 < pieces.size() && pieces[q + 1].src < at + n) ++q;
+            tiles.push_back({at, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
+        }
+    }
+    // no device byte may be written twice: two files, or two segments of one file, may share a tensor
+    std::vector<size_t> by_dst(pieces.size());
+    for (size_t k = 0; k < by_dst.size(); ++k) by_dst[k] = k;
+    std::sort(by_dst.begin(), by_dst.end(), [&](size_t a, size_t b) { return pieces[a].dst < pieces[b].dst; });
+    for (size_t k = 1; k < by_dst.size(); ++k)
+        if (pieces[by_dst[k - 1]].dst + pieces[by_dst[k - 1]].len > pieces[by_dst[k]].dst)
+            return fail(ctx, B200H_E_INVALID, "ranges " + std::to_string(range_of[by_dst[k - 1]]) + " and " +
+                                                  std::to_string(range_of[by_dst[k]]) + " write the same device bytes");
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    // stream-ordered allocation, as b200h_copy_ranges_to_host: no synchronisation
+    const size_t tile_bytes = tiles.size() * sizeof(LoadTile), bytes = tile_bytes + pieces.size() * sizeof(LoadPiece);
+    void* d_table = nullptr;
+    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
+    LoadTile* d_tiles = (LoadTile*)d_table;
+    LoadPiece* d_pieces = (LoadPiece*)((uint8_t*)d_table + tile_bytes);
+    CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tile_bytes, cudaMemcpyHostToDevice, st));
+    CU_TRY(ctx, cudaMemcpyAsync(d_pieces, pieces.data(), bytes - tile_bytes, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_load_ranges(d_tiles, tiles.size(), d_pieces, d_src, st);
     CU_TRY(ctx, cudaGetLastError());
     CU_TRY(ctx, cudaFreeAsync(d_table, st));
     return 0;

@@ -120,6 +120,21 @@ constexpr uint64_t kStageTileBytes = 64 << 10;
 // Every tile's copy, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the device can store to.
 int launch_stage_ranges(const StageTile* tiles, uint64_t ntiles, const StagePiece* pieces, void* dst, cudaStream_t st);
 
+// The inverse: ranges of one source buffer copied into segmented device files (b200hash_stage.cu).  A load piece is
+// the part of a range that lands in one segment (len > 0); the pieces of a range are listed in source order.  A load
+// tile is up to kStageTileBytes of one range's source, starting at a multiple of 16; it writes through pieces
+// [first_piece, first_piece + npieces), every piece that holds one of its source bytes.
+struct LoadPiece {
+    uint64_t src, dst, len;  // byte offset in the source buffer; device address
+};
+struct LoadTile {
+    uint64_t src;  // byte offset in the source buffer
+    uint32_t len, npieces;
+    uint64_t first_piece;
+};
+// Every tile's copy, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device can load from.
+int launch_load_ranges(const LoadTile* tiles, uint64_t ntiles, const LoadPiece* pieces, const void* src, cudaStream_t st);
+
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)
 cudaError_t configure_kernels();  // one-time cudaFuncSetAttribute calls for the current device

@@ -1,5 +1,6 @@
 // b200hash_stage.cu -- copy byte ranges of segmented device files to one destination buffer with full-width stores:
-// the blocks of a checkpoint in HBM that a volume server reports missing, on their way to page-locked host memory.
+// the blocks of a checkpoint in HBM that a volume server reports missing, on their way to page-locked host memory;
+// and back (load_ranges_kernel, below): downloaded blocks from page-locked host memory into the tensors of a file.
 //
 //   stage_ranges_kernel  persistent CTAs take destination tiles (kStageTileBytes of one range's destination, the last
 //                        tile of a range may be shorter); every thread produces whole, 16-byte aligned destination
@@ -134,7 +135,117 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
     }
 }
 
+// ---- the inverse direction: page-locked host memory -> segmented device files
+//
+//   load_ranges_kernel   persistent CTAs whose warps take source tiles (kStageTileBytes of one range's source, the
+//                        last tile of a range may be shorter).  The work is organised by SOURCE because the source is
+//                        now on the far side of PCIe: every source byte crosses it exactly once, as part of one aligned
+//                        16-byte load issued by one lane (a warp's 32 lanes read 512 consecutive bytes per load).  A
+//                        repeated read of mapped host memory is never relied on to hit a cache.
+//
+// Lane k of a chunk holds source word w = (the tile's first word) + 32 * chunk + k and builds, for every piece, the
+// aligned destination word whose last source byte lies in word w: with r = (piece device address - piece source
+// offset) & 15, that word takes the 16 source bytes [16w - r, 16w + 16 - r), i.e. bytes 16 - r .. 15 of word w - 1
+// (from lane k - 1 through __shfl_up_sync, or carried over from the previous chunk's lane 31) and bytes 0 .. 15 - r of
+// word w, joined with shift_bytes.  Every source byte belongs to exactly one such word per piece.  The word is stored
+// whole when all 16 bytes lie inside the piece; only at a piece's edges, and at a tile's first word, whose word w - 1
+// was read by the warp that has the tile before (it stores those bytes as the extra lane one past its last word), is
+// it stored in narrower parts.  Device bytes outside the pieces are never written.  Loads stay inside the 16-byte
+// aligned hull of the tile's source bytes, which lies in the same page-locked allocation as the bytes themselves.
+
+constexpr int kLoadChunks = 4;  // 32-word chunks in flight per warp
+
+// bytes [lo, hi) of v (0 <= lo < hi <= 16) to the 16-byte aligned `out`
+__device__ __forceinline__ void store_bytes(uint8_t* out, uint4 v, uint32_t lo, uint32_t hi) {
+    if (lo == 0 && hi == 16) {
+        *reinterpret_cast<uint4*>(out) = v;
+        return;
+    }
+    for (uint32_t j = lo; j < hi; ++j) {
+        const uint32_t k = j >> 2, x = k == 0 ? v.x : k == 1 ? v.y : k == 2 ? v.z : v.w;
+        out[j] = (uint8_t)(x >> (8 * (j & 3)));
+    }
+}
+
+__device__ __forceinline__ uint4 shfl_up_word(uint4 v) {
+    return make_uint4(__shfl_up_sync(0xffffffffu, v.x, 1), __shfl_up_sync(0xffffffffu, v.y, 1),
+                      __shfl_up_sync(0xffffffffu, v.z, 1), __shfl_up_sync(0xffffffffu, v.w, 1));
+}
+
+__device__ __forceinline__ uint4 shfl_last_word(uint4 v) {
+    return make_uint4(__shfl_sync(0xffffffffu, v.x, 31), __shfl_sync(0xffffffffu, v.y, 31),
+                      __shfl_sync(0xffffffffu, v.z, 31), __shfl_sync(0xffffffffu, v.w, 31));
+}
+
+// The destination words of source word w (see above) for pieces pc[p .. n).  Source offsets are relative to the
+// tile's first byte `ts` (a tile is at most 64 KiB): base = 16 * (w - the tile's first word); only source bytes in
+// [lo, hi), the words this lane holds, are stored.  p is the lane's cursor: pieces that end before anything word w
+// could take are skipped.
+__device__ __forceinline__ void load_word_out(const LoadPiece* __restrict__ pc, uint32_t& p, uint32_t n, uint64_t ts,
+                                              int32_t base, uint4 prev, uint4 cur, int32_t lo, int32_t hi) {
+    const uint64_t at = ts + (uint32_t)base;
+    while (p < n && pc[p].src + pc[p].len + 15 <= at) ++p;
+    for (uint32_t q = p; q < n && pc[q].src < at + 16; ++q) {
+        const LoadPiece piece = pc[q];
+        const uint32_t r = (uint32_t)(piece.dst - piece.src) & 15u;
+        const int32_t s0 = base - (int32_t)r;
+        // the piece clipped to [base - 16, base + 16): it may begin in an earlier tile or end in a later one
+        const int32_t from = piece.src + 16 <= at ? base - 16 : (int32_t)(piece.src - ts);
+        const int32_t to = piece.src + piece.len >= at + 16 ? base + 16 : (int32_t)(piece.src + piece.len - ts);
+        const int32_t a = max(max(s0, from), lo), b = min(min(s0 + 16, to), hi);
+        if (a >= b) continue;
+        store_bytes(reinterpret_cast<uint8_t*>(piece.dst + (ts - piece.src) + (uint64_t)(int64_t)s0),
+                    r ? shift_bytes(prev, cur, 16 - r) : cur, (uint32_t)(a - s0), (uint32_t)(b - s0));
+    }
+}
+
+__global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
+    load_ranges_kernel(const LoadTile* __restrict__ tiles, uint64_t ntiles, const LoadPiece* __restrict__ pieces,
+                       const uint8_t* __restrict__ src) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint4* words = reinterpret_cast<const uint4*>(src);
+    const uint4 zero = make_uint4(0, 0, 0, 0);
+    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
+    for (uint64_t t = (uint64_t)blockIdx.x * (kStageThreads / 32) + (threadIdx.x >> 5); t < ntiles; t += nwarps) {
+        const LoadTile tile = tiles[t];
+        const LoadPiece* __restrict__ pc = pieces + tile.first_piece;
+        const uint4* tw = words + (tile.src >> 4);
+        const int32_t nw = (int32_t)((tile.len + 15) >> 4);
+        uint32_t p = 0;
+        uint4 carry = zero;
+        // the tile's words [0, nw) are loaded; lane nw loads nothing and stores what word nw - 1 gives the destination
+        // words that begin there and end in the next tile's first word
+        for (int32_t c = 0; c <= nw; c += 32 * kLoadChunks) {
+            uint4 v[kLoadChunks];
+#pragma unroll
+            for (int i = 0; i < kLoadChunks; ++i) {
+                const int32_t w = c + i * 32 + (int32_t)lane;
+                v[i] = w < nw ? __ldg(tw + w) : zero;
+            }
+#pragma unroll
+            for (int i = 0; i < kLoadChunks; ++i) {
+                const int32_t w = c + i * 32 + (int32_t)lane;
+                uint4 prev = shfl_up_word(v[i]);
+                if (lane == 0) prev = carry;
+                carry = shfl_last_word(v[i]);
+                if (w <= nw)
+                    load_word_out(pc, p, tile.npieces, tile.src, w * 16, prev, v[i], w > 0 ? w * 16 - 16 : 0,
+                                  w < nw ? w * 16 + 16 : w * 16);
+            }
+        }
+    }
+}
+
 }  // namespace
+
+int launch_load_ranges(const LoadTile* tiles, uint64_t ntiles, const LoadPiece* pieces, const void* src, cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t per_cta = kStageThreads / 32, ctas = (ntiles + per_cta - 1) / per_cta;
+    const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
+    load_ranges_kernel<<<(int)(ctas < cap ? ctas : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
+                                                                                static_cast<const uint8_t*>(src));
+    return 1;
+}
 
 int launch_stage_ranges(const StageTile* tiles, uint64_t ntiles, const StagePiece* pieces, void* dst, cudaStream_t st) {
     if (!ntiles) return 0;

@@ -22,7 +22,8 @@ them.
 ``stage_ranges(files, ranges, dst, dst_offsets)`` is the bulk route off the device: any byte ranges of any number of
 device files into a page-locked buffer with ONE ``b200h_copy_ranges_to_host`` call, after which the tensors are not
 needed for those bytes.  The volumefs2 uploader uses it for the missing blocks when it is given
-``device_staging_bytes``.
+``device_staging_bytes``.  ``load_ranges(files, ranges, src, src_offsets)`` is the way back: ranges of a page-locked
+buffer into the files' tensors with ONE ``b200h_copy_ranges_from_host`` call (``volume.read_file_into_device``).
 """
 from __future__ import annotations
 
@@ -99,6 +100,28 @@ class _TensorBytes:
         event = torch.cuda.Event()
         event.record(self.stream)
         return event.synchronize
+
+    def _after_current(self):
+        """Order this source's stream after everything the current stream holds now."""
+        import torch
+
+        self.stream.wait_stream(torch.cuda.current_stream(self.segments[0].device))
+
+    def _publish(self):
+        """Make the current stream wait for everything queued on this source's stream so far; -> a callable that blocks
+        until that work has completed."""
+        import torch
+
+        event = torch.cuda.Event()
+        event.record(self.stream)
+        torch.cuda.current_stream(self.segments[0].device).wait_event(event)
+        return event.synchronize
+
+    @classmethod
+    def _new_tensor(cls, shape, dtype, ctx):
+        import torch
+
+        return torch.empty(shape, dtype=dtype, device=f"cuda:{ctx.device}")
 
     @classmethod
     def _to_device(cls, data: bytes, ctx):
@@ -249,12 +272,7 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
             raise ValueError("ranges without files")
         return Staged(dst, [], None)
     lead = sources[0]
-    ptrs, lens, first = [], [], [0]
-    for src in sources:
-        lead._after(src)
-        ptrs += [s.data_ptr() if s.numel() else 0 for s in src.segments]
-        lens += [s.numel() for s in src.segments]
-        first.append(len(lens))
+    ptrs, lens, first = _file_table(sources)
     with lead._on_stream():
         ctx.copy_ranges_to_host(ptrs, lens, first, ranges, dst, offsets, lead.stream_handle)
         done = lead._mark()
@@ -262,6 +280,60 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
         with sources[f].lock:
             sources[f].bytes_to_host += n
     return Staged(dst, [(at, n) for at, (_, _, n) in zip(offsets, ranges)], done)
+
+
+def _file_table(sources: list[_TensorBytes]):
+    """(segment pointers, lengths, file_first_seg) of ``sources``, with the first one's stream ordered after the
+    others'."""
+    lead = sources[0]
+    ptrs, lens, first = [], [], [0]
+    for src in sources:
+        lead._after(src)
+        ptrs += [s.data_ptr() if s.numel() else 0 for s in src.segments]
+        lens += [s.numel() for s in src.segments]
+        first.append(len(lens))
+    return ptrs, lens, first
+
+
+class Loaded:
+    """Ranges of a page-locked host buffer on their way into device files (``load_ranges``)."""
+
+    def __init__(self, done):
+        self._done = done
+
+    def wait(self) -> None:
+        """Blocks until the copy has completed (call it through ``asyncio.to_thread`` from a coroutine).  Only from
+        then on may the host change the source buffer."""
+        if self._done is not None:
+            self._done()
+            self._done = None
+
+
+def load_ranges(files: list["DeviceFile"], ranges, src: np.ndarray, src_offsets, ctx=None) -> Loaded:
+    """Write ``src[src_offsets[i]:]`` -- ``src`` a uint8 array over page-locked memory from ``ctx.host_alloc``, offsets
+    multiples of 16 -- into range i = ``(index into files, offset, length)`` of device files; no device byte may belong
+    to two ranges.  The mirror of ``stage_ranges``: ONE ``b200h_copy_ranges_from_host`` call (one kernel launch),
+    enqueued on the first file's stream, which is ordered after every file's stream and after the current stream (the
+    tensors may have been read since the files were made; they are not overwritten before that work).  The current
+    stream then waits for the copy, so work enqueued on it later sees the bytes without a host synchronisation.
+    Returns at once; ``wait()`` on the result blocks until the kernel has read ``src``.  ``DeviceFile`` itself stays a
+    read-only file object: this is the one way bytes get into its tensors."""
+    ctx = ctx or get_context()
+    sources = [f._src for f in files]
+    ranges = [(int(f), int(o), int(n)) for f, o, n in ranges]
+    offsets = [int(o) for o in src_offsets]
+    if len(offsets) != len(ranges):
+        raise ValueError("src_offsets needs one entry per range")
+    if not sources:
+        if ranges:
+            raise ValueError("ranges without files")
+        return Loaded(None)
+    lead = sources[0]
+    lead._after_current()
+    ptrs, lens, first = _file_table(sources)
+    with lead._on_stream():
+        ctx.copy_ranges_from_host(ptrs, lens, first, ranges, src, offsets, lead.stream_handle)
+    return Loaded(lead._publish())  # outside the block: the caller's current stream is the one that waits
 
 
 # ------------------------------------------------------------------------------------------ safetensors
@@ -746,4 +818,5 @@ class DeviceFile(io.RawIOBase):
         return f"<DeviceFile {self._src.nbytes} bytes in {len(segs)} segments on {segs[0].device}>"
 
 
-__all__ = ["DeviceFile", "BOUNCE_BYTES", "Staged", "hash_parts_many", "safetensors_layout", "stage_ranges"]
+__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "Staged", "hash_parts_many", "load_ranges", "safetensors_layout",
+           "stage_ranges"]

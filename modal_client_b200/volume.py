@@ -13,14 +13,20 @@ uploader -- all of a batch's ``DeviceFile``s, safetensors images of whole state 
 host; the volumefs1 uploader reads it like any other stream.  Given ``device_staging_bytes`` of page-locked host memory,
 the volumefs2 uploader copies those blocks off the device in waves of one ``stage_ranges`` call each and PUTs them from
 there, so the tensors are free again (``device_released``) after the last copy instead of after the last PUT.
+
+The way back (counterparts of ``Volume.read_file`` / ``read_file_into_fileobj``, py/modal/volume.py:878-1000):
+``read_file`` and ``read_file_into_fileobj`` through host memory, ``read_file_into_device`` straight into the tensors
+of a ``DeviceFile`` (blocks downloaded into page-locked memory, a wave per ``load_ranges`` call), and
+``read_safetensors``, a safetensors checkpoint back into CUDA tensors without a host copy of the file.
 """
 from __future__ import annotations
 
 import asyncio
 import functools
+import json
 import os
 import time
-from collections.abc import Callable
+from collections.abc import Callable, Mapping
 from io import BytesIO
 from pathlib import Path, PurePosixPath
 from typing import Any, BinaryIO
@@ -29,10 +35,10 @@ import numpy as np
 
 from . import _wire, blob_utils
 from ._logging import logger
-from .async_utils import bounded_map, retry
+from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
-from .device_file import DeviceFile, stage_ranges
-from .exception import ExecutionError
+from .device_file import BOUNCE_BYTES, DeviceFile, _st_dtypes, load_ranges, stage_ranges
+from .exception import ExecutionError, ServiceError
 from .http_utils import ClientSessionRegistry
 
 VOLUME_PUT_FILE_CLIENT_TIMEOUT = 60 * 60  # seconds a single file may take to become visible (volume.py:79)
@@ -377,6 +383,292 @@ async def _put_missing_blocks(file_specs, missing_blocks, put_responses: dict[by
         for task in running:
             task.cancel()
         await asyncio.gather(*running, return_exceptions=True)
+
+
+# -------------------------------------------------------------------------------------------------- reads
+#
+# The read direction of volumefs2: ``VolumeGetFile2`` names the blocks that hold a byte range of a file, one GET URL
+# per block, the first one sliced from ``start % BLOCK_SIZE`` and the last one cut at the end of the range; the server
+# zero-pads a block that was stored trimmed, so every body has exactly its slice's length.
+
+
+async def _raise_on_block_response_error(response) -> None:
+    """An HTTP status >= 400 of a block GET as the reference reports it (py/modal/volume.py:82-99): 503 is a
+    ``ServiceError``, anything else an ``ExecutionError``."""
+    if response.status < 400:
+        return
+    try:
+        body = await response.text()
+    except Exception:
+        body = "<unavailable>"
+    if response.status == 503:
+        raise ServiceError(f"Service temporarily unavailable: {body}")
+    raise ExecutionError(f"Request failed with status {response.status} {response.reason}: {body}")
+
+
+async def _get_file2(client, volume_id: str, path: str, start: int = 0, length: int = 0):
+    try:
+        return await client.stub.VolumeGetFile2(_wire.VolumeGetFile2Request(volume_id=volume_id, path=path, start=start,
+                                                                             len=length))
+    except Exception as exc:
+        if type(exc).__name__ == "NotFoundError":
+            raise FileNotFoundError(exc.args[0] if exc.args else path)
+        raise
+
+
+async def read_file(client, volume_id: str, path: str):
+    """Async generator of the file's block bodies, in order (py/modal/volume.py:878-920): ``cpu_count`` blocks are
+    fetched ahead, each GET is retried (5 attempts, 0.1 s base delay).  A missing path raises ``FileNotFoundError``."""
+    response = await _get_file2(client, volume_id, path)
+
+    @retry(n_attempts=5, base_delay=0.1, attempt_timeout=None)
+    async def read_block(url: str) -> bytes:
+        async with ClientSessionRegistry.get_session().get(url) as get_response:
+            await _raise_on_block_response_error(get_response)
+            return await get_response.content.read()
+
+    async for body in bounded_map_ordered(list(response.get_urls), read_block, concurrency=os.cpu_count() or 1):
+        yield body
+
+
+async def read_file_into_fileobj(client, volume_id: str, path: str, fileobj: BinaryIO,
+                                 progress_cb: Callable[..., Any] | None = None, concurrency: int | None = None) -> int:
+    """Write the whole file into ``fileobj`` from its current position, ``concurrency`` (``cpu_count``) blocks at a
+    time, each at its place in the file (py/modal/volume.py:923-1000); -> the number of bytes written.  Leaves the
+    position behind the last byte.  ``progress_cb(advance=n)`` is called as bytes are written."""
+    progress_cb = progress_cb or (lambda *_, **__: None)
+    response = await _get_file2(client, volume_id, path)
+    semaphore = asyncio.Semaphore(concurrency or os.cpu_count() or 1)
+    write_lock = asyncio.Lock()
+    start_pos = fileobj.tell()
+
+    @retry(n_attempts=5, base_delay=0.1, attempt_timeout=None)
+    async def download_block(idx: int, url: str) -> int:
+        block_start_pos = start_pos + idx * blob_utils.BLOCK_SIZE
+        written = 0
+        async with semaphore, ClientSessionRegistry.get_session().get(url) as get_response:
+            await _raise_on_block_response_error(get_response)
+            async for chunk in get_response.content.iter_any():
+                async with write_lock:
+                    fileobj.seek(block_start_pos + written)
+                    fileobj.write(chunk)
+                progress_cb(advance=len(chunk))
+                written += len(chunk)
+        return written
+
+    total = sum(await asyncio.gather(*[download_block(i, url) for i, url in enumerate(response.get_urls)]))
+    fileobj.seek(start_pos + total)
+    return total
+
+
+async def _block_slices(client, volume_id: str, path: str, start: int, n: int) -> list[tuple[str, int, int]]:
+    """[(GET URL, offset in the range, length), ...] of bytes [start, start + n) of the file, n > 0: one
+    ``VolumeGetFile2`` call, whose answer is checked against the file's size and the block geometry before any GET."""
+    BS = blob_utils.BLOCK_SIZE
+    response = await _get_file2(client, volume_id, path, start, n)
+    if start + n > response.size:
+        raise ValueError(f"{path}: bytes [{start}, {start + n}) lie beyond the end of the file ({response.size} bytes)")
+    if response.len != n:
+        raise ExecutionError(f"{path}: asked for {n} bytes at {start}, the server answered with {response.len}")
+    first, last = start // BS, (start + n - 1) // BS
+    urls = list(response.get_urls)
+    if len(urls) != last - first + 1:
+        raise ExecutionError(f"{path}: bytes [{start}, {start + n}) span {last - first + 1} blocks, the server named "
+                             f"{len(urls)}")
+    out = []
+    for k, url in enumerate(urls):
+        lo, hi = max(start, (first + k) * BS), min(start + n, (first + k + 1) * BS)
+        out.append((url, lo - start, hi - lo))
+    return out
+
+
+@retry(n_attempts=5, base_delay=0.1, attempt_timeout=None)
+async def _fetch_block(url: str, out: np.ndarray, want: int, semaphore: asyncio.Semaphore) -> None:
+    """out[:want] = the body of one block GET, which must be exactly ``want`` bytes long.  A retry starts over in the
+    same place."""
+    got = 0
+    async with semaphore, ClientSessionRegistry.get_session().get(url) as response:
+        await _raise_on_block_response_error(response)
+        async for chunk in response.content.iter_any():
+            if got + len(chunk) > want:
+                raise ExecutionError(f"block GET returned more than the {want} bytes of its slice")
+            out[got : got + len(chunk)] = np.frombuffer(chunk, np.uint8)
+            got += len(chunk)
+    if got != want:
+        raise ExecutionError(f"block GET returned {got} bytes, its slice has {want}")
+
+
+async def _read_range_host(client, volume_id: str, path: str, start: int, n: int) -> bytes:
+    """Bytes [start, start + n) of the file, through host memory (small reads: a safetensors header)."""
+    if n == 0:
+        return b""
+    out = np.empty(n, np.uint8)
+    semaphore = asyncio.Semaphore(os.cpu_count() or 1)
+    await gather_cancel_on_error(*[_fetch_block(url, out[at : at + m], m, semaphore)
+                                   for url, at, m in await _block_slices(client, volume_id, path, start, n)])
+    return out.tobytes()
+
+
+async def read_file_into_device(client, volume_id: str, path: str, dst: DeviceFile, *, start: int = 0,
+                                staging_bytes: int = 256 << 20, concurrency: int | None = None,
+                                progress_cb: Callable[..., Any] | None = None) -> int:
+    """Fill ``dst`` (a ``DeviceFile``: its tensors are written in place) with bytes [start, start + dst.nbytes) of the
+    file; -> the number of bytes written.
+
+    One ``VolumeGetFile2`` call names the blocks; its answer must match the size of ``dst`` and the block geometry, else
+    this raises before any GET.  The blocks are fetched, ``concurrency`` (``cpu_count``) at a time, straight into slots
+    of ``staging_bytes`` of page-locked memory (``ctx.host_alloc``, freed however the call ends) taken in two halves:
+    when a half's wave of blocks is complete it goes to the device with one ``load_ranges`` call while the next wave
+    downloads into the other half, and a half is refilled only after its previous copy has read it.  Each block body
+    must have exactly its slice's length (the server zero-pads blocks that were stored trimmed), else
+    ``ExecutionError`` after the GET's retries.  ``staging_bytes`` must hold two blocks (``ValueError``).
+    On return the bytes are ordered before work enqueued later on the current stream.  If the call raises, ``dst``
+    holds partial content: some of its bytes are the file's, the others what they were."""
+    BS = blob_utils.BLOCK_SIZE
+    if staging_bytes < 2 * BS:
+        raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
+    progress_cb = progress_cb or (lambda *_, **__: None)
+    n = dst.nbytes
+    if n == 0:
+        await _get_file2(client, volume_id, path, start, 1)  # the file must exist; nothing else to do
+        return 0
+    slices = await _block_slices(client, volume_id, path, start, n)
+    per_half = staging_bytes // 2 // BS  # block slots per half (every slot starts at a multiple of BLOCK_SIZE)
+    semaphore = asyncio.Semaphore(concurrency or os.cpu_count() or 1)
+    ctx = blob_utils.get_context()
+    buf = ctx.host_alloc(2 * per_half * BS)
+    loaded: list = [None, None]
+    try:
+        for k, w in enumerate(range(0, len(slices), per_half)):
+            wave, half = slices[w : w + per_half], k & 1
+            if loaded[half] is not None:
+                await asyncio.to_thread(loaded[half].wait)  # the half's previous copy has read it
+                loaded[half] = None
+            at = [(half * per_half + i) * BS for i in range(len(wave))]
+
+            async def fetch(i: int, url: str, m: int, a: int):
+                await _fetch_block(url, buf[a : a + m], m, semaphore)
+                progress_cb(advance=m)
+
+            await gather_cancel_on_error(*[fetch(i, url, m, a) for i, ((url, _, m), a) in enumerate(zip(wave, at))])
+            loaded[half] = load_ranges([dst], [(0, off, m) for _, off, m in wave], buf, at, ctx=ctx)
+    finally:
+        for pending in loaded:  # the copies must have read the buffer before it is freed
+            if pending is not None:
+                await asyncio.to_thread(pending.wait)
+        ctx.host_free(buf)
+    return n
+
+
+def _safetensors_entries(header: bytes, data_len: int):
+    """[(name, torch dtype, torch shape, start, end), ...] in data order, checked as the safetensors library checks a
+    header (a valid JSON object, known dtype tags, ``shape x element size`` = span, ``data_offsets`` tiling the data
+    region of ``data_len`` bytes without holes or overlap); ``ValueError`` otherwise."""
+    try:
+        meta = json.loads(header.decode("utf-8"))
+    except (UnicodeDecodeError, ValueError) as exc:
+        raise ValueError(f"safetensors header is not valid JSON: {exc}") from None
+    if not isinstance(meta, dict):
+        raise ValueError("safetensors header is not a JSON object")
+    extra = meta.pop("__metadata__", None)
+    if extra is not None and not (isinstance(extra, dict) and all(isinstance(v, str) for v in extra.values())):
+        raise ValueError("safetensors __metadata__ must map str to str")
+    by_tag = {tag: dtype for dtype, (tag, _) in _st_dtypes().items()}
+    entries = []
+    for name, info in meta.items():
+        if not isinstance(info, dict) or set(info) != {"dtype", "shape", "data_offsets"}:
+            raise ValueError(f"safetensors header: {name!r} needs exactly dtype, shape and data_offsets")
+        tag, shape, offs = info["dtype"], info["shape"], info["data_offsets"]
+        if tag not in by_tag:
+            raise ValueError(f"safetensors header: {name!r} has dtype {tag!r}, which this torch cannot hold")
+        ints = lambda v: isinstance(v, list) and all(isinstance(x, int) and not isinstance(x, bool) and x >= 0 for x in v)  # noqa: E731
+        if not ints(shape) or not ints(offs) or len(offs) != 2:
+            raise ValueError(f"safetensors header: {name!r} has a malformed shape or data_offsets")
+        dtype, shape = by_tag[tag], list(shape)
+        if tag == "F4":  # the header counts 4-bit values, the torch dtype holds two per element
+            if not shape or shape[-1] % 2:
+                raise ValueError(f"safetensors header: {name!r} is F4 with an odd or missing last dimension")
+            shape[-1] //= 2
+        size = dtype.itemsize
+        for d in shape:
+            size *= d
+        if offs[1] < offs[0] or offs[1] - offs[0] != size:
+            raise ValueError(f"safetensors header: {name!r} spans {offs[1] - offs[0]} bytes, its shape and dtype "
+                             f"need {size}")
+        entries.append((name, dtype, shape, offs[0], offs[1]))
+    entries.sort(key=lambda e: (e[3], e[4]))
+    at = 0
+    for name, _, _, lo, hi in entries:
+        if lo != at:
+            raise ValueError(f"safetensors header: {name!r} starts at {lo}, the data before it ends at {at}")
+        at = hi
+    if at != data_len:
+        raise ValueError(f"safetensors header: the tensors cover {at} bytes of a {data_len}-byte data region")
+    return entries
+
+
+def _check_into(into: Mapping, entries, ctx) -> None:
+    """Every mismatch between ``into`` and the header, in one ``ValueError``."""
+    problems = []
+    want = {name: (dtype, shape) for name, dtype, shape, _, _ in entries}
+    for name in sorted(set(want) - set(into)):
+        problems.append(f"{name!r} is in the file but not in into")
+    for name in sorted(set(into) - set(want)):
+        problems.append(f"{name!r} is in into but not in the file")
+    spans = []
+    for name in sorted(set(want) & set(into)):
+        t, (dtype, shape) = into[name], want[name]
+        if t.dtype != dtype or list(t.shape) != shape:
+            problems.append(f"{name!r}: the file holds {dtype} {shape}, into has {t.dtype} {list(t.shape)}")
+            continue
+        try:
+            DeviceFile._Source._check_tensor(t, ctx, f"into[{name!r}]")
+        except ValueError as exc:
+            problems.append(str(exc))
+            continue
+        if t.numel():
+            spans.append((t.data_ptr(), t.data_ptr() + t.numel() * t.element_size(), name))
+    spans.sort()
+    for (_, hi, a), (lo, _, b) in zip(spans, spans[1:]):
+        if lo < hi:
+            problems.append(f"into[{a!r}] and into[{b!r}] overlap")
+    if problems:
+        raise ValueError("read_safetensors(into=...): " + "; ".join(problems))
+
+
+async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping | None = None,
+                           staging_bytes: int = 256 << 20) -> dict:
+    """The safetensors file at ``path`` as ``{name: tensor}`` on the context's device, equal to what
+    ``safetensors.torch.load`` gives for the file's bytes (same names, dtypes, shapes and values; keys in data order).
+
+    The 8-byte header length and the header come through host memory (two small ranged reads) and are checked as the
+    safetensors library checks them, ``ValueError`` before any tensor is allocated.  The tensors are ``torch.empty`` on
+    the context's device, or with ``into=`` the caller's tensors, filled in place: names, dtypes and shapes must match
+    exactly and the tensors must be contiguous, on the context's device and not overlap; every mismatch is listed in one
+    ``ValueError`` before any block GET.  The data region then arrives with one ``read_file_into_device`` into a
+    ``DeviceFile`` over the tensors in data order (``staging_bytes`` as there)."""
+    ctx = blob_utils.get_context()
+    size = (await _get_file2(client, volume_id, path, 0, 8)).size
+    if size < 8:
+        raise ValueError(f"{path} ({size} bytes) is too short to be a safetensors file")
+    n = int.from_bytes(await _read_range_host(client, volume_id, path, 0, 8), "little")
+    if n > _ST_MAX_HEADER:
+        raise ValueError(f"safetensors header of {n} bytes is larger than {_ST_MAX_HEADER}")
+    if 8 + n > size:
+        raise ValueError(f"safetensors header of {n} bytes does not fit a {size}-byte file")
+    entries = _safetensors_entries(await _read_range_host(client, volume_id, path, 8, n), size - 8 - n)
+    if into is not None:
+        _check_into(into, entries, ctx)
+        tensors = [into[name] for name, *_ in entries]
+    else:
+        tensors = [DeviceFile._Source._new_tensor(shape, dtype, ctx) for _, dtype, shape, _, _ in entries]
+    if entries and size - 8 - n:
+        dst = DeviceFile._over(DeviceFile._Source(tensors, BOUNCE_BYTES))
+        await read_file_into_device(client, volume_id, path, dst, start=8 + n, staging_bytes=staging_bytes)
+    return {name: t for (name, *_), t in zip(entries, tensors)}
+
+
+_ST_MAX_HEADER = 100_000_000  # the safetensors library's bound on the header length
 
 
 # ---------------------------------------------------------------------------------- the reference's names

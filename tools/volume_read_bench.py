@@ -1,0 +1,195 @@
+"""tools/volume_read_bench.py -- reading a checkpoint from a volume back into GPU memory.
+
+(a) kernel: a seeded safetensors-shaped state dict (VRB_GIB, default 2 GiB: four large bf16 matrices plus hundreds of
+    small norms and biases) as DeviceFile.safetensors; every 8 MiB block of the file, from one page-locked buffer
+    (block k at offset k * BLOCK_SIZE, as read_file_into_device lays a wave out), written with ONE
+    b200h_copy_ranges_from_host call, against ONE cudaMemcpyAsync of as many bytes from one aligned page-locked buffer
+    into one device buffer.  CUDA events, VRB_REPS (5) runs each, alternating, best and median; GB/s and the share of
+    the copy engine's figure.  The tensors are checked against the source afterwards.
+(b) end to end over LOOPBACK (an in-process aiohttp block server on 127.0.0.1: it measures the client, not a network):
+    a VRB_E2E_GIB (1 GiB) safetensors file uploaded once, then read_safetensors against the reference's route
+    (read_file_into_fileobj into BytesIO, safetensors.torch.load, .to("cuda") per tensor), alternating, VRB_E2E_REPS
+    (2) runs each; host clock from call to a synchronised result, and the peak growth of the process's resident set
+    during the call (sampled every 2 ms).  The results are compared tensor by tensor.
+
+The card name and power limit are read in the same run.  Needs a GPU: nothing here falls back.
+One JSON line per arm; also written to $VRB_OUT/volume_read_bench.json when set."""
+import asyncio
+import json
+import os
+import statistics
+import sys
+import threading
+import time
+import types
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import torch
+
+from modal_client_b200 import DeviceFile, _backend, _lib, blob_utils, load_ranges, volume
+from tests.volume_read_server import running_volume_server
+
+GiB, MiB = 1 << 30, 1 << 20
+
+
+def gpu_info() -> dict:
+    import subprocess
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
+    name, power, clock = [x.strip() for x in q.split(",")]
+    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
+
+
+def state_dict(total: int, seed: int = 0) -> dict:
+    """Four large bf16 matrices holding most of ``total`` bytes, plus 400 small norms / biases of odd sizes."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    sd = {}
+    for i in range(400):
+        n = 1000 + 37 * i
+        sd[f"layers.{i}.norm.weight"] = torch.randn(n, device="cuda", generator=g).to(torch.bfloat16)
+        if i % 2:
+            sd[f"layers.{i}.bias"] = torch.randn(n + 3, device="cuda", generator=g)
+    left = total - sum(t.numel() * t.element_size() for t in sd.values())
+    cols = 8192
+    for i in range(4):
+        rows = left // 4 // 2 // cols
+        sd[f"mat.{i}.weight"] = torch.randn(rows, cols, device="cuda", generator=g).to(torch.bfloat16)
+    return sd
+
+
+def events_ms(fn) -> float:
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    a.record()
+    fn()
+    b.record()
+    b.synchronize()
+    return a.elapsed_time(b)
+
+
+def kernel_arm(ctx, info, out):
+    BS = blob_utils.BLOCK_SIZE
+    sd = state_dict(int(float(os.environ.get("VRB_GIB", "2")) * GiB))
+    f = DeviceFile.safetensors(sd)
+    n = f.nbytes
+    ranges = [(0, o, min(BS, n - o)) for o in range(0, n, BS)]
+    offsets = [o for _, o, _ in ranges]
+    src = ctx.host_alloc(n)
+    try:
+        src[:] = torch.randint(0, 256, (n,), dtype=torch.uint8).numpy()
+        yard_src = torch.from_numpy(src.copy()).pin_memory()
+        yard_dst = torch.empty(n, dtype=torch.uint8, device="cuda")
+        times = {"load_ranges": [], "memcpy": []}
+        load = lambda: load_ranges([f], ranges, src, offsets, ctx=ctx)  # noqa: E731
+        load().wait()
+        yard_dst.copy_(yard_src, non_blocking=True)
+        for _ in range(int(os.environ.get("VRB_REPS", "5"))):
+            times["load_ranges"].append(events_ms(load))
+            times["memcpy"].append(events_ms(lambda: yard_dst.copy_(yard_src, non_blocking=True)))
+        torch.cuda.synchronize()
+        image = b"".join(s.cpu().numpy().tobytes() for s in f._src.segments)
+        ok = image == src.tobytes()
+        best = {k: min(v) for k, v in times.items()}
+        for arm, v in times.items():
+            out.append({"arm": f"kernel.{arm}", "bytes": n, "ranges": len(ranges), "tensors": len(sd),
+                        "best_ms": round(best[arm], 3), "median_ms": round(statistics.median(v), 3),
+                        "range_ms": [round(min(v), 3), round(max(v), 3)], "GB_s": round(n / best[arm] / 1e6, 2),
+                        "share_of_memcpy": round(best["memcpy"] / best[arm], 3), "bytes_equal": ok, **info})
+            print(json.dumps(out[-1]), flush=True)
+    finally:
+        torch.cuda.synchronize()
+        ctx.host_free(src)
+
+
+class PeakRss:
+    """Peak growth of the resident set while the block runs (sampled)."""
+
+    def __enter__(self):
+        self.base = self.peak = self._rss()
+        self.stop = threading.Event()
+        self.t = threading.Thread(target=self._run, daemon=True)
+        self.t.start()
+        return self
+
+    @staticmethod
+    def _rss() -> int:
+        with open("/proc/self/statm") as fh:
+            return int(fh.read().split()[1]) * os.sysconf("SC_PAGE_SIZE")
+
+    def _run(self):
+        while not self.stop.wait(0.002):
+            self.peak = max(self.peak, self._rss())
+
+    def __exit__(self, *exc):
+        self.stop.set()
+        self.t.join()
+        self.peak = max(self.peak, self._rss())
+        self.growth = self.peak - self.base
+
+
+async def e2e_arm(info, out):
+    import io
+
+    from safetensors.torch import load as st_load
+
+    sd = state_dict(int(float(os.environ.get("VRB_E2E_GIB", "1")) * GiB), seed=1)
+    async with running_volume_server(blob_utils.BLOCK_SIZE) as (stub, _):
+        client = types.SimpleNamespace(stub=stub)
+        batch = volume.VolumeUploadContextManager2("vo-b", client)
+        async with batch:
+            batch.put_file(DeviceFile.safetensors(sd), "/m.safetensors")
+        size = len(stub.volume_files["/m.safetensors"][0])
+
+        async def ours():
+            got = await volume.read_safetensors(client, "vo-b", "/m.safetensors")
+            torch.cuda.synchronize()
+            return got
+
+        async def reference_route():
+            buf = io.BytesIO()
+            await volume.read_file_into_fileobj(client, "vo-b", "/m.safetensors", buf)
+            host = st_load(buf.getvalue())
+            del buf
+            got = {k: v.to("cuda") for k, v in host.items()}
+            torch.cuda.synchronize()
+            return got
+
+        res = {"read_safetensors": [], "fileobj_load_to_cuda": []}
+        for _ in range(int(os.environ.get("VRB_E2E_REPS", "2"))):
+            for arm, fn in (("read_safetensors", ours), ("fileobj_load_to_cuda", reference_route)):
+                with PeakRss() as rss:
+                    t0 = time.perf_counter()
+                    got = await fn()
+                    dt = time.perf_counter() - t0
+                equal = sorted(got) == sorted(sd) and all(torch.equal(got[k].view(torch.uint8), sd[k].view(torch.uint8)) for k in sd)
+                del got
+                res[arm].append((dt, rss.growth, equal))
+        for arm, v in res.items():
+            ts = [t for t, _, _ in v]
+            out.append({"arm": f"e2e_loopback.{arm}", "bytes": size, "median_s": round(statistics.median(ts), 3),
+                        "range_s": [round(min(ts), 3), round(max(ts), 3)],
+                        "peak_rss_growth_GB": round(max(g for _, g, _ in v) / 1e9, 3),
+                        "tensors_equal": all(e for _, _, e in v), **info})
+            print(json.dumps(out[-1]), flush=True)
+
+
+def main():
+    if not torch.cuda.is_available():
+        raise SystemExit("volume_read_bench needs a GPU")
+    info = gpu_info()
+    ctx = _lib.Context(0, pinned_bytes=64 << 20, device_bytes=512 << 20)
+    _backend.set_context(ctx)
+    out = []
+    kernel_arm(ctx, info, out)
+    asyncio.run(e2e_arm(info, out))
+    if os.environ.get("VRB_OUT"):
+        os.makedirs(os.environ["VRB_OUT"], exist_ok=True)
+        with open(os.path.join(os.environ["VRB_OUT"], "volume_read_bench.json"), "w") as fh:
+            json.dump(out, fh, indent=1)
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
