@@ -441,16 +441,8 @@ class Context:
         ``dst``, a uint8 array over page-locked memory from ``host_alloc``: range i = ``(file, offset, len)`` lands at
         ``dst[dst_offsets[i]:]`` (offsets multiples of 16, destinations disjoint).  One kernel launch, only enqueued on
         ``stream``: ``dst`` holds the bytes once that stream's work has completed."""
-        segs = _segments(seg_ptrs, seg_lens)
-        ffs, nfiles = _segment_args(file_first_seg)
-        rg = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 3)
-        offs = np.ascontiguousarray(dst_offsets, dtype=np.uint64)
-        if offs.shape != (len(rg),):
-            raise ValueError("dst_offsets needs one entry per range")
-        rc = self._L.b200h_copy_ranges_to_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs), nfiles,
-                                               _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(dst.ctypes.data),
-                                               dst.size, _np_ptr(offs) if len(rg) else None, stream or None)
-        self._check(rc, "b200h_copy_ranges_to_host")
+        self._copy_ranges("b200h_copy_ranges_to_host", "dst_offsets", seg_ptrs, seg_lens, file_first_seg, ranges, dst,
+                          dst_offsets, stream)
 
     def copy_ranges_from_host(self, seg_ptrs, seg_lens, file_first_seg, ranges, src: np.ndarray, src_offsets,
                               stream: int = 0) -> None:
@@ -458,17 +450,21 @@ class Context:
         memory from ``host_alloc``, offsets multiples of 16) is written to range i = ``(file, offset, len)`` of files
         made of device buffers; no device byte may belong to two ranges.  One kernel launch, only enqueued on
         ``stream``: ``src`` must stay unchanged until that stream's work has completed."""
+        self._copy_ranges("b200h_copy_ranges_from_host", "src_offsets", seg_ptrs, seg_lens, file_first_seg, ranges, src,
+                          src_offsets, stream)
+
+    def _copy_ranges(self, entry: str, offsets_name: str, seg_ptrs, seg_lens, file_first_seg, ranges, host: np.ndarray,
+                     host_offsets, stream: int) -> None:
         segs = _segments(seg_ptrs, seg_lens)
         ffs, nfiles = _segment_args(file_first_seg)
         rg = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 3)
-        offs = np.ascontiguousarray(src_offsets, dtype=np.uint64)
+        offs = np.ascontiguousarray(host_offsets, dtype=np.uint64)
         if offs.shape != (len(rg),):
-            raise ValueError("src_offsets needs one entry per range")
-        rc = self._L.b200h_copy_ranges_from_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
-                                                 nfiles, _np_ptr(rg) if len(rg) else None, len(rg),
-                                                 ctypes.c_void_p(src.ctypes.data), src.size,
-                                                 _np_ptr(offs) if len(rg) else None, stream or None)
-        self._check(rc, "b200h_copy_ranges_from_host")
+            raise ValueError(f"{offsets_name} needs one entry per range")
+        rc = getattr(self._L, entry)(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs), nfiles,
+                                     _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(host.ctypes.data),
+                                     host.size, _np_ptr(offs) if len(rg) else None, stream or None)
+        self._check(rc, entry)
 
     # -- files: stat + read + hash entirely inside the library (native reader threads, no mmap / Python I/O)
     @staticmethod

@@ -25,7 +25,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <mutex>
 #include <new>
 #include <string>
@@ -792,16 +791,65 @@ uint64_t split_fixed_parts(uint64_t len, uint64_t part_len, std::vector<uint64_t
     return nparts;
 }
 
+// The file table of the segmented entry points: file f is the concatenation of segments
+// [file_first_seg[f], file_first_seg[f + 1]), segment s holding seg_lens[s] bytes (both arrays the caller's).
+struct FileTable {
+    const uint64_t* seg_lens;
+    const uint64_t* file_first_seg;
+    std::vector<uint64_t> seg_start;  // offset of every segment in its file
+    std::vector<uint64_t> size;       // bytes of every file
+};
+
+// Checks the table and fills `t`; returns 0, or B200H_E_INVALID with the reason in `err` (no context needed, so
+// b200h_segment_parts_preview runs it without a GPU).
+int file_table(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles, FileTable& t,
+               std::string& err) {
+    if (nsegs && !seg_lens) return err = "segments must not be NULL", B200H_E_INVALID;
+    if (!file_first_seg) return err = "file_first_seg must not be NULL (it has nfiles + 1 entries)", B200H_E_INVALID;
+    if (file_first_seg[0] != 0) return err = "file_first_seg[0] must be 0", B200H_E_INVALID;
+    if (file_first_seg[nfiles] != nsegs) return err = "file_first_seg[nfiles] must equal nsegs", B200H_E_INVALID;
+    for (uint64_t f = 0; f < nfiles; ++f)
+        if (file_first_seg[f + 1] < file_first_seg[f]) return err = "file_first_seg must not decrease", B200H_E_INVALID;
+    t.seg_lens = seg_lens;
+    t.file_first_seg = file_first_seg;
+    t.seg_start.assign(nsegs, 0);
+    t.size.assign(nfiles, 0);
+    for (uint64_t f = 0; f < nfiles; ++f)
+        for (uint64_t s = file_first_seg[f]; s < file_first_seg[f + 1]; ++s) {
+            if (t.size[f] + seg_lens[s] < t.size[f]) return err = "a file is larger than 2^64 - 1 bytes", B200H_E_INVALID;
+            t.seg_start[s] = t.size[f];
+            t.size[f] += seg_lens[s];
+        }
+    return 0;
+}
+
+// Calls piece(segment, offset in the segment, n) for every segment that holds some of the bytes
+// [offset, offset + len) of file `file`, in file order; empty segments yield no piece.  len > 0, inside the file.
+template <class Piece>
+void file_pieces(const FileTable& t, uint64_t file, uint64_t offset, uint64_t len, Piece&& piece) {
+    const uint64_t* start = t.seg_start.data();
+    // the last segment of the file that starts at or before the first byte (it is not empty: offset < the file's size)
+    uint64_t s = std::upper_bound(start + t.file_first_seg[file], start + t.file_first_seg[file + 1], offset) - start - 1;
+    for (uint64_t done = 0; done < len; ++s) {
+        const uint64_t in = offset + done - start[s];
+        if (in >= t.seg_lens[s]) continue;  // an empty segment
+        const uint64_t n = std::min(t.seg_lens[s] - in, len - done);
+        piece(s, in, n);
+        done += n;
+    }
+}
+
 constexpr uint64_t kInPlace = ~0ull;
 
 // Where every part of a segmented batch is hashed: b200h_segment_parts_preview reports it, and
-// b200h_hash_segment_parts_device builds its tables from it.  File f is the concatenation of segments
-// [file_first_seg[f], file_first_seg[f + 1]); its parts are cut by split_fixed_parts and listed file-major.  A part
-// that lies inside one segment is hashed where it is; a part that spans two or more segments is gathered into a wave
-// slot at the next multiple of 16.  Waves are contiguous ranges of parts: a new wave starts at the gathered part that
-// would take the current wave's staging beyond wave_cap (a wave always takes its first gathered part, so a part larger
-// than wave_cap gets a wave of its own).  Parts without a gathered part between them share a wave.
+// b200h_hash_segment_parts_device builds its tables from it.  The parts of every file of the table are cut by
+// split_fixed_parts and listed file-major.  A part that lies inside one segment is hashed where it is; a part that spans
+// two or more segments is gathered into a wave slot at the next multiple of 16.  Waves are contiguous ranges of parts:
+// a new wave starts at the gathered part that would take the current wave's staging beyond wave_cap (a wave always
+// takes its first gathered part, so a part larger than wave_cap gets a wave of its own).  Parts without a gathered part
+// between them share a wave.
 struct SegmentParts {
+    std::vector<uint64_t> file;      // the file of every part
     std::vector<uint64_t> off, len;  // part i: bytes [off[i], off[i] + len[i]) of its file
     std::vector<uint64_t> seg;       // the segment holding the part's first byte
     std::vector<uint64_t> seg_off;   // offset of that byte inside the segment
@@ -812,31 +860,21 @@ struct SegmentParts {
 };
 
 // Fills `p`; returns 0, or B200H_E_INVALID with the reason in `err`.
-int layout_segment_parts(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
-                         uint64_t part_len, uint64_t wave_cap, SegmentParts& p, std::string& err) {
+int layout_segment_parts(const FileTable& t, uint64_t part_len, uint64_t wave_cap, SegmentParts& p, std::string& err) {
     if (part_len == 0) return err = "part_len must be > 0", B200H_E_INVALID;
     if (wave_cap == 0) return err = "wave_bytes must be > 0", B200H_E_INVALID;
-    if (nsegs && !seg_lens) return err = "segments must not be NULL", B200H_E_INVALID;
-    if (!file_first_seg) return err = "file_first_seg must not be NULL (it has nfiles + 1 entries)", B200H_E_INVALID;
-    if (file_first_seg[0] != 0) return err = "file_first_seg[0] must be 0", B200H_E_INVALID;
-    if (file_first_seg[nfiles] != nsegs) return err = "file_first_seg[nfiles] must equal nsegs", B200H_E_INVALID;
-    for (uint64_t f = 0; f < nfiles; ++f)
-        if (file_first_seg[f + 1] < file_first_seg[f]) return err = "file_first_seg must not decrease", B200H_E_INVALID;
-    for (uint64_t f = 0; f < nfiles; ++f) {
-        const uint64_t a = file_first_seg[f], b = file_first_seg[f + 1];
-        uint64_t size = 0;
-        for (uint64_t s = a; s < b; ++s) {
-            if (size + seg_lens[s] < size) return err = "a file is larger than 2^64 - 1 bytes", B200H_E_INVALID;
-            size += seg_lens[s];
-        }
+    for (uint64_t f = 0; f < t.size.size(); ++f) {
         const size_t first = p.off.size();
-        split_fixed_parts(size, part_len, p.off, p.len);
-        uint64_t s = a, s_start = 0;  // segment s holds file bytes [s_start, s_start + seg_lens[s])
+        split_fixed_parts(t.size[f], part_len, p.off, p.len);
         for (size_t i = first; i < p.off.size(); ++i) {
-            while (s_start + seg_lens[s] <= p.off[i]) s_start += seg_lens[s++];  // skips empty segments too
-            p.seg.push_back(s);
-            p.seg_off.push_back(p.off[i] - s_start);
-            p.stage.push_back(p.off[i] + p.len[i] <= s_start + seg_lens[s] ? kInPlace : 0);
+            uint64_t npieces = 0;
+            file_pieces(t, f, p.off[i], p.len[i], [&](uint64_t s, uint64_t in, uint64_t) {
+                if (npieces++) return;
+                p.seg.push_back(s);
+                p.seg_off.push_back(in);
+            });
+            p.file.push_back(f);
+            p.stage.push_back(npieces == 1 ? kInPlace : 0);
         }
     }
     const uint64_t nparts = p.off.size();
@@ -866,6 +904,7 @@ int layout_segment_parts(const uint64_t* seg_lens, uint64_t nsegs, const uint64_
 
 // A pointer that is not memory of ctx's device would fault the kernels, so every device range an entry point takes is
 // checked before anything is enqueued: its first and last byte (the allocation in between is the caller's promise).
+// Needs cudaSetDevice(ctx->device).
 bool device_range_ok(b200h_ctx* ctx, const void* ptr, uint64_t len) {
     if (!len) return true;
     for (const uint8_t* q : {(const uint8_t*)ptr, (const uint8_t*)ptr + (len - 1)}) {
@@ -878,6 +917,50 @@ bool device_range_ok(b200h_ctx* ctx, const void* ptr, uint64_t len) {
     return true;
 }
 
+// Every segment an entry point takes, checked before anything is enqueued: not NULL when it has bytes, not wrapping the
+// address space, and device_range_ok.  `noun` names a segment in the message.  Needs cudaSetDevice(ctx->device).
+int segments_on_device(b200h_ctx* ctx, const b200h_segment* segs, uint64_t n, const char* noun) {
+    for (uint64_t i = 0; i < n; ++i) {
+        const uintptr_t p = (uintptr_t)segs[i].d_ptr;
+        std::string fault;
+        if (segs[i].len && !p) fault = " is NULL";
+        else if (p + segs[i].len < p) fault = " wraps the address space";
+        else if (!device_range_ok(ctx, segs[i].d_ptr, segs[i].len))
+            fault = " is not device memory on cuda:" + std::to_string(ctx->device);
+        if (!fault.empty()) return fail(ctx, B200H_E_INVALID, noun + (" " + std::to_string(i)) + fault);
+    }
+    return 0;
+}
+
+// The file table of segs[0 .. nsegs) (see file_table); `seg_lens` receives their lengths and backs t.seg_lens.
+int segment_file_table(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                       uint64_t nfiles, std::vector<uint64_t>& seg_lens, FileTable& t) {
+    seg_lens.resize(segs ? nsegs : 0);
+    for (uint64_t s = 0; s < seg_lens.size(); ++s) seg_lens[s] = segs[s].len;
+    std::string err;
+    if (int rc = file_table(segs ? seg_lens.data() : nullptr, nsegs, file_first_seg, nfiles, t, err))
+        return fail(ctx, rc, err);
+    return 0;
+}
+
+// Uploads the tables a and b (in that order) into one stream-ordered allocation on `st`, runs launch(device a,
+// device b) and frees the allocation behind it: no synchronisation, and no scratch shared with other streams' calls.
+template <class A, class B, class Launch>
+int launch_with_tables(b200h_ctx* ctx, cudaStream_t st, const std::vector<A>& a, const std::vector<B>& b,
+                       Launch&& launch) {
+    const size_t a_bytes = a.size() * sizeof(A), bytes = a_bytes + b.size() * sizeof(B);
+    void* d_table = nullptr;
+    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
+    A* d_a = (A*)d_table;
+    B* d_b = (B*)((uint8_t*)d_table + a_bytes);
+    CU_TRY(ctx, cudaMemcpyAsync(d_a, a.data(), a_bytes, cudaMemcpyHostToDevice, st));
+    CU_TRY(ctx, cudaMemcpyAsync(d_b, b.data(), bytes - a_bytes, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch(d_a, d_b);
+    CU_TRY(ctx, cudaGetLastError());
+    CU_TRY(ctx, cudaFreeAsync(d_table, st));
+    return 0;
+}
+
 // b200h_hash_segment_parts_device with ctx->mu held, on stream `st`.  d_etag_msg != NULL (b200h_hash_fixed_parts_device):
 // two more words, the ETag message {0, nparts * 16}, ride the part-table upload, even when there are no parts, and
 // *d_etag_msg points at them.
@@ -887,25 +970,19 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
     if (((uintptr_t)d_sha256 | (uintptr_t)d_md5) & 15u)
         return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
-    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
-    std::vector<uint64_t> seg_lens(nsegs);
-    for (uint64_t s = 0; s < nsegs; ++s) {
-        if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
-        seg_lens[s] = segs[s].len;
-    }
+    std::vector<uint64_t> seg_lens;
+    FileTable t;
+    if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
+    // before the layout, whose part list the segments' lengths size
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
     SegmentParts p;
     std::string err;
-    if (int rc = layout_segment_parts(seg_lens.data(), nsegs, file_first_seg, nfiles, part_len,
-                                      std::max(ctx->dwave_cap, ctx->dwave_want), p, err))
+    if (int rc = layout_segment_parts(t, part_len, std::max(ctx->dwave_cap, ctx->dwave_want), p, err))
         return fail(ctx, rc, err);
     const uint64_t nparts = p.off.size();
     if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
         return fail(ctx, B200H_E_INVALID, "flags select neither SHA256 nor MD5");
-    CU_TRY(ctx, cudaSetDevice(ctx->device));
-    for (uint64_t s = 0; s < nsegs; ++s)
-        if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
-            return fail(ctx, B200H_E_INVALID,
-                        "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
     if (nparts_out) *nparts_out = nparts;
     if (nparts == 0 && !d_etag_msg) return 0;
     uint64_t stage_max = 0;
@@ -929,16 +1006,13 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
                 continue;
             }
             table[i] = (uint64_t)(uintptr_t)(slot + p.stage[i]);
-            uint64_t s = p.seg[i], so = p.seg_off[i], done = 0;
-            while (done < p.len[i]) {
-                const uint64_t piece = std::min(seg_lens[s] - so, p.len[i] - done);
-                for (uint64_t t = 0; t < piece; t += kGatherTileBytes)
-                    tiles.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + so + t, table[i] + done + t,
-                                     std::min(kGatherTileBytes, piece - t)});
-                done += piece;
-                ++s;
-                so = 0;
-            }
+            uint64_t at = table[i];
+            file_pieces(t, p.file[i], p.off[i], p.len[i], [&](uint64_t s, uint64_t in, uint64_t n) {
+                for (uint64_t k = 0; k < n; k += kGatherTileBytes)
+                    tiles.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in + k, at + k,
+                                     std::min(kGatherTileBytes, n - k)});
+                at += n;
+            });
         }
         wave_tiles[w + 1] = tiles.size();
     }
@@ -1345,17 +1419,9 @@ int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, 
     if (n && !ranges) return fail(ctx, B200H_E_INVALID, "ranges must not be NULL");
     if (n && !d_crc_out) return fail(ctx, B200H_E_INVALID, "d_crc_out must not be NULL");
     if ((uintptr_t)d_crc_out & 3u) return fail(ctx, B200H_E_INVALID, "d_crc_out must be 4-byte aligned");
-    for (uint64_t i = 0; i < n; ++i) {
-        if (ranges[i].len && !ranges[i].d_ptr) return fail(ctx, B200H_E_INVALID, "range " + std::to_string(i) + " is NULL");
-        if ((uintptr_t)ranges[i].d_ptr + ranges[i].len < (uintptr_t)ranges[i].d_ptr)
-            return fail(ctx, B200H_E_INVALID, "range " + std::to_string(i) + " wraps the address space");
-    }
     if (n == 0) return 0;
     CU_TRY(ctx, cudaSetDevice(ctx->device));
-    for (uint64_t i = 0; i < n; ++i)
-        if (!device_range_ok(ctx, ranges[i].d_ptr, ranges[i].len))
-            return fail(ctx, B200H_E_INVALID,
-                        "range " + std::to_string(i) + " is not device memory on cuda:" + std::to_string(ctx->device));
+    if (int rc = segments_on_device(ctx, ranges, n, "range")) return rc;
     if (!device_range_ok(ctx, d_crc_out, n * sizeof(uint32_t)))
         return fail(ctx, B200H_E_INVALID, "d_crc_out is not device memory on cuda:" + std::to_string(ctx->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
@@ -1370,40 +1436,9 @@ int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, 
     }
     CU_TRY(ctx, cudaMemcpyAsync(d_crc_out, init.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     if (first[n] == 0) return 0;
-    // stream-ordered allocation: no synchronisation, and no scratch shared with other streams' calls
-    const size_t rs_bytes = n * sizeof(CrcRange), bytes = rs_bytes + (n + 1) * sizeof(uint64_t);
-    void* d_table = nullptr;
-    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
-    CrcRange* d_ranges = (CrcRange*)d_table;
-    uint64_t* d_first = (uint64_t*)((uint8_t*)d_table + rs_bytes);
-    CU_TRY(ctx, cudaMemcpyAsync(d_ranges, rs.data(), rs_bytes, cudaMemcpyHostToDevice, st));
-    CU_TRY(ctx, cudaMemcpyAsync(d_first, first.data(), (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-    ctx->launches += launch_crc32(d_ranges, d_first, n, first[n], d_crc_out, st);
-    CU_TRY(ctx, cudaGetLastError());
-    CU_TRY(ctx, cudaFreeAsync(d_table, st));
-    return 0;
-}
-
-// The file table of the range-copy entries (segs / file_first_seg as for b200h_hash_segment_parts_device), checked;
-// seg_start[s] = offset of segment s in its file, file_size[f].
-static int segment_files(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
-                         uint64_t nfiles, std::vector<uint64_t>& seg_start, std::vector<uint64_t>& file_size) {
-    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segs must not be NULL");
-    if (!file_first_seg) return fail(ctx, B200H_E_INVALID, "file_first_seg must not be NULL (it has nfiles + 1 entries)");
-    if (file_first_seg[0] != 0) return fail(ctx, B200H_E_INVALID, "file_first_seg[0] must be 0");
-    if (file_first_seg[nfiles] != nsegs) return fail(ctx, B200H_E_INVALID, "file_first_seg[nfiles] must equal nsegs");
-    for (uint64_t f = 0; f < nfiles; ++f)
-        if (file_first_seg[f + 1] < file_first_seg[f]) return fail(ctx, B200H_E_INVALID, "file_first_seg must not decrease");
-    seg_start.assign(nsegs, 0);
-    file_size.assign(nfiles, 0);
-    for (uint64_t f = 0; f < nfiles; ++f)
-        for (uint64_t s = file_first_seg[f]; s < file_first_seg[f + 1]; ++s) {
-            if (segs[s].len && !segs[s].d_ptr) return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(s) + " is NULL");
-            if (file_size[f] + segs[s].len < file_size[f]) return fail(ctx, B200H_E_INVALID, "a file is larger than 2^64 - 1 bytes");
-            seg_start[s] = file_size[f];
-            file_size[f] += segs[s].len;
-        }
-    return 0;
+    return launch_with_tables(ctx, st, rs, first, [&](const CrcRange* d_ranges, const uint64_t* d_first) {
+        return launch_crc32(d_ranges, d_first, n, first[n], d_crc_out, st);
+    });
 }
 
 // The device's address of [h, h + bytes), or NULL unless it is page-locked host memory ctx's device can reach
@@ -1420,21 +1455,86 @@ static void* pinned_device_pointer(b200h_ctx* ctx, const void* h, uint64_t bytes
     return d;
 }
 
-// Calls piece(device address, offset in the host buffer, n) for every part of range r that lies in one segment, in
-// file order (the range lands at / comes from host offset `at`; r.len > 0 and within its file).
-static void range_pieces(const b200h_segment* segs, const std::vector<uint64_t>& seg_start, const uint64_t* file_first_seg,
-                         const b200h_file_range& r, uint64_t at,
-                         const std::function<void(uint64_t, uint64_t, uint64_t)>& piece) {
-    const uint64_t a = file_first_seg[r.file], b = file_first_seg[r.file + 1];
-    // the last segment of the file that starts at or before the range's first byte and is not empty
-    uint64_t s = std::upper_bound(seg_start.begin() + a, seg_start.begin() + b, r.offset) - seg_start.begin() - 1;
-    for (uint64_t done = 0; done < r.len; ++s) {
-        const uint64_t in = r.offset + done - seg_start[s];
-        if (in >= segs[s].len) continue;  // an empty segment
-        const uint64_t n = std::min(segs[s].len - in, r.len - done);
-        piece((uint64_t)(uintptr_t)segs[s].d_ptr + in, at + done, n);
-        done += n;
+// b200h_copy_ranges_to_host (to_host) and b200h_copy_ranges_from_host: range i of the segmented files and bytes
+// [host_offsets[i], host_offsets[i] + len) of the page-locked buffer `host` are copied one way or the other.
+static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, uint64_t nsegs,
+                       const uint64_t* file_first_seg, uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges,
+                       const void* host, uint64_t host_bytes, const uint64_t* host_offsets, void* cuda_stream) {
+    const std::string buf = to_host ? "h_dst" : "h_src", offsets = to_host ? "dst_offsets" : "src_offsets",
+                      noun = to_host ? "destination" : "source";
+    std::vector<uint64_t> seg_lens;
+    FileTable t;
+    if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
+    if (nranges && (!ranges || !host_offsets))
+        return fail(ctx, B200H_E_INVALID, "ranges and " + offsets + " must not be NULL");
+    if (nranges && !host) return fail(ctx, B200H_E_INVALID, buf + " must not be NULL");
+    if ((uintptr_t)host & 15u) return fail(ctx, B200H_E_INVALID, buf + " must be 16-byte aligned");
+    std::vector<uint64_t> order;  // the non-empty ranges
+    for (uint64_t i = 0; i < nranges; ++i) {
+        const b200h_file_range& r = ranges[i];
+        const std::string name = "range " + std::to_string(i);
+        if (r.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
+        if (r.offset > t.size[r.file] || r.len > t.size[r.file] - r.offset)
+            return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
+        if (host_offsets[i] & 15u)
+            return fail(ctx, B200H_E_INVALID, name + ": its " + noun + " offset is not a multiple of 16");
+        if (host_offsets[i] > host_bytes || r.len > host_bytes - host_offsets[i])
+            return fail(ctx, B200H_E_INVALID, name + ": its " + noun + " reaches past " + buf + "_bytes");
+        if (r.len) order.push_back(i);
     }
+    if (to_host) {  // no host byte may be written twice
+        std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return host_offsets[a] < host_offsets[b]; });
+        for (size_t k = 1; k < order.size(); ++k)
+            if (host_offsets[order[k - 1]] + ranges[order[k - 1]].len > host_offsets[order[k]])
+                return fail(ctx, B200H_E_INVALID, "the destinations of ranges " + std::to_string(order[k - 1]) + " and " +
+                                                      std::to_string(order[k]) + " overlap");
+    }
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
+    if (nranges == 0) return 0;
+    void* d_host = pinned_device_pointer(ctx, host, host_bytes);
+    if (!d_host)
+        return fail(ctx, B200H_E_INVALID,
+                    buf + " is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
+    if (order.empty()) return 0;
+
+    // pieces (range x segment, in file order within a range) and the tiles of host bytes that use them
+    std::vector<RangePiece> pieces;
+    std::vector<RangeTile> tiles;
+    std::vector<uint64_t> range_of;  // per piece: the range it belongs to (for the overlap message)
+    for (uint64_t i = 0; i < nranges; ++i) {
+        const b200h_file_range& r = ranges[i];
+        if (!r.len) continue;
+        const size_t first = pieces.size();
+        uint64_t at = host_offsets[i];
+        file_pieces(t, r.file, r.offset, r.len, [&](uint64_t s, uint64_t in, uint64_t n) {
+            pieces.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in, at, n});
+            range_of.push_back(i);
+            at += n;
+        });
+        size_t p = first;
+        for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
+            const uint64_t n = std::min(kStageTileBytes, r.len - o), h = host_offsets[i] + o;
+            while (pieces[p].host + pieces[p].len <= h) ++p;
+            size_t q = p;
+            while (q + 1 < pieces.size() && pieces[q + 1].host < h + n) ++q;
+            tiles.push_back({h, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
+        }
+    }
+    if (!to_host) {  // no device byte may be written twice: two files, or two segments of one file, may share a tensor
+        std::vector<size_t> by_dev(pieces.size());
+        for (size_t k = 0; k < by_dev.size(); ++k) by_dev[k] = k;
+        std::sort(by_dev.begin(), by_dev.end(), [&](size_t a, size_t b) { return pieces[a].dev < pieces[b].dev; });
+        for (size_t k = 1; k < by_dev.size(); ++k)
+            if (pieces[by_dev[k - 1]].dev + pieces[by_dev[k - 1]].len > pieces[by_dev[k]].dev)
+                return fail(ctx, B200H_E_INVALID, "ranges " + std::to_string(range_of[by_dev[k - 1]]) + " and " +
+                                                      std::to_string(range_of[by_dev[k]]) + " write the same device bytes");
+    }
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    return launch_with_tables(ctx, st, tiles, pieces, [&](const RangeTile* d_tiles, const RangePiece* d_pieces) {
+        return to_host ? launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_host, st)
+                       : launch_load_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
+    });
 }
 
 int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
@@ -1443,72 +1543,8 @@ int b200h_copy_ranges_to_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     if (!ctx) return B200H_E_INVALID;
     B200H_RANGE("b200h_copy_ranges_to_host");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    std::vector<uint64_t> seg_start, file_size;
-    if (int rc = segment_files(ctx, segs, nsegs, file_first_seg, nfiles, seg_start, file_size)) return rc;
-    if (nranges && (!ranges || !dst_offsets)) return fail(ctx, B200H_E_INVALID, "ranges and dst_offsets must not be NULL");
-    if (nranges && !h_dst) return fail(ctx, B200H_E_INVALID, "h_dst must not be NULL");
-    if ((uintptr_t)h_dst & 15u) return fail(ctx, B200H_E_INVALID, "h_dst must be 16-byte aligned");
-    std::vector<uint64_t> order;  // the non-empty ranges, by destination
-    for (uint64_t i = 0; i < nranges; ++i) {
-        const b200h_file_range& r = ranges[i];
-        const std::string name = "range " + std::to_string(i);
-        if (r.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
-        if (r.offset > file_size[r.file] || r.len > file_size[r.file] - r.offset)
-            return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
-        if (dst_offsets[i] & 15u) return fail(ctx, B200H_E_INVALID, name + ": its destination offset is not a multiple of 16");
-        if (dst_offsets[i] > h_dst_bytes || r.len > h_dst_bytes - dst_offsets[i])
-            return fail(ctx, B200H_E_INVALID, name + ": its destination reaches past h_dst_bytes");
-        if (r.len) order.push_back(i);
-    }
-    std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return dst_offsets[a] < dst_offsets[b]; });
-    for (size_t k = 1; k < order.size(); ++k)
-        if (dst_offsets[order[k - 1]] + ranges[order[k - 1]].len > dst_offsets[order[k]])
-            return fail(ctx, B200H_E_INVALID, "the destinations of ranges " + std::to_string(order[k - 1]) + " and " +
-                                                  std::to_string(order[k]) + " overlap");
-    if (nranges == 0) return 0;
-    CU_TRY(ctx, cudaSetDevice(ctx->device));
-    // the destination must be page-locked host memory the device can store to (pageable memory would fault the kernel)
-    void* d_dst = pinned_device_pointer(ctx, h_dst, h_dst_bytes);
-    if (!d_dst)
-        return fail(ctx, B200H_E_INVALID,
-                    "h_dst is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
-    for (uint64_t s = 0; s < nsegs; ++s)
-        if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
-            return fail(ctx, B200H_E_INVALID,
-                        "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
-    if (order.empty()) return 0;
-
-    // pieces (range x segment, in destination order within a range) and the tiles that draw from them
-    std::vector<StagePiece> pieces;
-    std::vector<StageTile> tiles;
-    for (uint64_t i = 0; i < nranges; ++i) {
-        const b200h_file_range& r = ranges[i];
-        if (!r.len) continue;
-        const size_t first = pieces.size();
-        range_pieces(segs, seg_start, file_first_seg, r, dst_offsets[i],
-                     [&](uint64_t dev, uint64_t host, uint64_t n) { pieces.push_back({dev, host, n}); });
-        size_t p = first;
-        for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
-            const uint64_t n = std::min(kStageTileBytes, r.len - o), d = dst_offsets[i] + o;
-            while (pieces[p].dst + pieces[p].len <= d) ++p;
-            size_t q = p;
-            while (q + 1 < pieces.size() && pieces[q + 1].dst < d + n) ++q;
-            tiles.push_back({d, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
-        }
-    }
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    // stream-ordered allocation, as b200h_crc32_device: no synchronisation, no scratch shared with other streams' calls
-    const size_t tile_bytes = tiles.size() * sizeof(StageTile), bytes = tile_bytes + pieces.size() * sizeof(StagePiece);
-    void* d_table = nullptr;
-    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
-    StageTile* d_tiles = (StageTile*)d_table;
-    StagePiece* d_pieces = (StagePiece*)((uint8_t*)d_table + tile_bytes);
-    CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tile_bytes, cudaMemcpyHostToDevice, st));
-    CU_TRY(ctx, cudaMemcpyAsync(d_pieces, pieces.data(), bytes - tile_bytes, cudaMemcpyHostToDevice, st));
-    ctx->launches += launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_dst, st);
-    CU_TRY(ctx, cudaGetLastError());
-    CU_TRY(ctx, cudaFreeAsync(d_table, st));
-    return 0;
+    return copy_ranges(ctx, true, segs, nsegs, file_first_seg, nfiles, ranges, nranges, h_dst, h_dst_bytes, dst_offsets,
+                       cuda_stream);
 }
 
 int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
@@ -1517,77 +1553,8 @@ int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint6
     if (!ctx) return B200H_E_INVALID;
     B200H_RANGE("b200h_copy_ranges_from_host");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    std::vector<uint64_t> seg_start, file_size;
-    if (int rc = segment_files(ctx, segs, nsegs, file_first_seg, nfiles, seg_start, file_size)) return rc;
-    if (nranges && (!ranges || !src_offsets)) return fail(ctx, B200H_E_INVALID, "ranges and src_offsets must not be NULL");
-    if (nranges && !h_src) return fail(ctx, B200H_E_INVALID, "h_src must not be NULL");
-    if ((uintptr_t)h_src & 15u) return fail(ctx, B200H_E_INVALID, "h_src must be 16-byte aligned");
-    uint64_t nonempty = 0;
-    for (uint64_t i = 0; i < nranges; ++i) {
-        const b200h_file_range& r = ranges[i];
-        const std::string name = "range " + std::to_string(i);
-        if (r.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
-        if (r.offset > file_size[r.file] || r.len > file_size[r.file] - r.offset)
-            return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
-        if (src_offsets[i] & 15u) return fail(ctx, B200H_E_INVALID, name + ": its source offset is not a multiple of 16");
-        if (src_offsets[i] > h_src_bytes || r.len > h_src_bytes - src_offsets[i])
-            return fail(ctx, B200H_E_INVALID, name + ": its source reaches past h_src_bytes");
-        nonempty += r.len != 0;
-    }
-    if (nranges == 0) return 0;
-    CU_TRY(ctx, cudaSetDevice(ctx->device));
-    const void* d_src = pinned_device_pointer(ctx, h_src, h_src_bytes);
-    if (!d_src)
-        return fail(ctx, B200H_E_INVALID,
-                    "h_src is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
-    for (uint64_t s = 0; s < nsegs; ++s)
-        if (!device_range_ok(ctx, segs[s].d_ptr, segs[s].len))
-            return fail(ctx, B200H_E_INVALID,
-                        "segment " + std::to_string(s) + " is not device memory on cuda:" + std::to_string(ctx->device));
-    if (!nonempty) return 0;
-
-    // pieces (range x segment, in source order within a range) and the tiles that read through them
-    std::vector<LoadPiece> pieces;
-    std::vector<LoadTile> tiles;
-    std::vector<uint64_t> range_of;  // per piece: the range it belongs to (for the overlap message)
-    for (uint64_t i = 0; i < nranges; ++i) {
-        const b200h_file_range& r = ranges[i];
-        if (!r.len) continue;
-        const size_t first = pieces.size();
-        range_pieces(segs, seg_start, file_first_seg, r, src_offsets[i], [&](uint64_t dev, uint64_t host, uint64_t n) {
-            pieces.push_back({host, dev, n});
-            range_of.push_back(i);
-        });
-        size_t p = first;
-        for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
-            const uint64_t n = std::min(kStageTileBytes, r.len - o), at = src_offsets[i] + o;
-            while (pieces[p].src + pieces[p].len <= at) ++p;
-            size_t q = p;
-            while (q + 1 < pieces.size() && pieces[q + 1].src < at + n) ++q;
-            tiles.push_back({at, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
-        }
-    }
-    // no device byte may be written twice: two files, or two segments of one file, may share a tensor
-    std::vector<size_t> by_dst(pieces.size());
-    for (size_t k = 0; k < by_dst.size(); ++k) by_dst[k] = k;
-    std::sort(by_dst.begin(), by_dst.end(), [&](size_t a, size_t b) { return pieces[a].dst < pieces[b].dst; });
-    for (size_t k = 1; k < by_dst.size(); ++k)
-        if (pieces[by_dst[k - 1]].dst + pieces[by_dst[k - 1]].len > pieces[by_dst[k]].dst)
-            return fail(ctx, B200H_E_INVALID, "ranges " + std::to_string(range_of[by_dst[k - 1]]) + " and " +
-                                                  std::to_string(range_of[by_dst[k]]) + " write the same device bytes");
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    // stream-ordered allocation, as b200h_copy_ranges_to_host: no synchronisation
-    const size_t tile_bytes = tiles.size() * sizeof(LoadTile), bytes = tile_bytes + pieces.size() * sizeof(LoadPiece);
-    void* d_table = nullptr;
-    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
-    LoadTile* d_tiles = (LoadTile*)d_table;
-    LoadPiece* d_pieces = (LoadPiece*)((uint8_t*)d_table + tile_bytes);
-    CU_TRY(ctx, cudaMemcpyAsync(d_tiles, tiles.data(), tile_bytes, cudaMemcpyHostToDevice, st));
-    CU_TRY(ctx, cudaMemcpyAsync(d_pieces, pieces.data(), bytes - tile_bytes, cudaMemcpyHostToDevice, st));
-    ctx->launches += launch_load_ranges(d_tiles, tiles.size(), d_pieces, d_src, st);
-    CU_TRY(ctx, cudaGetLastError());
-    CU_TRY(ctx, cudaFreeAsync(d_table, st));
-    return 0;
+    return copy_ranges(ctx, false, segs, nsegs, file_first_seg, nfiles, ranges, nranges, h_src, h_src_bytes, src_offsets,
+                       cuda_stream);
 }
 
 // ---------------------------------------------------------------------------------------------- files
@@ -1967,9 +1934,11 @@ int b200h_plan_preview(const uint64_t* lengths, uint64_t n, uint32_t flags, uint
 int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
                                 uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out, uint64_t* nwaves_out,
                                 uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap) {
+    FileTable t;
     SegmentParts p;
     std::string err;
-    if (int rc = layout_segment_parts(seg_lens, nsegs, file_first_seg, nfiles, part_len, wave_bytes, p, err)) return rc;
+    if (int rc = file_table(seg_lens, nsegs, file_first_seg, nfiles, t, err)) return rc;
+    if (int rc = layout_segment_parts(t, part_len, wave_bytes, p, err)) return rc;
     const uint64_t nparts = p.off.size();
     if (nparts_out) *nparts_out = nparts;
     if (nwaves_out) *nwaves_out = p.wave_bytes.size();

@@ -104,36 +104,24 @@ int launch_crc32(const CrcRange* ranges, const uint64_t* first, uint64_t n, uint
 // (host arithmetic on CRC values; no data involved)
 uint32_t crc32_length_term(uint64_t len);
 
-// Ranges of segmented device files copied to one destination buffer (b200hash_stage.cu).  A piece is the part of a
-// range that lies in one segment (len > 0); the pieces of a range are listed in destination order and cover its
-// destination without gaps.  A tile is up to kStageTileBytes of one range's destination, starting at a multiple of 16;
-// it draws from pieces [first_piece, first_piece + npieces), the first of which holds the tile's first byte.
-struct StagePiece {
-    uint64_t src, dst, len;  // device address; byte offset in the destination buffer
+// Ranges of segmented device files copied to or from one host buffer (b200hash_stage.cu).  A piece is the part of a
+// range that lies in one segment (len > 0); the pieces of a range are listed in file order and cover its bytes of the
+// host buffer without gaps.  A tile is up to kStageTileBytes of one range's bytes of the host buffer, starting at a
+// multiple of 16; it uses pieces [first_piece, first_piece + npieces), every piece that holds one of its bytes.
+struct RangePiece {
+    uint64_t dev, host, len;  // device address; byte offset in the host buffer
 };
-struct StageTile {
-    uint64_t dst;  // byte offset in the destination buffer
+struct RangeTile {
+    uint64_t host;  // byte offset in the host buffer
     uint32_t len, npieces;
     uint64_t first_piece;
 };
 constexpr uint64_t kStageTileBytes = 64 << 10;
-// Every tile's copy, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the device can store to.
-int launch_stage_ranges(const StageTile* tiles, uint64_t ntiles, const StagePiece* pieces, void* dst, cudaStream_t st);
-
-// The inverse: ranges of one source buffer copied into segmented device files (b200hash_stage.cu).  A load piece is
-// the part of a range that lands in one segment (len > 0); the pieces of a range are listed in source order.  A load
-// tile is up to kStageTileBytes of one range's source, starting at a multiple of 16; it writes through pieces
-// [first_piece, first_piece + npieces), every piece that holds one of its source bytes.
-struct LoadPiece {
-    uint64_t src, dst, len;  // byte offset in the source buffer; device address
-};
-struct LoadTile {
-    uint64_t src;  // byte offset in the source buffer
-    uint32_t len, npieces;
-    uint64_t first_piece;
-};
-// Every tile's copy, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device can load from.
-int launch_load_ranges(const LoadTile* tiles, uint64_t ntiles, const LoadPiece* pieces, const void* src, cudaStream_t st);
+// Every tile's copy device -> host, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the device
+// can store to.
+int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, void* dst, cudaStream_t st);
+// The inverse, host -> device; `src` is 16-byte aligned memory the device can load from.
+int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
 
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)

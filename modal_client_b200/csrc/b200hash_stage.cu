@@ -53,27 +53,27 @@ __device__ __forceinline__ uint4 load_word(const uint8_t* src) {
 }
 
 // the piece of pc[lo .. n) that holds destination offset d (the pieces of a range tile its destination without gaps)
-__device__ __forceinline__ uint32_t find_piece(const StagePiece* __restrict__ pc, uint32_t lo, uint32_t n, uint64_t d) {
+__device__ __forceinline__ uint32_t find_piece(const RangePiece* __restrict__ pc, uint32_t lo, uint32_t n, uint64_t d) {
     uint32_t hi = n - 1;
     while (lo < hi) {
         const uint32_t mid = (lo + hi + 1) >> 1;
-        if (pc[mid].dst <= d) lo = mid;
+        if (pc[mid].host <= d) lo = mid;
         else hi = mid - 1;
     }
     return lo;
 }
 
 __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
-    stage_ranges_kernel(const StageTile* __restrict__ tiles, uint64_t ntiles, const StagePiece* __restrict__ pieces,
+    stage_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
                         uint8_t* __restrict__ dst) {
     for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const StageTile tile = tiles[t];
-        const StagePiece* __restrict__ pc = pieces + tile.first_piece;
-        uint8_t* out = dst + tile.dst;
+        const RangeTile tile = tiles[t];
+        const RangePiece* __restrict__ pc = pieces + tile.first_piece;
+        uint8_t* out = dst + tile.host;
         const uint32_t words = tile.len >> 4, tail = tile.len & 15u;
         if (tile.npieces == 1) {
             // the whole tile comes from one segment: one phase, no lookups
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(pc->src) + (tile.dst - pc->dst);
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(pc->dev) + (tile.host - pc->host);
             const uint32_t sh = (uint32_t)((uintptr_t)src & 15u);
             const uint4* a = reinterpret_cast<const uint4*>(src - sh);
             uint4* o = reinterpret_cast<uint4*>(out);
@@ -105,32 +105,32 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
         }
         uint32_t cur = 0;
         for (uint32_t w = threadIdx.x; w < words; w += kStageThreads) {
-            const uint64_t d = tile.dst + (uint64_t)w * 16;
-            if (d >= pc[cur].dst + pc[cur].len) cur = find_piece(pc, cur + 1, tile.npieces, d);
-            const uint64_t in = d - pc[cur].dst, left = pc[cur].len - in;
+            const uint64_t d = tile.host + (uint64_t)w * 16;
+            if (d >= pc[cur].host + pc[cur].len) cur = find_piece(pc, cur + 1, tile.npieces, d);
+            const uint64_t in = d - pc[cur].host, left = pc[cur].len - in;
             uint4 v;
             if (left >= 16) {
-                v = load_word(reinterpret_cast<const uint8_t*>(pc[cur].src) + in);
+                v = load_word(reinterpret_cast<const uint8_t*>(pc[cur].dev) + in);
             } else {
                 uint32_t r[4] = {0, 0, 0, 0};
                 uint32_t i = cur;
-                uint64_t end = pc[i].dst + pc[i].len;
+                uint64_t end = pc[i].host + pc[i].len;
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     while (d + j >= end) {
                         ++i;
-                        end = pc[i].dst + pc[i].len;
+                        end = pc[i].host + pc[i].len;
                     }
-                    r[j >> 2] |= (uint32_t)reinterpret_cast<const uint8_t*>(pc[i].src)[d + j - pc[i].dst] << (8 * (j & 3));
+                    r[j >> 2] |= (uint32_t)reinterpret_cast<const uint8_t*>(pc[i].dev)[d + j - pc[i].host] << (8 * (j & 3));
                 }
                 v = make_uint4(r[0], r[1], r[2], r[3]);
             }
             *reinterpret_cast<uint4*>(dst + d) = v;
         }
         if (threadIdx.x < tail) {
-            const uint64_t d = tile.dst + (uint64_t)words * 16 + threadIdx.x;
+            const uint64_t d = tile.host + (uint64_t)words * 16 + threadIdx.x;
             const uint32_t i = find_piece(pc, 0, tile.npieces, d);
-            dst[d] = reinterpret_cast<const uint8_t*>(pc[i].src)[d - pc[i].dst];
+            dst[d] = reinterpret_cast<const uint8_t*>(pc[i].dev)[d - pc[i].host];
         }
     }
 }
@@ -181,35 +181,35 @@ __device__ __forceinline__ uint4 shfl_last_word(uint4 v) {
 // tile's first byte `ts` (a tile is at most 64 KiB): base = 16 * (w - the tile's first word); only source bytes in
 // [lo, hi), the words this lane holds, are stored.  p is the lane's cursor: pieces that end before anything word w
 // could take are skipped.
-__device__ __forceinline__ void load_word_out(const LoadPiece* __restrict__ pc, uint32_t& p, uint32_t n, uint64_t ts,
+__device__ __forceinline__ void load_word_out(const RangePiece* __restrict__ pc, uint32_t& p, uint32_t n, uint64_t ts,
                                               int32_t base, uint4 prev, uint4 cur, int32_t lo, int32_t hi) {
     const uint64_t at = ts + (uint32_t)base;
-    while (p < n && pc[p].src + pc[p].len + 15 <= at) ++p;
-    for (uint32_t q = p; q < n && pc[q].src < at + 16; ++q) {
-        const LoadPiece piece = pc[q];
-        const uint32_t r = (uint32_t)(piece.dst - piece.src) & 15u;
+    while (p < n && pc[p].host + pc[p].len + 15 <= at) ++p;
+    for (uint32_t q = p; q < n && pc[q].host < at + 16; ++q) {
+        const RangePiece piece = pc[q];
+        const uint32_t r = (uint32_t)(piece.dev - piece.host) & 15u;
         const int32_t s0 = base - (int32_t)r;
         // the piece clipped to [base - 16, base + 16): it may begin in an earlier tile or end in a later one
-        const int32_t from = piece.src + 16 <= at ? base - 16 : (int32_t)(piece.src - ts);
-        const int32_t to = piece.src + piece.len >= at + 16 ? base + 16 : (int32_t)(piece.src + piece.len - ts);
+        const int32_t from = piece.host + 16 <= at ? base - 16 : (int32_t)(piece.host - ts);
+        const int32_t to = piece.host + piece.len >= at + 16 ? base + 16 : (int32_t)(piece.host + piece.len - ts);
         const int32_t a = max(max(s0, from), lo), b = min(min(s0 + 16, to), hi);
         if (a >= b) continue;
-        store_bytes(reinterpret_cast<uint8_t*>(piece.dst + (ts - piece.src) + (uint64_t)(int64_t)s0),
+        store_bytes(reinterpret_cast<uint8_t*>(piece.dev + (ts - piece.host) + (uint64_t)(int64_t)s0),
                     r ? shift_bytes(prev, cur, 16 - r) : cur, (uint32_t)(a - s0), (uint32_t)(b - s0));
     }
 }
 
 __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
-    load_ranges_kernel(const LoadTile* __restrict__ tiles, uint64_t ntiles, const LoadPiece* __restrict__ pieces,
+    load_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
                        const uint8_t* __restrict__ src) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint4* words = reinterpret_cast<const uint4*>(src);
     const uint4 zero = make_uint4(0, 0, 0, 0);
     const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
     for (uint64_t t = (uint64_t)blockIdx.x * (kStageThreads / 32) + (threadIdx.x >> 5); t < ntiles; t += nwarps) {
-        const LoadTile tile = tiles[t];
-        const LoadPiece* __restrict__ pc = pieces + tile.first_piece;
-        const uint4* tw = words + (tile.src >> 4);
+        const RangeTile tile = tiles[t];
+        const RangePiece* __restrict__ pc = pieces + tile.first_piece;
+        const uint4* tw = words + (tile.host >> 4);
         const int32_t nw = (int32_t)((tile.len + 15) >> 4);
         uint32_t p = 0;
         uint4 carry = zero;
@@ -229,7 +229,7 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
                 if (lane == 0) prev = carry;
                 carry = shfl_last_word(v[i]);
                 if (w <= nw)
-                    load_word_out(pc, p, tile.npieces, tile.src, w * 16, prev, v[i], w > 0 ? w * 16 - 16 : 0,
+                    load_word_out(pc, p, tile.npieces, tile.host, w * 16, prev, v[i], w > 0 ? w * 16 - 16 : 0,
                                   w < nw ? w * 16 + 16 : w * 16);
             }
         }
@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
 
 }  // namespace
 
-int launch_load_ranges(const LoadTile* tiles, uint64_t ntiles, const LoadPiece* pieces, const void* src, cudaStream_t st) {
+int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
     if (!ntiles) return 0;
     const uint64_t per_cta = kStageThreads / 32, ctas = (ntiles + per_cta - 1) / per_cta;
     const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
@@ -247,7 +247,7 @@ int launch_load_ranges(const LoadTile* tiles, uint64_t ntiles, const LoadPiece* 
     return 1;
 }
 
-int launch_stage_ranges(const StageTile* tiles, uint64_t ntiles, const StagePiece* pieces, void* dst, cudaStream_t st) {
+int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, void* dst, cudaStream_t st) {
     if (!ntiles) return 0;
     const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
     stage_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,

@@ -213,12 +213,7 @@ def _hash_sources(sources: list[_TensorBytes], ctx, part_len: int, flags: int):
     if part_len <= 0:
         raise ValueError("part_len must be > 0")
     lead = sources[0]
-    ptrs, lens, first = [], [], [0]
-    for src in sources:
-        lead._after(src)
-        ptrs += [s.data_ptr() if s.numel() else 0 for s in src.segments]
-        lens += [s.numel() for s in src.segments]
-        first.append(len(lens))
+    ptrs, lens, first = _file_table(sources)
     n = sum(-(-src.nbytes // part_len) for src in sources)
     with lead._on_stream():
         d_sha, d_md5, d_trim = _outputs(n, flags, lead.segments[0].device)
@@ -262,14 +257,8 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
     Returns at once; ``wait()`` on the result blocks until the bytes are in ``dst``.  Every file's ``bytes_to_host``
     grows by the bytes of its ranges."""
     ctx = ctx or get_context()
-    sources = [f._src for f in files]
-    ranges = [(int(f), int(o), int(n)) for f, o, n in ranges]
-    offsets = [int(o) for o in dst_offsets]
-    if len(offsets) != len(ranges):
-        raise ValueError("dst_offsets needs one entry per range")
+    sources, ranges, offsets = _range_args(files, ranges, dst_offsets, "dst_offsets")
     if not sources:
-        if ranges:
-            raise ValueError("ranges without files")
         return Staged(dst, [], None)
     lead = sources[0]
     ptrs, lens, first = _file_table(sources)
@@ -293,6 +282,18 @@ def _file_table(sources: list[_TensorBytes]):
         lens += [s.numel() for s in src.segments]
         first.append(len(lens))
     return ptrs, lens, first
+
+
+def _range_args(files: list["DeviceFile"], ranges, offsets, offsets_name: str):
+    """(sources, ranges as int triples, offsets as ints) of a ``stage_ranges`` / ``load_ranges`` call, checked."""
+    sources = [f._src for f in files]
+    ranges = [(int(f), int(o), int(n)) for f, o, n in ranges]
+    offsets = [int(o) for o in offsets]
+    if len(offsets) != len(ranges):
+        raise ValueError(f"{offsets_name} needs one entry per range")
+    if ranges and not sources:
+        raise ValueError("ranges without files")
+    return sources, ranges, offsets
 
 
 class Loaded:
@@ -319,14 +320,8 @@ def load_ranges(files: list["DeviceFile"], ranges, src: np.ndarray, src_offsets,
     Returns at once; ``wait()`` on the result blocks until the kernel has read ``src``.  ``DeviceFile`` itself stays a
     read-only file object: this is the one way bytes get into its tensors."""
     ctx = ctx or get_context()
-    sources = [f._src for f in files]
-    ranges = [(int(f), int(o), int(n)) for f, o, n in ranges]
-    offsets = [int(o) for o in src_offsets]
-    if len(offsets) != len(ranges):
-        raise ValueError("src_offsets needs one entry per range")
+    sources, ranges, offsets = _range_args(files, ranges, src_offsets, "src_offsets")
     if not sources:
-        if ranges:
-            raise ValueError("ranges without files")
         return Loaded(None)
     lead = sources[0]
     lead._after_current()

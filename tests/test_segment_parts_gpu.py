@@ -180,7 +180,8 @@ def test_segment_parts_reject_foreign_pointers_before_launching(ctx):
     dev = torch.zeros(4096, dtype=torch.uint8, device="cuda:0")
     cases = [([dev.data_ptr(), host.ctypes.data], [4096, 4096]),  # host memory
              ([host.ctypes.data, dev.data_ptr()], [16, 4096]),
-             ([dev.data_ptr(), 0], [10, 5])]                       # NULL with bytes behind it
+             ([dev.data_ptr(), 0], [10, 5]),                       # NULL with bytes behind it
+             ([dev.data_ptr()], [2**64 - dev.data_ptr() + 16])]    # an address range that wraps
     if torch.cuda.device_count() > 1:  # another device's memory
         other = torch.zeros(64, dtype=torch.uint8, device="cuda:1")
         cases.append(([dev.data_ptr(), other.data_ptr()], [64, 64]))

@@ -46,15 +46,23 @@ class StagingContext(FakeDeviceContext):
         assert all(at % 16 == 0 for at in dst_offsets) and all(hi <= dst.size for _, hi in spans)
         assert all(a[1] <= b[0] for a, b in zip(spans, spans[1:]))
         for (f, off, n), at in zip(ranges, dst_offsets):
-            segs = list(zip(seg_ptrs[file_first_seg[f] : file_first_seg[f + 1]],
-                            seg_lens[file_first_seg[f] : file_first_seg[f + 1]]))
-            assert off + n <= sum(ln for _, ln in segs)
-            start = 0
-            for p, ln in segs:
-                lo, hi = max(off, start), min(off + n, start + ln)
-                if lo < hi:
-                    ctypes.memmove(dst.ctypes.data + at + lo - off, int(p) + lo - start, hi - lo)
-                start += ln
+            for p, into, k in range_pieces(seg_ptrs, seg_lens, file_first_seg, f, off, n):
+                ctypes.memmove(dst.ctypes.data + at + into, p, k)
+
+
+def range_pieces(seg_ptrs, seg_lens, file_first_seg, f, off, n):
+    """(address, offset into the range, bytes) of every segment piece of range ``(f, off, n)``, which must lie inside
+    its file."""
+    segs = list(zip(seg_ptrs[file_first_seg[f] : file_first_seg[f + 1]],
+                    seg_lens[file_first_seg[f] : file_first_seg[f + 1]]))
+    assert off + n <= sum(ln for _, ln in segs)
+    pieces, start = [], 0
+    for p, ln in segs:
+        lo, hi = max(off, start), min(off + n, start + ln)
+        if lo < hi:
+            pieces.append((int(p) + lo - start, lo - off, hi - lo))
+        start += ln
+    return pieces
 
 
 class _StagedHostSegments(_HostSegments):

@@ -182,6 +182,7 @@ def test_bad_arguments_are_rejected_before_anything_is_enqueued(ctx, pinned):
     cases = {
         "foreign segment": dict(ptrs=[host.data_ptr()]),
         "NULL segment": dict(ptrs=[0]),
+        "segment whose address range wraps": dict(lens=[2**64 - seg.data_ptr() + 16]),
         "pageable destination": dict(dst=pageable[-pageable.ctypes.data % 16 :][:4096]),
         "misaligned destination": dict(offsets=[0, 136]),
         "overlapping destinations": dict(offsets=[0, 96]),

@@ -21,7 +21,7 @@ from modal_client_b200 import _lib, blob_utils, volume
 from modal_client_b200.exception import ExecutionError
 from modal_client_b200.synth import synth_bytes
 from tests.test_device_file_cpu import HostDeviceFile, _HostSegments
-from tests.test_stage_ranges_cpu import StagingContext
+from tests.test_stage_ranges_cpu import StagingContext, range_pieces
 from tests.volume_read_server import running_volume_server
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -38,16 +38,9 @@ class ReadContext(StagingContext):
         assert all(at + n <= src.size for (_, _, n), at in zip(ranges, src_offsets))
         written = []
         for (f, off, n), at in zip(ranges, src_offsets):
-            segs = list(zip(seg_ptrs[file_first_seg[f] : file_first_seg[f + 1]],
-                            seg_lens[file_first_seg[f] : file_first_seg[f + 1]]))
-            assert off + n <= sum(ln for _, ln in segs)
-            start = 0
-            for p, ln in segs:
-                lo, hi = max(off, start), min(off + n, start + ln)
-                if lo < hi:
-                    written.append((int(p) + lo - start, int(p) + hi - start))
-                    ctypes.memmove(int(p) + lo - start, src.ctypes.data + at + lo - off, hi - lo)
-                start += ln
+            for p, into, k in range_pieces(seg_ptrs, seg_lens, file_first_seg, f, off, n):
+                written.append((p, p + k))
+                ctypes.memmove(p, src.ctypes.data + at + into, k)
         written.sort()
         assert all(a[1] <= b[0] for a, b in zip(written, written[1:])), "two ranges write the same device bytes"
 

@@ -147,6 +147,7 @@ def test_bad_arguments_are_rejected_before_anything_is_enqueued(ctx, pinned):
     cases = {
         "host segment": dict(ptrs=[host.data_ptr()]),
         "NULL segment": dict(ptrs=[0]),
+        "segment whose address range wraps": dict(lens=[2**64 - seg.data_ptr() + 16]),
         "overlapping destinations": dict(ranges=[(0, 0, 100), (0, 99, 100)]),
         "the same tensor in two files": dict(ptrs=[seg.data_ptr()] * 2, lens=[4096] * 2, first=[0, 1, 2],
                                              ranges=[(0, 0, 100), (1, 50, 10)]),
