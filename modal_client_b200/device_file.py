@@ -470,12 +470,12 @@ class _Skeleton:
 
 
 class _ZipRecord:
-    __slots__ = ("name", "flags", "crc", "size", "local", "data", "crc_at")
+    __slots__ = ("name", "flags", "crc", "size", "local", "data", "crc_at", "cd_at")
 
 
-def _parse_zip(sk: _Skeleton, size: int) -> list[_ZipRecord]:
-    """The records of the archive in file order, from its central directory (ZIP64 records included); raises
-    ``ValueError`` on anything torch.save does not write (compression, extra bytes between records, ...)."""
+def _zip_directory(sk: _Skeleton) -> tuple[int, int]:
+    """(record count, central directory offset) of the archive, from its end-of-central-directory record (in the last
+    piece) or the ZIP64 end record it points to."""
     tail_start, tail = sk.pieces[-1][0], sk.pieces[-1][1]
     end = bytes(tail).rfind(_ZIP_END.to_bytes(4, "little"))
     if end < 0:
@@ -490,11 +490,20 @@ def _parse_zip(sk: _Skeleton, size: int) -> list[_ZipRecord]:
         if sk.u(z64, 4) != _ZIP64_END:
             raise ValueError("torch.save layout: ZIP64 end record missing")
         count, cd_off = sk.u(z64 + 32, 8), sk.u(z64 + 48, 8)
-    records, at = [], cd_off
+    return count, cd_off
+
+
+def _central_directory(sk: _Skeleton) -> list[_ZipRecord]:
+    """The records of the archive in central-directory order (name, flags, CRC, size, local header offset, and
+    ``cd_at``, the offset of the entry), ZIP64 fields included; raises ``ValueError`` on a record that is not stored
+    uncompressed."""
+    count, at = _zip_directory(sk)
+    records = []
     for _ in range(count):
         if sk.u(at, 4) != _ZIP_CENTRAL:
             raise ValueError(f"torch.save layout: no central directory entry at {at}")
         r = _ZipRecord()
+        r.cd_at = at
         r.flags, method, r.crc = sk.u(at + 8, 2), sk.u(at + 10, 2), sk.u(at + 16, 4)
         comp, r.size, nlen, xlen, clen = (sk.u(at + 20, 4), sk.u(at + 24, 4), sk.u(at + 28, 2), sk.u(at + 30, 2),
                                           sk.u(at + 32, 2))
@@ -516,19 +525,36 @@ def _parse_zip(sk: _Skeleton, size: int) -> list[_ZipRecord]:
             x += 4 + n
         if method != 0 or comp != r.size:
             raise ValueError(f"torch.save layout: record {r.name!r} is not stored uncompressed")
-        if sk.u(r.local, 4) != _ZIP_LOCAL:
-            raise ValueError(f"torch.save layout: no local header for {r.name!r}")
-        r.data = r.local + 30 + sk.u(r.local + 26, 2) + sk.u(r.local + 28, 2)
+        records.append(r)
+        at = x_end + clen
+    return records
+
+
+def _local_data_offset(sk, r: _ZipRecord) -> int:
+    """File offset of ``r``'s data, from its local header (signature, the name as in the central directory, then the
+    name and extra lengths).  ``sk``: anything with the ``_Skeleton`` reads that holds the header's bytes."""
+    if sk.u(r.local, 4) != _ZIP_LOCAL:
+        raise ValueError(f"torch.save layout: no local header for {r.name!r}")
+    nlen, xlen = sk.u(r.local + 26, 2), sk.u(r.local + 28, 2)
+    if sk.read(r.local + 30, nlen) != r.name.encode("utf-8"):
+        raise ValueError(f"torch.save layout: the local header of {r.name!r} names another record")
+    return r.local + 30 + nlen + xlen
+
+
+def _parse_zip(sk: _Skeleton, size: int) -> list[_ZipRecord]:
+    """The records of the archive in file order, from its central directory (ZIP64 records included); raises
+    ``ValueError`` on anything torch.save does not write (compression, extra bytes between records, ...)."""
+    records = _central_directory(sk)
+    for r in records:
+        r.data = _local_data_offset(sk, r)
         if r.flags & 8:  # CRC and sizes follow the data in a descriptor; the local header's CRC stays 0
-            r.crc_at = [r.data + r.size + 4, at + 16]
+            r.crc_at = [r.data + r.size + 4, r.cd_at + 16]
             if sk.u(r.data + r.size, 4) != _ZIP_DESCRIPTOR or sk.u(r.data + r.size + 4, 4) != r.crc:
                 raise ValueError(f"torch.save layout: bad data descriptor for {r.name!r}")
         else:
-            r.crc_at = [r.local + 14, at + 16]
+            r.crc_at = [r.local + 14, r.cd_at + 16]
             if sk.u(r.local + 14, 4) != r.crc:
                 raise ValueError(f"torch.save layout: local and central CRC of {r.name!r} differ")
-        records.append(r)
-        at = x_end + clen
     if [r.local for r in records] != sorted(r.local for r in records) or (records and records[-1].data > size):
         raise ValueError("torch.save layout: records out of order")
     return records

@@ -17,7 +17,8 @@ there, so the tensors are free again (``device_released``) after the last copy i
 The way back (counterparts of ``Volume.read_file`` / ``read_file_into_fileobj``, py/modal/volume.py:878-1000):
 ``read_file`` and ``read_file_into_fileobj`` through host memory, ``read_file_into_device`` straight into the tensors
 of a ``DeviceFile`` (blocks downloaded into page-locked memory, a wave per ``load_ranges`` call), and
-``read_safetensors``, a safetensors checkpoint back into CUDA tensors without a host copy of the file.
+``read_safetensors``, a safetensors checkpoint back into CUDA tensors without a host copy of the file, and
+``read_torch_save``, a torch.save checkpoint back into CUDA storages, its zip CRC-32s checked on the device.
 """
 from __future__ import annotations
 
@@ -33,7 +34,7 @@ from typing import Any, BinaryIO
 
 import numpy as np
 
-from . import _wire, blob_utils
+from . import _wire, blob_utils, device_file
 from ._logging import logger
 from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
@@ -533,6 +534,20 @@ async def read_file_into_device(client, volume_id: str, path: str, dst: DeviceFi
         await _get_file2(client, volume_id, path, start, 1)  # the file must exist; nothing else to do
         return 0
     slices = await _block_slices(client, volume_id, path, start, n)
+    await _load_in_waves(slices, dst, lambda wave, at, _: ([(0, off, m) for _, off, m in wave], at), staging_bytes,
+                         concurrency, progress_cb)
+    return n
+
+
+async def _load_in_waves(slices, dst: DeviceFile, plan, staging_bytes: int, concurrency: int | None,
+                         progress_cb: Callable[..., Any]) -> None:
+    """Download ``slices`` (``_block_slices``) into ``dst``: every block goes to its own ``BLOCK_SIZE`` slot of a
+    page-locked buffer (``ctx.host_alloc``) of two halves, a wave per half; when a wave is complete,
+    ``plan(wave, at, buf)`` -- the wave's slices, their offsets in the buffer and the buffer -- gives the
+    ``(ranges, src_offsets)`` of its one ``load_ranges`` call.  A half is refilled only after its previous copy has read
+    it, so ``plan`` may still read the previous wave's slots; every copy has read the buffer before it is freed, however
+    the call ends."""
+    BS = blob_utils.BLOCK_SIZE
     per_half = staging_bytes // 2 // BS  # block slots per half (every slot starts at a multiple of BLOCK_SIZE)
     semaphore = asyncio.Semaphore(concurrency or os.cpu_count() or 1)
     ctx = blob_utils.get_context()
@@ -546,18 +561,18 @@ async def read_file_into_device(client, volume_id: str, path: str, dst: DeviceFi
                 loaded[half] = None
             at = [(half * per_half + i) * BS for i in range(len(wave))]
 
-            async def fetch(i: int, url: str, m: int, a: int):
+            async def fetch(url: str, m: int, a: int):
                 await _fetch_block(url, buf[a : a + m], m, semaphore)
                 progress_cb(advance=m)
 
-            await gather_cancel_on_error(*[fetch(i, url, m, a) for i, ((url, _, m), a) in enumerate(zip(wave, at))])
-            loaded[half] = load_ranges([dst], [(0, off, m) for _, off, m in wave], buf, at, ctx=ctx)
+            await gather_cancel_on_error(*[fetch(url, m, a) for (url, _, m), a in zip(wave, at)])
+            ranges, src_offsets = plan(wave, at, buf)
+            loaded[half] = load_ranges([dst], ranges, buf, src_offsets, ctx=ctx)
     finally:
         for pending in loaded:  # the copies must have read the buffer before it is freed
             if pending is not None:
                 await asyncio.to_thread(pending.wait)
         ctx.host_free(buf)
-    return n
 
 
 def _safetensors_entries(header: bytes, data_len: int):
@@ -669,6 +684,248 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
 
 
 _ST_MAX_HEADER = 100_000_000  # the safetensors library's bound on the header length
+
+
+_ZIP_TAIL = 1 << 16  # the end of a torch.save file read first: its end records and, usually, its central directory
+_ZIP_TRAILER = 1 << 12  # read before the central directory too: torch.save's version and serialization id records
+
+
+def _check_format_version(path: str, prefix: str, small: dict) -> None:
+    """The archive's format version as torch's own reader checks it (the range this torch reads), ``ValueError``
+    otherwise: ``torch._C.PyTorchFileReader`` over a zip of the version records alone."""
+    import zipfile
+
+    import torch
+
+    b = BytesIO()
+    with zipfile.ZipFile(b, "w") as z:
+        for name in ("version", ".data/version"):
+            if name in small:
+                z.writestr(prefix + name, small[name])
+    try:
+        torch._C.PyTorchFileReader(BytesIO(b.getvalue()))
+    except RuntimeError as exc:
+        raise ValueError(f"{path}: {exc}") from None
+
+
+class _ArchiveRecords:
+    """What ``torch.serialization._load`` reads a torch.save archive through (the reader interface of
+    ``torch._C.PyTorchFileReader``, record names without the archive prefix): the small records from host memory, and
+    for every ``data/<key>`` record the pickle references a new, empty storage of the record's size
+    (``DeviceFile._Source._empty``), kept in ``storages`` to be filled afterwards."""
+
+    def __init__(self, small: dict, data: dict, ctx):
+        self.small, self.data, self.ctx = small, data, ctx
+        self.storages: dict = {}  # record name -> uint8 tensor over the storage
+
+    def has_record(self, name: str) -> bool:
+        return name in self.small or name in self.data
+
+    def get_record(self, name: str) -> bytes:
+        if name not in self.small:
+            raise ValueError(f"torch.save archive: no record {name!r} among its small records")
+        return self.small[name]
+
+    def get_all_records(self) -> list[str]:
+        return [*self.small, *self.data]
+
+    def serialization_id(self) -> str:
+        return self.small.get(".data/serialization_id", b"").decode("ascii", "replace")
+
+    def get_storage_from_record(self, name: str, nbytes: int, _storage_type):
+        r = self.data.get(name)
+        if r is None:
+            raise ValueError(f"torch.save archive: the pickle references {name!r}, which has no record")
+        if r.size != nbytes:
+            raise ValueError(f"torch.save archive: the pickle gives {name!r} {nbytes} bytes, its record holds {r.size}")
+        if name not in self.storages:
+            self.storages[name] = DeviceFile._Source._empty(nbytes, self.ctx)
+        return self.storages[name]
+
+
+class _StorageWaves:
+    """The ``plan`` of ``read_torch_save``'s waves: the staged span starts at file offset ``span_at``, the storages'
+    ``records`` are the segments of the destination file, in file order.  Before a wave's storage bytes are written,
+    the local header of every storage whose data starts in it is checked against the central directory; it is in this
+    wave's or the previous wave's slots (those are not refilled yet).  Also the ``_Skeleton`` reads over those slots."""
+
+    def __init__(self, path: str, records, span_at: int):
+        self.path, self.records, self.span_at = path, records, span_at
+        self.seg_at = np.concatenate([[0], np.cumsum([r.size for r in records])]).tolist()
+        self.window: list = [[], []]  # (offset in the span, length, buffer offset) of the previous and current slices
+        self.checked = self.open = 0  # storages whose header was checked / the first one not completely written
+        self.buf = None
+
+    def read(self, off: int, n: int) -> bytes:
+        out, lo = bytearray(), off - self.span_at
+        for o, m, a in self.window[0] + self.window[1]:
+            x, y = max(lo, o), min(lo + n, o + m)
+            if x < y:
+                out += self.buf[a + x - o : a + y - o].tobytes()
+        if len(out) != n:
+            raise ValueError(f"{self.path}: bytes [{off}, {off + n}) of a local header are not in the staging buffer")
+        return bytes(out)
+
+    def u(self, off: int, n: int) -> int:
+        return int.from_bytes(self.read(off, n), "little")
+
+    def __call__(self, wave, at, buf):
+        self.buf = buf
+        self.window = [self.window[1], [(o, m, a) for (_, o, m), a in zip(wave, at)]]
+        lo, hi = wave[0][1] + self.span_at, wave[-1][1] + wave[-1][2] + self.span_at  # file offsets of the wave
+        recs = self.records
+        while self.checked < len(recs) and recs[self.checked].data < hi:
+            r = recs[self.checked]
+            got = device_file._local_data_offset(self, r)
+            if got != r.data:
+                raise ValueError(f"{self.path}: the local header of {r.name!r} puts its data at {got}, but the central "
+                                 f"directory leaves room for it only at {r.data} (its data must end right before the "
+                                 f"next record)")
+            self.checked += 1
+        while self.open < len(recs) and recs[self.open].data + recs[self.open].size <= lo:
+            self.open += 1
+        ranges, offsets = [], []
+        for i in range(self.open, len(recs)):
+            d, n = recs[i].data, recs[i].size
+            if d >= hi:
+                break
+            for (_, o, m), a in zip(wave, at):
+                x, y = max(d, o + self.span_at), min(d + n, o + self.span_at + m)
+                if x < y:
+                    ranges.append((0, self.seg_at[i] + x - d, y - x))
+                    offsets.append(a + x - o - self.span_at)
+        return ranges, offsets
+
+
+def _crc_mismatches(pairs) -> list[str]:
+    """``pairs``: (record, computed CRC-32); the records whose stored CRC-32 is not 0 and differs, as text."""
+    return [f"{r.name} (stored {r.crc:08x}, computed {c:08x})" for r, c in pairs if r.crc and r.crc != c]
+
+
+async def read_torch_save(client, volume_id: str, path: str, *, weights_only: bool = True,
+                          staging_bytes: int = 256 << 20):
+    """The torch.save checkpoint at ``path``, loaded as ``torch.load(f, map_location=f"cuda:{ctx.device}",
+    weights_only=weights_only)`` loads the file's bytes (same structure, types, dtypes, shapes, strides and values;
+    storages shared in the file are shared in the result, CPU-saved ones are on the device too), without assembling the
+    image in host memory or HBM, and with the stored CRC-32 of every record it reads checked (unreferenced data records
+    are neither read nor checked).
+
+    The end of the file (end records, central directory, and the small records after the data records: ``version``,
+    ``.data/serialization_id``), then the region before the first data record (``data.pkl`` and the other small
+    records) come through host memory in ranged reads.  The small records' CRC-32s are checked with zlib, the format
+    version as torch's own reader checks it, and ``data.pkl`` is unpickled by torch's own loader (``find_class``
+    remapping, the ``weights_only`` allow-lists, the tensor rebuilds), every storage it references being a new, empty
+    tensor on the device.  Only then does one ``VolumeGetFile2`` call name the blocks from the first referenced data
+    record to the end of the last one: at most five calls in all for an archive torch.save wrote, whatever the number
+    of storages.  The blocks go through ``staging_bytes`` of page-locked memory (two halves, as
+    ``read_file_into_device``) and every complete wave writes the storages' bytes in it with one ``load_ranges`` call.
+    Where each storage's data starts is taken from the central directory before the download (its data ends right
+    before the next record's local header, less its data descriptor); each storage's own local header, read from the
+    staging buffer, must name the record and put the data there, else ``ValueError`` (an archive with bytes between
+    records, for one).  Last, one ``crc32_device`` call on the current stream covers every loaded storage with a stored
+    CRC-32 (torch writes 0 when CRCs are off: not checked), and the values are read back once.  A mismatch raises
+    ``ExecutionError`` naming every bad record.  On return the bytes are ordered before work enqueued later on the
+    current stream.
+
+    ``ValueError`` before any GET of the data region: not a zip archive (the legacy format included), a TorchScript
+    archive, a compressed record, a format version this torch does not read, a ``byteorder`` other than little, a
+    storage whose data is not 16-byte aligned, a storage whose size differs from its record's (``torch.load`` refuses
+    it too) or that has no record; torch's ``pickle.UnpicklingError`` for a global ``weights_only`` refuses;
+    ``FileNotFoundError`` for a missing path."""
+    import pickle
+    import zlib
+
+    import torch
+
+    BS = blob_utils.BLOCK_SIZE
+    if staging_bytes < 2 * BS:
+        raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
+    ctx = blob_utils.get_context()
+    size = (await _get_file2(client, volume_id, path, 0, 1)).size
+    # the end of the file as ONE piece: a central directory field may lie on either side of any read's edge
+    end_at = max(0, size - _ZIP_TAIL)
+    end = bytearray(await _read_range_host(client, volume_id, path, end_at, size - end_at))
+
+    async def extend_end(lo: int):
+        nonlocal end, end_at
+        if lo < end_at:
+            end = bytearray(await _read_range_host(client, volume_id, path, lo, end_at - lo)) + end
+            end_at = lo
+
+    try:
+        _, cd_off = device_file._zip_directory(device_file._Skeleton([(end_at, end)]))
+    except ValueError:
+        raise ValueError(f"{path} is not a torch.save zip archive (no end-of-central-directory record)") from None
+    if not 0 <= cd_off <= size:
+        raise ValueError(f"{path}: the central directory offset {cd_off} lies outside the {size}-byte file")
+    await extend_end(max(0, cd_off - _ZIP_TRAILER))
+    records = sorted(device_file._central_directory(device_file._Skeleton([(end_at, end)])), key=lambda r: r.local)
+    if not records:
+        raise ValueError(f"{path}: the zip archive holds no records")
+    prefix = records[0].name.split("/", 1)[0] + "/"
+    if any(not r.name.startswith(prefix) for r in records):
+        raise ValueError(f"{path}: the archive's records do not share one prefix ({prefix!r})")
+    rel = {r.name[len(prefix) :]: r for r in records}
+    if "constants.pkl" in rel:
+        raise ValueError(f"{path} is a TorchScript archive; load it with torch.jit.load")
+    if "data.pkl" not in rel:
+        raise ValueError(f"{path}: the archive has no data.pkl record")
+    data = {n: r for n, r in rel.items() if n.startswith("data/")}
+    # Where every data record's bytes must start, known before any of them is downloaded: its data ends where the next
+    # local header (or the central directory) begins, less the data descriptor torch's zip writer puts after every
+    # non-empty record (ZIP64-sized from 4 GiB on).  Each local header is checked against this as it arrives.
+    for r, nxt in zip(records, [r.local for r in records[1:]] + [cd_off]):
+        desc = 0 if not r.flags & 8 else 24 if r.local >= 0xFFFFFFFF or r.size >= 0xFFFFFFFF else 16
+        r.data = nxt - desc - r.size
+    head_end = min([r.local for r in data.values()] + [cd_off])
+    # the small records after the data records (torch.save: version, .data/serialization_id) end up in the end piece
+    await extend_end(min([r.local for n, r in rel.items() if n not in data and r.local > head_end], default=end_at))
+    pieces = [(end_at, end)]
+    if head_end >= end_at:
+        await extend_end(0)
+        pieces = [(0, end)]
+    elif head_end:
+        pieces.insert(0, (0, bytearray(await _read_range_host(client, volume_id, path, 0, head_end))))
+    sk = device_file._Skeleton(pieces)
+    small = {}
+    for n, r in rel.items():
+        if n not in data:
+            r.data = device_file._local_data_offset(sk, r)
+            if r.local < head_end and r.data + r.size > head_end:
+                raise ValueError(f"{path}: record {r.name!r} runs into the data records")
+            small[n] = sk.read(r.data, r.size)
+    bad = _crc_mismatches((rel[n], zlib.crc32(b)) for n, b in small.items())
+    if bad:
+        raise ExecutionError(f"{path}: CRC-32 mismatch in " + ", ".join(bad))
+    _check_format_version(path, prefix, small)
+    if small.get("byteorder", b"little") != b"little":
+        raise ValueError(f"{path}: byteorder {small['byteorder']!r} is not supported (only little-endian archives)")
+
+    reader = _ArchiveRecords(small, data, ctx)
+    loader = torch.serialization._weights_only_unpickler if weights_only else pickle
+    obj = torch.serialization._load(reader, lambda storage, _location: storage, loader, encoding="utf-8")
+
+    loads = sorted(((data[n], t) for n, t in reader.storages.items() if t.numel()), key=lambda e: e[0].local)
+    for r, _ in loads:
+        if r.data % 16:
+            raise ValueError(f"{path}: the data of {r.name!r} starts at {r.data}, which is not 16-byte aligned")
+    if not loads:
+        return obj
+    span_at = loads[0][0].local & ~15  # 16-aligned, so that every storage sits 16-aligned in its block slot
+    span_end = loads[-1][0].data + loads[-1][0].size
+    slices = await _block_slices(client, volume_id, path, span_at, span_end - span_at)
+    dst = DeviceFile._over(DeviceFile._Source([t for _, t in loads], BOUNCE_BYTES))
+    plan = _StorageWaves(path, [r for r, _ in loads], span_at)
+    await _load_in_waves(slices, dst, plan, staging_bytes, None, lambda **_: None)
+    checked = [(r, t) for r, t in loads if r.crc]
+    if checked:
+        crc = DeviceFile._Source._empty(4 * len(checked), ctx).view(torch.int32)
+        ctx.crc32_device([t.data_ptr() for _, t in checked], [t.numel() for _, t in checked], crc.data_ptr(),
+                         DeviceFile._Source._current_stream(ctx))
+        bad = _crc_mismatches(zip([r for r, _ in checked], crc.cpu().numpy().view(np.uint32).tolist()))
+        if bad:
+            raise ExecutionError(f"{path}: CRC-32 mismatch in " + ", ".join(bad))
+    return obj
 
 
 # ---------------------------------------------------------------------------------- the reference's names

@@ -11,6 +11,13 @@
     (read_file_into_fileobj into BytesIO, safetensors.torch.load, .to("cuda") per tensor), alternating, VRB_E2E_REPS
     (2) runs each; host clock from call to a synchronised result, and the peak growth of the process's resident set
     during the call (sampled every 2 ms).  The results are compared tensor by tensor.
+(c) the same for a torch.save training checkpoint of VRB_E2E_GIB, uploaded once with DeviceFile.torch_save: a state
+    dict shaped as in (b) plus an Adam state dict (``exp_avg`` / ``exp_avg_sq`` of the small tensors, CPU ``step``
+    tensors), read with read_torch_save against read_file_into_fileobj into BytesIO + torch.load(map_location="cuda"),
+    alternating, timed and compared bitwise as in (b).  Then the CRC launch alone (one crc32_device call over the loaded
+    storages, CUDA events, best of VRB_REPS) against the load_ranges time of arm (a), when it ran.
+
+VRB_ARMS (default "abc") picks the arms.
 
 The card name and power limit are read in the same run.  Needs a GPU: nothing here falls back.
 One JSON line per arm; also written to $VRB_OUT/volume_read_bench.json when set."""
@@ -175,15 +182,110 @@ async def e2e_arm(info, out):
             print(json.dumps(out[-1]), flush=True)
 
 
+def training_checkpoint(total: int, seed: int = 2) -> dict:
+    """``state_dict(total)`` as the model, and the Adam state of its small tensors after one step."""
+    sd = state_dict(total, seed)
+    small = [k for k in sd if not k.startswith("mat.")]
+    params = [torch.nn.Parameter(sd[k].float()) for k in small]
+    opt = torch.optim.Adam(params, lr=1e-3)
+    for p in params:
+        p.grad = torch.ones_like(p)
+    opt.step()
+    return {"model": sd, "optim": opt.state_dict(), "step": 1}
+
+
+def _flat(obj, at=""):
+    if isinstance(obj, torch.Tensor):
+        yield at, obj
+    elif isinstance(obj, dict):
+        for k, v in obj.items():
+            yield from _flat(v, f"{at}/{k}")
+    elif isinstance(obj, (list, tuple)):
+        for i, v in enumerate(obj):
+            yield from _flat(v, f"{at}/{i}")
+
+
+def _bitwise_equal(a, b) -> bool:
+    fa, fb = list(_flat(a)), list(_flat(b))
+    return [k for k, _ in fa] == [k for k, _ in fb] and all(
+        x.device == y.device and x.dtype == y.dtype and x.shape == y.shape and x.stride() == y.stride() and
+        torch.equal(x.reshape(-1).view(torch.uint8), y.reshape(-1).view(torch.uint8)) for (_, x), (_, y) in zip(fa, fb))
+
+
+async def torch_save_arm(ctx, info, out):
+    import io
+
+    ckpt = training_checkpoint(int(float(os.environ.get("VRB_E2E_GIB", "1")) * GiB))
+    async with running_volume_server(blob_utils.BLOCK_SIZE) as (stub, _):
+        client = types.SimpleNamespace(stub=stub)
+        batch = volume.VolumeUploadContextManager2("vo-b", client)
+        async with batch:
+            batch.put_file(DeviceFile.torch_save(ckpt), "/ckpt.pt")
+        size = len(stub.volume_files["/ckpt.pt"][0])
+        want = torch.load(io.BytesIO(stub.volume_files["/ckpt.pt"][0]), map_location="cuda")
+
+        async def ours():
+            got = await volume.read_torch_save(client, "vo-b", "/ckpt.pt")
+            torch.cuda.synchronize()
+            return got
+
+        async def reference_route():
+            buf = io.BytesIO()
+            await volume.read_file_into_fileobj(client, "vo-b", "/ckpt.pt", buf)
+            buf.seek(0)
+            got = torch.load(buf, map_location="cuda")
+            del buf
+            torch.cuda.synchronize()
+            return got
+
+        res = {"read_torch_save": [], "fileobj_torch_load_cuda": []}
+        for _ in range(int(os.environ.get("VRB_E2E_REPS", "2"))):
+            for arm, fn in (("read_torch_save", ours), ("fileobj_torch_load_cuda", reference_route)):
+                with PeakRss() as rss:
+                    t0 = time.perf_counter()
+                    got = await fn()
+                    dt = time.perf_counter() - t0
+                equal = _bitwise_equal(got, want)
+                if arm == "read_torch_save":
+                    kept = got
+                del got
+                res[arm].append((dt, rss.growth, equal))
+        for arm, v in res.items():
+            ts = [t for t, _, _ in v]
+            out.append({"arm": f"torch_save_loopback.{arm}", "bytes": size, "median_s": round(statistics.median(ts), 3),
+                        "range_s": [round(min(ts), 3), round(max(ts), 3)],
+                        "peak_rss_growth_GB": round(max(g for _, g, _ in v) / 1e9, 3),
+                        "bitwise_equal_to_torch_load": all(e for _, _, e in v), **info})
+            print(json.dumps(out[-1]), flush=True)
+    storages = {t.untyped_storage().data_ptr(): t.untyped_storage() for _, t in _flat(kept) if t.untyped_storage().nbytes()}
+    ptrs, lens = list(storages), [st.nbytes() for st in storages.values()]
+    crc = torch.empty(len(ptrs), dtype=torch.int32, device="cuda")
+    stream = torch.cuda.current_stream().cuda_stream or 1
+    launch = lambda: ctx.crc32_device(ptrs, lens, crc.data_ptr(), stream)  # noqa: E731
+    launch()
+    ms = [events_ms(launch) for _ in range(int(os.environ.get("VRB_REPS", "5")))]
+    load = next((o for o in out if o["arm"] == "kernel.load_ranges"), None)
+    row = {"arm": "torch_save.crc32_device", "storages": len(ptrs), "bytes": sum(lens), "best_ms": round(min(ms), 3),
+           "median_ms": round(statistics.median(ms), 3), "GB_s": round(sum(lens) / min(ms) / 1e6, 2)}
+    if load is not None:  # load_ranges of arm (a) scaled to these bytes
+        row["share_of_load_ranges_at_arm_a_rate"] = round(min(ms) / (sum(lens) / (load["GB_s"] * 1e6)), 4)
+    out.append({**row, **info})
+    print(json.dumps(out[-1]), flush=True)
+
+
 def main():
     if not torch.cuda.is_available():
         raise SystemExit("volume_read_bench needs a GPU")
     info = gpu_info()
     ctx = _lib.Context(0, pinned_bytes=64 << 20, device_bytes=512 << 20)
     _backend.set_context(ctx)
-    out = []
-    kernel_arm(ctx, info, out)
-    asyncio.run(e2e_arm(info, out))
+    out, arms = [], os.environ.get("VRB_ARMS", "abc")
+    if "a" in arms:
+        kernel_arm(ctx, info, out)
+    if "b" in arms:
+        asyncio.run(e2e_arm(info, out))
+    if "c" in arms:
+        asyncio.run(torch_save_arm(ctx, info, out))
     if os.environ.get("VRB_OUT"):
         os.makedirs(os.environ["VRB_OUT"], exist_ok=True)
         with open(os.path.join(os.environ["VRB_OUT"], "volume_read_bench.json"), "w") as fh:
