@@ -230,6 +230,36 @@ int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint6
                                 uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, const void* h_src,
                                 uint64_t h_src_bytes, const uint64_t* src_offsets, void* cuda_stream);
 
+/* A box of a host buffer: `rows` rows of `width` bytes, row r at h_src + src_offset + r * src_pitch (any byte phase),
+ * written packed to bytes [offset, offset + rows * width) of file `file` of a segmented batch. */
+typedef struct b200h_box {
+    uint64_t file, offset;
+    uint64_t width, rows;
+    uint64_t src_offset, src_pitch;
+} b200h_box;
+
+/* Like b200h_copy_ranges_from_host, for strided sources: box i of h_src is written packed to its destination run of
+ * files that live in device memory as many buffers, described as there (segs, file_first_seg; host arrays).  A box's
+ * run may cross any number of segments; rows * width == 0 copies nothing.  `boxes` is a host array.  Neither h_src
+ * nor the sources need any alignment (h_src may be a view into what b200h_host_alloc returns), and sources may overlap.
+ * Every argument is checked before any work is enqueued, B200H_E_INVALID otherwise: the rules of the segment-parts entry
+ * for segs / file_first_seg, file < nfiles, the destination inside its file and the last source byte inside
+ * h_src_bytes (both without overflow), src_pitch >= width when rows > 1, h_src page-locked host memory the context's
+ * device can reach (cudaPointerGetAttributes), and no device byte written by two boxes (checked on the resolved device
+ * addresses).
+ * ONE kernel launch (load_boxes_kernel) per call, none when every box is empty; the tables it uploads grow with the
+ * boxes and their 64 KiB tiles of source words, never with the rows, which the kernel expands.  It reads h_src straight
+ * over PCIe, every source byte that lands once, in aligned 16-byte loads inside the 16-byte hull of its row; bytes
+ * between rows are read only inside those words.  Device stores are full aligned 16-byte words except at the ends of a
+ * box's run, at segment edges and at one word per 64 KiB tile.  Device bytes outside every box are not written.
+ * The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream), as the range entries do: h_src must
+ * stay unchanged, and the device bytes are there, once the work enqueued on the stream has completed.
+ * Replaces: _read_file_into_fileobj (py/modal/volume.py:923-1000) followed by the host-side get_slice of the
+ * safetensors library and a per-tensor .to("cuda"), to give each tensor-parallel rank its slice of a checkpoint. */
+int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                               uint64_t nfiles, const b200h_box* boxes, uint64_t nboxes, const void* h_src,
+                               uint64_t h_src_bytes, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

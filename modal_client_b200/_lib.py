@@ -34,7 +34,7 @@ ABI_SYMBOLS = (
     "b200h_last_outlier_count", "b200h_hash_batch_device_hl", "b200h_combine_stats", "b200h_plan_sync_count",
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
-    "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host",
+    "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host", "b200h_copy_boxes_from_host",
 )
 
 
@@ -114,6 +114,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_copy_ranges_to_host.restype = i32
         L.b200h_copy_ranges_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
         L.b200h_copy_ranges_from_host.restype = i32
+        L.b200h_copy_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
+        L.b200h_copy_boxes_from_host.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -452,6 +454,21 @@ class Context:
         ``stream``: ``src`` must stay unchanged until that stream's work has completed."""
         self._copy_ranges("b200h_copy_ranges_from_host", "src_offsets", seg_ptrs, seg_lens, file_first_seg, ranges, src,
                           src_offsets, stream)
+
+    def copy_boxes_from_host(self, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray, stream: int = 0) -> None:
+        """Write boxes of ``src`` (a uint8 array over page-locked memory from ``host_alloc``) packed into files made of
+        device buffers (described as for ``hash_segment_parts_device``): box i = ``(file, offset, width, rows,
+        src_offset, src_pitch)`` writes ``rows`` rows of ``width`` bytes, row r from ``src[src_offset + r *
+        src_pitch:]`` (any alignment), to bytes ``[offset, offset + rows * width)`` of its file; no device byte may
+        belong to two boxes.  One kernel launch, only enqueued on ``stream``: ``src`` must stay unchanged until that
+        stream's work has completed."""
+        segs = _segments(seg_ptrs, seg_lens)
+        ffs, nfiles = _segment_args(file_first_seg)
+        bx = np.ascontiguousarray(boxes, dtype=np.uint64).reshape(-1, 6)
+        rc = self._L.b200h_copy_boxes_from_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
+                                                nfiles, _np_ptr(bx) if len(bx) else None, len(bx),
+                                                ctypes.c_void_p(src.ctypes.data), src.size, stream or None)
+        self._check(rc, "b200h_copy_boxes_from_host")
 
     def _copy_ranges(self, entry: str, offsets_name: str, seg_ptrs, seg_lens, file_first_seg, ranges, host: np.ndarray,
                      host_offsets, stream: int) -> None:

@@ -1557,6 +1557,102 @@ int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint6
                        cuda_stream);
 }
 
+int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                               uint64_t nfiles, const b200h_box* boxes, uint64_t nboxes, const void* h_src,
+                               uint64_t h_src_bytes, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_boxes_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    std::vector<uint64_t> seg_lens;
+    FileTable t;
+    if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
+    if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
+    if (nboxes && !h_src) return fail(ctx, B200H_E_INVALID, "h_src must not be NULL");
+    bool any = false;
+    for (uint64_t i = 0; i < nboxes; ++i) {
+        const b200h_box& b = boxes[i];
+        const std::string name = "box " + std::to_string(i);
+        if (b.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
+        if (b.width && b.rows > ~0ull / b.width) return fail(ctx, B200H_E_INVALID, name + ": rows * width overflows");
+        const uint64_t n = b.rows * b.width;
+        if (b.offset > t.size[b.file] || n > t.size[b.file] - b.offset)
+            return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
+        if (b.rows > 1 && b.src_pitch < b.width) return fail(ctx, B200H_E_INVALID, name + ": src_pitch is less than width");
+        if (!n) continue;
+        // src_offset + (rows - 1) * src_pitch + width <= h_src_bytes, without overflow
+        const bool fits = (b.rows == 1 || b.src_pitch <= h_src_bytes / (b.rows - 1)) &&
+                          b.width <= h_src_bytes - (b.rows - 1) * b.src_pitch &&
+                          b.src_offset <= h_src_bytes - (b.rows - 1) * b.src_pitch - b.width;
+        if (!fits) return fail(ctx, B200H_E_INVALID, name + ": its source reaches past h_src_bytes");
+        any = true;
+    }
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
+    if (nboxes == 0) return 0;
+    void* d_host = pinned_device_pointer(ctx, h_src, h_src_bytes);
+    if (!d_host)
+        return fail(ctx, B200H_E_INVALID,
+                    "h_src is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
+    if (!any) return 0;
+
+    // h_src may sit at any phase (a view into page-locked memory): the kernel reads aligned words from the aligned-down
+    // base, so every source offset in the tables is taken from there.  The words it reads hold selected bytes, so they
+    // lie in the same page-locked pages as the bytes themselves.
+    const uint64_t phase = (uintptr_t)d_host & 15u;
+    // pieces (box x segment, in destination order within a box; `host` = offset in the box's packed run) and the tiles
+    // of every box's virtual source words (see BoxTile): neither grows with the rows
+    std::vector<RangePiece> pieces;
+    std::vector<BoxTile> tiles;
+    std::vector<uint64_t> box_of;  // per piece: the box it belongs to (for the overlap message)
+    for (uint64_t i = 0; i < nboxes; ++i) {
+        const b200h_box& bx = boxes[i];
+        const uint64_t n = bx.rows * bx.width;
+        if (!n) continue;
+        BoxTile b{};
+        const bool run = bx.rows == 1 || bx.src_pitch == bx.width;  // one contiguous source run
+        b.src = bx.src_offset + phase;
+        b.width = run ? n : bx.width;
+        b.rows = run ? 1 : bx.rows;
+        b.pitch = run ? n : bx.src_pitch;
+        b.hull = b.pitch - b.width < 16 ? 0 : ((b.width + 14) >> 4) + 1;
+        const uint64_t last = b.src + (b.rows - 1) * b.pitch;  // the last row's first source byte
+        const uint64_t nv = b.hull ? (b.rows - 1) * b.hull + ((last + b.width - 1) >> 4) - (last >> 4) + 1
+                                   : ((last + b.width - 1) >> 4) - (b.src >> 4) + 1;
+        const size_t first = pieces.size();
+        uint64_t at = 0;
+        file_pieces(t, bx.file, bx.offset, n, [&](uint64_t s, uint64_t in, uint64_t len) {
+            pieces.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in, at, len});
+            box_of.push_back(i);
+            at += len;
+        });
+        size_t p = first;
+        for (uint64_t v0 = 0; v0 < nv; v0 += kStageTileBytes / 16) {
+            b.v0 = v0;
+            b.nv = (uint32_t)std::min(kStageTileBytes / 16, nv - v0);
+            b.dlo = box_dest_at(b, v0);
+            b.dhi = v0 + b.nv == nv ? n : box_dest_at(b, v0 + b.nv);
+            while (pieces[p].host + pieces[p].len <= b.dlo) ++p;
+            size_t q = p;
+            while (q + 1 < pieces.size() && pieces[q + 1].host < b.dhi) ++q;
+            b.first_piece = p;
+            b.npieces = (uint32_t)(q - p + 1);
+            tiles.push_back(b);
+        }
+    }
+    // no device byte may be written twice: two files, or two segments of one file, may share a tensor
+    std::vector<size_t> by_dev(pieces.size());
+    for (size_t k = 0; k < by_dev.size(); ++k) by_dev[k] = k;
+    std::sort(by_dev.begin(), by_dev.end(), [&](size_t a, size_t b) { return pieces[a].dev < pieces[b].dev; });
+    for (size_t k = 1; k < by_dev.size(); ++k)
+        if (pieces[by_dev[k - 1]].dev + pieces[by_dev[k - 1]].len > pieces[by_dev[k]].dev)
+            return fail(ctx, B200H_E_INVALID, "boxes " + std::to_string(box_of[by_dev[k - 1]]) + " and " +
+                                                  std::to_string(box_of[by_dev[k]]) + " write the same device bytes");
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    return launch_with_tables(ctx, st, tiles, pieces, [&](const BoxTile* d_tiles, const RangePiece* d_pieces) {
+        return launch_load_boxes(d_tiles, tiles.size(), d_pieces, (const uint8_t*)d_host - phase, st);
+    });
+}
+
 // ---------------------------------------------------------------------------------------------- files
 
 int b200h_stat_files(b200h_ctx* ctx, const char* const* paths, uint64_t n, uint64_t* sizes_out, uint32_t* modes_out) {

@@ -123,6 +123,39 @@ int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiec
 // The inverse, host -> device; `src` is 16-byte aligned memory the device can load from.
 int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
 
+// Boxes of a host buffer copied into segmented device files (load_boxes_kernel, b200hash_stage.cu).  A box is `rows`
+// rows of `width` bytes, row r at byte src + r * pitch of the host buffer, packed into one destination run.  Its source
+// is read as a stream of aligned 16-byte "virtual" words: when pitch - width < 16 the rows' hulls touch and every word
+// of the box's source span is read once (hull == 0: virtual word v is word (src >> 4) + v); otherwise the hulls are
+// disjoint and row r owns the `hull` virtual words r * hull + k, holding words ((src + r * pitch) >> 4) + k, the last
+// one empty when the row's phase needs one word less.  A tile is up to kStageTileBytes / 16 consecutive virtual words of
+// one box; it writes the packed destination bytes [dlo, dhi) whose source lies in its words, through the pieces
+// [first_piece, first_piece + npieces) of the box's destination (RangePiece; `host` is the piece's offset in the run).
+struct BoxTile {
+    uint64_t src, pitch, width, rows, hull;  // the box (rows == 1 or pitch >= width); src from the aligned base
+    uint64_t v0;                             // first virtual word
+    uint64_t dlo, dhi;                       // packed destination bytes written
+    uint64_t first_piece;
+    uint32_t nv, npieces;  // virtual words; pieces
+};
+// The first packed destination byte of the box whose source lies in virtual word v or later (rows * width if none).
+__host__ __device__ inline uint64_t box_dest_at(const BoxTile& b, uint64_t v) {
+    if (b.hull) {
+        const uint64_t r = v / b.hull, k = v % b.hull;
+        if (r >= b.rows) return b.rows * b.width;
+        const uint64_t s = b.src + r * b.pitch, x = (s >> 4) + k;
+        if (x > ((s + b.width - 1) >> 4)) return (r + 1) * b.width;
+        return r * b.width + (x * 16 > s ? x * 16 - s : 0);
+    }
+    if (v == 0) return 0;
+    const uint64_t t = ((b.src >> 4) + v) * 16 - b.src, r = t / b.pitch, c = t % b.pitch;
+    if (r >= b.rows) return b.rows * b.width;
+    return c >= b.width ? (r + 1) * b.width : r * b.width + c;
+}
+// Every tile's copy host -> device, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device can
+// load from (the tiles' source offsets count from it).
+int launch_load_boxes(const BoxTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
+
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)
 cudaError_t configure_kernels();  // one-time cudaFuncSetAttribute calls for the current device

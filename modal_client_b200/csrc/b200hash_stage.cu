@@ -236,7 +236,134 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
     }
 }
 
+// ---- boxes: rows of a page-locked host buffer, `pitch` bytes apart, packed into segmented device files
+//
+//   load_boxes_kernel    persistent CTAs whose warps take tiles of a box's virtual source words (BoxTile), tile t on
+//                        CTA t % gridDim.x so that a call with few tiles still spreads over every SM.  Lane k of a
+//                        chunk loads virtual word 128 * chunk + 32 * i + k (i < kLoadChunks) with one aligned 16-byte
+//                        load, so every source byte that lands crosses PCIe once and no load leaves its row's hull (the
+//                        bytes between rows are read only inside the hull words, or, when rows are less than 16 bytes
+//                        apart, because every such byte lies in one).  The loads run two chunks ahead in registers,
+//                        so they are in flight while the warp stores the current chunk; a chunk goes to the warp's
+//                        ring in shared memory (two chunks) when its turn comes.
+//                        The warp stores every destination word whose last byte's source has arrived: an aligned
+//                        device word of one piece, built from two ring words and shift_bytes when its 16 bytes are one
+//                        run of one row, byte by byte from the ring otherwise (a word across rows; narrow rows).  A
+//                        destination word's bytes come from at most 33 consecutive virtual words, so the previous
+//                        chunk is still in the ring.  Words are stored whole except at the run's ends, at piece edges
+//                        and at the seam of two tiles, where each tile stores the bytes its words hold.
+
+constexpr uint32_t kBoxChunk = 32 * kLoadChunks;  // virtual words loaded per warp and step
+constexpr uint32_t kBoxRing = 2 * kBoxChunk;
+// 64-bit row arithmetic needs more than the 64 registers of 4 CTAs per SM; 16 warps of 2 KiB loads each per SM still
+// keep far more in flight than PCIe's bandwidth-delay product
+constexpr int kBoxCtasPerSm = 2;
+
+// The virtual word of source byte s, which lies in row r of the box.
+__device__ __forceinline__ uint64_t box_virtual(const BoxTile& b, uint64_t r, uint64_t s) {
+    return b.hull ? r * b.hull + (s >> 4) - ((b.src + r * b.pitch) >> 4) : (s >> 4) - (b.src >> 4);
+}
+
+// Lane `lane`'s words of the chunk that starts at virtual word b.v0 + c (zero where a row's last slot is empty).
+__device__ __forceinline__ void box_load_chunk(const BoxTile& b, const uint4* words, uint32_t c, uint32_t lane,
+                                               uint4 (&v)[kLoadChunks]) {
+#pragma unroll
+    for (int i = 0; i < kLoadChunks; ++i) {
+        const uint32_t j = c + i * 32 + lane;
+        v[i] = make_uint4(0, 0, 0, 0);
+        if (j < b.nv) {
+            const uint64_t g = b.v0 + j;
+            if (b.hull) {
+                const uint64_t r = g / b.hull, s = b.src + r * b.pitch, x = (s >> 4) + g % b.hull;
+                if (x <= (s + b.width - 1) >> 4) v[i] = __ldg(words + x);
+            } else {
+                v[i] = __ldg(words + (b.src >> 4) + g);
+            }
+        }
+    }
+}
+
+// Destination words of piece `pc` whose bytes (clipped to the piece and to [b.dlo, b.dhi)) end in [from, upto).
+// Word bounds are compared as device addresses: a piece's first word may begin before its packed offset 0.
+__device__ __forceinline__ void box_words_out(const BoxTile& b, const RangePiece pc, const uint4* ring, uint64_t from,
+                                              uint64_t upto, uint32_t lane) {
+    const uint64_t qlo = max(pc.host, b.dlo), qhi = min(pc.host + pc.len, b.dhi);
+    const uint64_t lo = max(from, qlo), hi = min(upto, qhi);
+    if (lo >= hi) return;
+    const uint64_t base = pc.dev - pc.host;  // device address of packed byte d: base + d (mod 2^64)
+    const uint64_t qa = base + qlo, qe = base + qhi, ha = base + hi;
+    // a word whose bytes go on past `hi` waits for the next step
+    const uint64_t w1 = hi < qhi ? ha >> 4 : ((ha - 1) >> 4) + 1;
+    for (uint64_t w = ((base + lo) >> 4) + lane; w < w1; w += 32) {
+        const uint64_t ws = w * 16, aa = max(ws, qa), ea = min(ws + 16, qe);
+        const uint32_t jlo = (uint32_t)(aa - ws), jhi = (uint32_t)(ea - ws);
+        const uint64_t a = aa - base;
+        uint64_t r = a / b.width, c = a % b.width;
+        uint4 v;
+        if (jhi - jlo == 16 && c + 16 <= b.width) {
+            const uint64_t s = b.src + r * b.pitch + c;
+            const uint32_t slot = (uint32_t)(box_virtual(b, r, s) - b.v0), sh = (uint32_t)s & 15u;
+            const uint4 w0 = ring[slot % kBoxRing];
+            v = sh ? shift_bytes(w0, ring[(slot + 1) % kBoxRing], sh) : w0;
+        } else {
+            uint64_t x[2] = {0, 0};
+#pragma unroll 1
+            for (uint32_t j = jlo; j < jhi; ++j) {
+                const uint64_t s = b.src + r * b.pitch + c;
+                const uint8_t* word =
+                    reinterpret_cast<const uint8_t*>(ring + (uint32_t)(box_virtual(b, r, s) - b.v0) % kBoxRing);
+                const uint64_t byte = (uint64_t)word[s & 15u] << (8 * (j & 7));
+                if (j < 8) x[0] |= byte;
+                else x[1] |= byte;
+                if (++c == b.width) c = 0, ++r;
+            }
+            v = make_uint4((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
+        }
+        store_bytes(reinterpret_cast<uint8_t*>(ws), v, jlo, jhi);
+    }
+}
+
+__global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
+    load_boxes_kernel(const BoxTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
+                      const uint8_t* __restrict__ src) {
+    __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
+    const uint32_t lane = threadIdx.x & 31u;
+    uint4* ring = rings[threadIdx.x >> 5];
+    const uint4* words = reinterpret_cast<const uint4*>(src);
+    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
+    for (uint64_t t = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; t < ntiles; t += nwarps) {
+        const BoxTile b = tiles[t];
+        const RangePiece* __restrict__ pc = pieces + b.first_piece;
+        uint64_t from = b.dlo;
+        uint4 v[kLoadChunks], u[kLoadChunks];  // chunks c and c + 1, loaded
+        box_load_chunk(b, words, 0, lane, v);
+        box_load_chunk(b, words, kBoxChunk, lane, u);
+        for (uint32_t c = 0; c < b.nv; c += kBoxChunk) {
+            // the ring's other half holds chunk c - 1, which this step's words may still need
+#pragma unroll
+            for (int i = 0; i < kLoadChunks; ++i) {
+                ring[(c + i * 32 + lane) % kBoxRing] = v[i];
+                v[i] = u[i];
+            }
+            __syncwarp();
+            box_load_chunk(b, words, c + 2 * kBoxChunk, lane, u);
+            const uint64_t upto = c + kBoxChunk >= b.nv ? b.dhi : box_dest_at(b, b.v0 + c + kBoxChunk);
+            for (uint32_t q = 0; q < b.npieces; ++q) box_words_out(b, pc[q], ring, from, upto, lane);
+            __syncwarp();
+            from = upto;
+        }
+    }
+}
+
 }  // namespace
+
+int launch_load_boxes(const BoxTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
+    load_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
+                                                                                   static_cast<const uint8_t*>(src));
+    return 1;
+}
 
 int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
     if (!ntiles) return 0;

@@ -23,7 +23,9 @@ them.
 device files into a page-locked buffer with ONE ``b200h_copy_ranges_to_host`` call, after which the tensors are not
 needed for those bytes.  The volumefs2 uploader uses it for the missing blocks when it is given
 ``device_staging_bytes``.  ``load_ranges(files, ranges, src, src_offsets)`` is the way back: ranges of a page-locked
-buffer into the files' tensors with ONE ``b200h_copy_ranges_from_host`` call (``volume.read_file_into_device``).
+buffer into the files' tensors with ONE ``b200h_copy_ranges_from_host`` call (``volume.read_file_into_device``), and
+``load_boxes(files, boxes, src)`` the strided form: rows of a page-locked buffer, any distance apart and at any phase,
+packed into the files with ONE ``b200h_copy_boxes_from_host`` call (``volume.read_safetensors_slices``).
 """
 from __future__ import annotations
 
@@ -329,6 +331,31 @@ def load_ranges(files: list["DeviceFile"], ranges, src: np.ndarray, src_offsets,
     with lead._on_stream():
         ctx.copy_ranges_from_host(ptrs, lens, first, ranges, src, offsets, lead.stream_handle)
     return Loaded(lead._publish())  # outside the block: the caller's current stream is the one that waits
+
+
+def load_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> Loaded:
+    """Write boxes of ``src`` -- a uint8 array over page-locked memory from ``ctx.host_alloc`` -- into device files:
+    box i = ``(index into files, offset, width, rows, src_offset, src_pitch)`` writes ``rows`` rows of ``width`` bytes,
+    row r from ``src[src_offset + r * src_pitch:]`` (no alignment needed; ``src_pitch >= width`` when ``rows > 1``),
+    packed into bytes ``[offset, offset + rows * width)`` of its file; no device byte may belong to two boxes.  ONE
+    ``b200h_copy_boxes_from_host`` call (one kernel launch, none when every box is empty), ordered as ``load_ranges``:
+    on the first file's stream, after every file's stream and the current stream, and the current stream then waits
+    for the copy.  Returns at once; ``wait()`` on the result blocks until the kernel has read ``src``."""
+    ctx = ctx or get_context()
+    sources = [f._src for f in files]
+    boxes = [tuple(int(x) for x in b) for b in boxes]
+    if any(len(b) != 6 for b in boxes):
+        raise ValueError("a box is (file, offset, width, rows, src_offset, src_pitch)")
+    if boxes and not sources:
+        raise ValueError("boxes without files")
+    if not sources:
+        return Loaded(None)
+    lead = sources[0]
+    lead._after_current()
+    ptrs, lens, first = _file_table(sources)
+    with lead._on_stream():
+        ctx.copy_boxes_from_host(ptrs, lens, first, boxes, src, lead.stream_handle)
+    return Loaded(lead._publish())
 
 
 # ------------------------------------------------------------------------------------------ safetensors
@@ -839,5 +866,5 @@ class DeviceFile(io.RawIOBase):
         return f"<DeviceFile {self._src.nbytes} bytes in {len(segs)} segments on {segs[0].device}>"
 
 
-__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "Staged", "hash_parts_many", "load_ranges", "safetensors_layout",
-           "stage_ranges"]
+__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "Staged", "hash_parts_many", "load_boxes", "load_ranges",
+           "safetensors_layout", "stage_ranges"]

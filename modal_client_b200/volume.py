@@ -17,8 +17,9 @@ there, so the tensors are free again (``device_released``) after the last copy i
 The way back (counterparts of ``Volume.read_file`` / ``read_file_into_fileobj``, py/modal/volume.py:878-1000):
 ``read_file`` and ``read_file_into_fileobj`` through host memory, ``read_file_into_device`` straight into the tensors
 of a ``DeviceFile`` (blocks downloaded into page-locked memory, a wave per ``load_ranges`` call), and
-``read_safetensors``, a safetensors checkpoint back into CUDA tensors without a host copy of the file, and
-``read_torch_save``, a torch.save checkpoint back into CUDA storages, its zip CRC-32s checked on the device.
+``read_safetensors``, a safetensors checkpoint back into CUDA tensors without a host copy of the file,
+``read_safetensors_slices``, slices of its tensors (a tensor-parallel rank's rows or columns) downloading only the blocks
+they touch, and ``read_torch_save``, a torch.save checkpoint back into CUDA storages, its zip CRC-32s checked on the device.
 """
 from __future__ import annotations
 
@@ -38,7 +39,7 @@ from . import _wire, blob_utils, device_file
 from ._logging import logger
 from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
-from .device_file import BOUNCE_BYTES, DeviceFile, _st_dtypes, load_ranges, stage_ranges
+from .device_file import BOUNCE_BYTES, DeviceFile, _st_dtypes, load_boxes, load_ranges, stage_ranges
 from .exception import ExecutionError, ServiceError
 from .http_utils import ClientSessionRegistry
 
@@ -534,19 +535,20 @@ async def read_file_into_device(client, volume_id: str, path: str, dst: DeviceFi
         await _get_file2(client, volume_id, path, start, 1)  # the file must exist; nothing else to do
         return 0
     slices = await _block_slices(client, volume_id, path, start, n)
-    await _load_in_waves(slices, dst, lambda wave, at, _: ([(0, off, m) for _, off, m in wave], at), staging_bytes,
-                         concurrency, progress_cb)
+    await _load_in_waves(slices, lambda wave, at, buf, ctx: load_ranges([dst], [(0, off, m) for _, off, m in wave], buf,
+                                                                        at, ctx=ctx),
+                         staging_bytes, concurrency, progress_cb)
     return n
 
 
-async def _load_in_waves(slices, dst: DeviceFile, plan, staging_bytes: int, concurrency: int | None,
+async def _load_in_waves(slices, load, staging_bytes: int, concurrency: int | None,
                          progress_cb: Callable[..., Any]) -> None:
-    """Download ``slices`` (``_block_slices``) into ``dst``: every block goes to its own ``BLOCK_SIZE`` slot of a
+    """Download ``slices`` (``_block_slices``) to the device: every block goes to its own ``BLOCK_SIZE`` slot of a
     page-locked buffer (``ctx.host_alloc``) of two halves, a wave per half; when a wave is complete,
-    ``plan(wave, at, buf)`` -- the wave's slices, their offsets in the buffer and the buffer -- gives the
-    ``(ranges, src_offsets)`` of its one ``load_ranges`` call.  A half is refilled only after its previous copy has read
-    it, so ``plan`` may still read the previous wave's slots; every copy has read the buffer before it is freed, however
-    the call ends."""
+    ``load(wave, at, buf, ctx)`` -- the wave's slices, their offsets in the buffer, the buffer and the context -- makes
+    its one copy (``load_ranges`` or ``load_boxes``) and returns the ``Loaded``.  A half is refilled only after its
+    previous copy has read it, so ``load`` may still read the previous wave's slots; every copy has read the buffer
+    before it is freed, however the call ends."""
     BS = blob_utils.BLOCK_SIZE
     per_half = staging_bytes // 2 // BS  # block slots per half (every slot starts at a multiple of BLOCK_SIZE)
     semaphore = asyncio.Semaphore(concurrency or os.cpu_count() or 1)
@@ -566,8 +568,7 @@ async def _load_in_waves(slices, dst: DeviceFile, plan, staging_bytes: int, conc
                 progress_cb(advance=m)
 
             await gather_cancel_on_error(*[fetch(url, m, a) for (url, _, m), a in zip(wave, at)])
-            ranges, src_offsets = plan(wave, at, buf)
-            loaded[half] = load_ranges([dst], ranges, buf, src_offsets, ctx=ctx)
+            loaded[half] = load(wave, at, buf, ctx)
     finally:
         for pending in loaded:  # the copies must have read the buffer before it is freed
             if pending is not None:
@@ -576,8 +577,8 @@ async def _load_in_waves(slices, dst: DeviceFile, plan, staging_bytes: int, conc
 
 
 def _safetensors_entries(header: bytes, data_len: int):
-    """[(name, torch dtype, torch shape, start, end), ...] in data order, checked as the safetensors library checks a
-    header (a valid JSON object, known dtype tags, ``shape x element size`` = span, ``data_offsets`` tiling the data
+    """(``__metadata__`` or None, [(name, torch dtype, torch shape, start, end), ...] in data order), checked as the
+    safetensors library checks a header (a valid JSON object, known dtype tags, ``shape x element size`` = span, ``data_offsets`` tiling the data
     region of ``data_len`` bytes without holes or overlap); ``ValueError`` otherwise."""
     try:
         meta = json.loads(header.decode("utf-8"))
@@ -619,22 +620,25 @@ def _safetensors_entries(header: bytes, data_len: int):
         at = hi
     if at != data_len:
         raise ValueError(f"safetensors header: the tensors cover {at} bytes of a {data_len}-byte data region")
-    return entries
+    return extra, entries
 
 
-def _check_into(into: Mapping, entries, ctx) -> None:
-    """Every mismatch between ``into`` and the header, in one ``ValueError``."""
+def _check_into(into: Mapping, entries, ctx, sliced: bool = False) -> None:
+    """Every mismatch between ``into`` and the header's tensors (``sliced``: the selected slices, for
+    ``read_safetensors_slices``), in one ``ValueError``."""
     problems = []
     want = {name: (dtype, shape) for name, dtype, shape, _, _ in entries}
+    there, what, holds = ("selected", "read_safetensors_slices", "the slice is") if sliced else \
+        ("in the file", "read_safetensors", "the file holds")
     for name in sorted(set(want) - set(into)):
-        problems.append(f"{name!r} is in the file but not in into")
+        problems.append(f"{name!r} is {there} but not in into")
     for name in sorted(set(into) - set(want)):
-        problems.append(f"{name!r} is in into but not in the file")
+        problems.append(f"{name!r} is in into but not {there}")
     spans = []
     for name in sorted(set(want) & set(into)):
         t, (dtype, shape) = into[name], want[name]
         if t.dtype != dtype or list(t.shape) != shape:
-            problems.append(f"{name!r}: the file holds {dtype} {shape}, into has {t.dtype} {list(t.shape)}")
+            problems.append(f"{name!r}: {holds} {dtype} {shape}, into has {t.dtype} {list(t.shape)}")
             continue
         try:
             DeviceFile._Source._check_tensor(t, ctx, f"into[{name!r}]")
@@ -648,7 +652,7 @@ def _check_into(into: Mapping, entries, ctx) -> None:
         if lo < hi:
             problems.append(f"into[{a!r}] and into[{b!r}] overlap")
     if problems:
-        raise ValueError("read_safetensors(into=...): " + "; ".join(problems))
+        raise ValueError(f"{what}(into=...): " + "; ".join(problems))
 
 
 async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping | None = None,
@@ -663,15 +667,7 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
     ``ValueError`` before any block GET.  The data region then arrives with one ``read_file_into_device`` into a
     ``DeviceFile`` over the tensors in data order (``staging_bytes`` as there)."""
     ctx = blob_utils.get_context()
-    size = (await _get_file2(client, volume_id, path, 0, 8)).size
-    if size < 8:
-        raise ValueError(f"{path} ({size} bytes) is too short to be a safetensors file")
-    n = int.from_bytes(await _read_range_host(client, volume_id, path, 0, 8), "little")
-    if n > _ST_MAX_HEADER:
-        raise ValueError(f"safetensors header of {n} bytes is larger than {_ST_MAX_HEADER}")
-    if 8 + n > size:
-        raise ValueError(f"safetensors header of {n} bytes does not fit a {size}-byte file")
-    entries = _safetensors_entries(await _read_range_host(client, volume_id, path, 8, n), size - 8 - n)
+    size, n, _, entries = await _read_safetensors_header(client, volume_id, path)
     if into is not None:
         _check_into(into, entries, ctx)
         tensors = [into[name] for name, *_ in entries]
@@ -684,6 +680,209 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
 
 
 _ST_MAX_HEADER = 100_000_000  # the safetensors library's bound on the header length
+
+
+async def _read_safetensors_header(client, volume_id: str, path: str):
+    """(file size, header length, ``__metadata__`` or None, ``_safetensors_entries``) of the safetensors file at
+    ``path``: three ``VolumeGetFile2`` calls (the size, then the 8-byte length and the header through host memory)."""
+    size = (await _get_file2(client, volume_id, path, 0, 8)).size
+    if size < 8:
+        raise ValueError(f"{path} ({size} bytes) is too short to be a safetensors file")
+    n = int.from_bytes(await _read_range_host(client, volume_id, path, 0, 8), "little")
+    if n > _ST_MAX_HEADER:
+        raise ValueError(f"safetensors header of {n} bytes is larger than {_ST_MAX_HEADER}")
+    if 8 + n > size:
+        raise ValueError(f"safetensors header of {n} bytes does not fit a {size}-byte file")
+    metadata, entries = _safetensors_entries(await _read_range_host(client, volume_id, path, 8, n), size - 8 - n)
+    return size, n, metadata, entries
+
+
+async def read_safetensors_header(client, volume_id: str, path: str):
+    """(``__metadata__`` or None, {name: (torch dtype, shape tuple)} in data order) of the safetensors file at
+    ``path``, read and checked as ``read_safetensors`` reads its header (three ``VolumeGetFile2`` calls, no data): what
+    a caller needs to work out its slices for ``read_safetensors_slices``."""
+    _, _, metadata, entries = await _read_safetensors_header(client, volume_id, path)
+    return metadata, {name: (dtype, tuple(shape)) for name, dtype, shape, _, _ in entries}
+
+
+def _slice_bounds(name: str, shape, index):
+    """([(lo, hi) per dimension], kept: [bool per dimension]) of ``full[index]`` for a tensor of ``shape``: ``index``
+    an int, a slice of step 1, ``...`` or a tuple of these.  ``TypeError`` / ``ValueError`` / ``IndexError`` as the
+    class of the problem, as torch raises them."""
+    items = index if isinstance(index, tuple) else (index,)
+    for x in items:
+        if x is Ellipsis:
+            continue
+        if isinstance(x, bool) or not isinstance(x, (int, slice)):
+            raise TypeError(f"{name!r}: index {x!r} is not an int, a slice or ...; only those are supported")
+        if isinstance(x, slice):
+            if x.step not in (None, 1):
+                raise ValueError(f"{name!r}: slice {x!r} has a step other than 1")
+            for v in (x.start, x.stop):
+                if v is not None and (isinstance(v, bool) or not isinstance(v, int)):
+                    raise TypeError(f"{name!r}: slice {x!r} has a bound that is not an int or None")
+    ellipses = sum(x is Ellipsis for x in items)
+    if ellipses > 1:
+        raise IndexError(f"{name!r}: an index can only have a single ellipsis ('...')")
+    rank = len(shape)
+    if len(items) - ellipses > rank:
+        raise IndexError(f"{name!r}: too many indices for tensor of dimension {rank}")
+    if ellipses:
+        at = next(i for i, x in enumerate(items) if x is Ellipsis)
+        items = items[:at] + (slice(None),) * (rank - len(items) + 1) + items[at + 1 :]
+    items = items + (slice(None),) * (rank - len(items))
+    bounds, kept = [], []
+    for dim, (x, d) in enumerate(zip(items, shape)):
+        if isinstance(x, slice):
+            lo, hi, _ = x.indices(d)
+            bounds.append((lo, max(lo, hi)))
+            kept.append(True)
+        else:
+            if not -d <= x < d:
+                raise IndexError(f"{name!r}: index {x} is out of bounds for dimension {dim} with size {d}")
+            bounds.append((x % d, x % d + 1))
+            kept.append(False)
+    return bounds, kept
+
+
+def _slice_runs(shape, bounds, itemsize: int, start: int):
+    """The selection ``bounds`` of a C-contiguous tensor at file offset ``start``, as patterns ``(F, W, P, R)``: R rows
+    of W bytes, row r at file offset F + r * P (P >= W), in the order their bytes are packed into the result.  The
+    trailing whole dimensions merge into the row width; the dimensions out to the next partial one, which must be whole
+    but for the outermost, make the rows at one pitch; the dimensions outside that are enumerated."""
+    import itertools
+
+    if any(hi == lo for lo, hi in bounds):
+        return []
+    rank = len(shape)
+    whole = [lo == 0 and hi == d for (lo, hi), d in zip(bounds, shape)]
+    stride = [itemsize] * (rank + 1)  # stride[j]: bytes per index step of dimension j (stride[rank] = one element)
+    for j in range(rank - 1, -1, -1):
+        stride[j] = stride[j + 1] * shape[j]
+    k = max((j for j in range(rank) if not whole[j]), default=-1)
+    if k < 0:  # the whole tensor (a 0-d tensor included)
+        return [(start, stride[0] if rank else itemsize, stride[0] if rank else itemsize, 1)]
+    width = (bounds[k][1] - bounds[k][0]) * stride[k + 1]
+    m = max((j for j in range(k) if not whole[j]), default=-1)  # the rows run over dimensions max(m, 0) .. k - 1
+    rows = 1
+    for j in range(max(m, 0), k):
+        rows *= bounds[j][1] - bounds[j][0]
+    pitch = stride[k] if k else width
+    base = start + bounds[k][0] * stride[k + 1] + (bounds[m][0] * stride[m + 1] if m >= 0 else 0)
+    return [(base + sum(i * stride[j + 1] for j, i in enumerate(combo)), width, pitch, rows)
+            for combo in itertools.product(*[range(lo, hi) for lo, hi in bounds[: max(m, 0)]])]
+
+
+def _touched_blocks(runs, BS: int) -> set:
+    """The blocks (file offset // BS) that hold a byte of a row of ``runs``."""
+    out = set()
+    for F, W, P, R in runs:
+        if R == 1 or P - W < BS:  # no block fits between two rows: every block of the span is touched
+            out.update(range(F // BS, (F + (R - 1) * P + W - 1) // BS + 1))
+        else:
+            for r in range(R):
+                out.update(range((F + r * P) // BS, (F + r * P + W - 1) // BS + 1))
+    return out
+
+
+def _clip_run(run, dest: int, s0: int, s1: int, at: int):
+    """The boxes ``(dest offset, width, rows, staging offset, pitch)`` of the bytes of ``run`` (packed from ``dest``)
+    that lie in file bytes [s0, s1), staged contiguously from buffer offset ``at``: a partial first row, the whole
+    rows at the run's pitch, a partial last row."""
+    F, W, P, R = run
+    if F >= s1 or F + (R - 1) * P + W <= s0:
+        return []
+    ra = 0 if s0 <= F else max(0, (s0 - F - W) // P + 1)  # the first row that ends after s0
+    rb = min(R - 1, (s1 - F - 1) // P)  # the last row that starts before s1
+    if ra > rb:
+        return []
+
+    def part(r):
+        c0, c1 = max(0, s0 - F - r * P), min(W, s1 - F - r * P)
+        return (dest + r * W + c0, c1 - c0, 1, at + F + r * P + c0 - s0, c1 - c0)
+
+    if ra == rb:
+        return [part(ra)]
+    out, tail = [], []
+    if F + ra * P < s0:
+        out.append(part(ra))
+        ra += 1
+    if F + rb * P + W > s1:
+        tail.append(part(rb))
+        rb -= 1
+    if ra <= rb:
+        out.append((dest + ra * W, W, rb - ra + 1, at + F + ra * P - s0, P))
+    return out + tail
+
+
+async def read_safetensors_slices(client, volume_id: str, path: str, select: Mapping, *, into: Mapping | None = None,
+                                  staging_bytes: int = 256 << 20) -> dict:
+    """Slices of tensors of the safetensors file at ``path``: ``{name: full[index]}`` for every ``name: index`` of
+    ``select``, in its order, each a new contiguous tensor on the context's device (``full`` as ``read_safetensors``
+    returns it; for these index forms also what ``safe_open(...).get_slice(name)[index]`` gives).  An index is an int
+    (negative allowed), a slice of step 1 (bounds clamped as Python clamps them), at most one ``...``, or a tuple of
+    these no longer than the tensor's rank; ``...`` or ``()`` is the whole tensor.  Anything else raises before any data
+    GET: ``TypeError`` for ``None``, lists, tensors and bools, ``ValueError`` for other steps, ``IndexError`` for an
+    out-of-range int or too many indices, and one ``ValueError`` naming every unknown name.
+
+    The header is read as ``read_safetensors`` reads it.  Then ONE ``VolumeGetFile2`` call covers the first touched
+    block to the last touched byte, and exactly the touched blocks (those holding a selected byte) are fetched, once
+    each, into the page-locked waves of ``read_file_into_device`` (``staging_bytes`` as there).  Each complete wave
+    goes to the device with one ``load_boxes`` call: every selection is cut into boxes (rows at one pitch, the trailing
+    whole dimensions merged into the row), split where the staging stops being contiguous, at a wave's edge or a
+    skipped block.  Of HBM, the call allocates only the results and the copy's small stream-ordered tables.  With ``into=`` the caller's tensors are filled
+    in place: the sliced shapes and the dtypes must match, and the tensors must be contiguous, on the context's device
+    and not overlap, every mismatch in one ``ValueError`` before any data GET.  On return and on error, ordering and
+    partial content are as for ``read_safetensors``."""
+    BS = blob_utils.BLOCK_SIZE
+    if staging_bytes < 2 * BS:
+        raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
+    ctx = blob_utils.get_context()
+    _, n, _, entries = await _read_safetensors_header(client, volume_id, path)
+    by_name = {e[0]: e for e in entries}
+    unknown = [name for name in select if name not in by_name]
+    if unknown:
+        raise ValueError(f"{path}: no tensors named {', '.join(repr(u) for u in unknown)}")
+    plans = []  # (name, dtype, result shape, runs)
+    for name, index in select.items():
+        _, dtype, shape, lo, _ = by_name[name]
+        bounds, kept = _slice_bounds(name, shape, index)
+        result = [hi - b for (b, hi), k in zip(bounds, kept) if k]
+        plans.append((name, dtype, result, _slice_runs(shape, bounds, dtype.itemsize, 8 + n + lo)))
+    if into is not None:
+        _check_into(into, [(name, dtype, result, 0, 0) for name, dtype, result, _ in plans], ctx, sliced=True)
+        tensors = [into[name] for name, *_ in plans]
+    else:
+        tensors = [DeviceFile._Source._new_tensor(result, dtype, ctx) for _, dtype, result, _ in plans]
+    runs, base = [], 0  # (run, its packed offset in the one file over every result tensor)
+    for (_, _, _, rs), t in zip(plans, tensors):
+        dest = base
+        for run in rs:
+            runs.append((run, dest))
+            dest += run[1] * run[3]
+        base += t.numel() * t.element_size()
+    touched = _touched_blocks([r for r, _ in runs], BS)
+    if touched:
+        first = min(touched) * BS
+        end = max(F + (R - 1) * P + W for (F, W, P, R), _ in runs)
+        slices = [s for s in await _block_slices(client, volume_id, path, first, end - first)
+                  if (first + s[1]) // BS in touched]
+        dst = DeviceFile._over(DeviceFile._Source(tensors, BOUNCE_BYTES))
+
+        def load(wave, at, buf, ctx):
+            boxes, k = [], 0
+            while k < len(wave):  # a stretch: blocks adjacent in the file and in the buffer
+                e = k + 1
+                while e < len(wave) and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and at[e] == at[e - 1] + wave[e - 1][2]:
+                    e += 1
+                s0, s1 = first + wave[k][1], first + wave[e - 1][1] + wave[e - 1][2]
+                for run, d in runs:
+                    boxes += [(0, *b) for b in _clip_run(run, d, s0, s1, at[k])]
+                k = e
+            return load_boxes([dst], boxes, buf, ctx=ctx)
+
+        await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
+    return {name: t for (name, *_), t in zip(plans, tensors)}
 
 
 _ZIP_TAIL = 1 << 16  # the end of a torch.save file read first: its end records and, usually, its central directory
@@ -916,7 +1115,11 @@ async def read_torch_save(client, volume_id: str, path: str, *, weights_only: bo
     slices = await _block_slices(client, volume_id, path, span_at, span_end - span_at)
     dst = DeviceFile._over(DeviceFile._Source([t for _, t in loads], BOUNCE_BYTES))
     plan = _StorageWaves(path, [r for r, _ in loads], span_at)
-    await _load_in_waves(slices, dst, plan, staging_bytes, None, lambda **_: None)
+    def load(wave, at, buf, ctx):
+        ranges, src_offsets = plan(wave, at, buf)
+        return load_ranges([dst], ranges, buf, src_offsets, ctx=ctx)
+
+    await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
     checked = [(r, t) for r, t in loads if r.crc]
     if checked:
         crc = DeviceFile._Source._empty(4 * len(checked), ctx).view(torch.int32)

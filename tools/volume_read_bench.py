@@ -17,7 +17,22 @@
     alternating, timed and compared bitwise as in (b).  Then the CRC launch alone (one crc32_device call over the loaded
     storages, CUDA events, best of VRB_REPS) against the load_ranges time of arm (a), when it ran.
 
-VRB_ARMS (default "abc") picks the arms.
+(d) slices for tensor parallelism, rank VRB_RANK (3) of 8 of a Llama-shaped bf16 layer stack (hidden 2048, kv 512,
+    intermediate 5632): q, k, v, gate and up sliced on dim 0, o and down on dim 1, the norms whole.
+    kernel: one 128 MiB wave laid out as _load_in_waves lays it out (16 blocks of the file in consecutive 8 MiB slots,
+    the data region starting at 8 mod 16 as safetensors headers leave it), its boxes planned as read_safetensors_slices
+    plans them, written into one packed device buffer by (1) ONE load_boxes call, (2) one cudaMemcpy2DAsync per box
+    from the same page-locked buffer (ctypes on libcudart), (3) load_ranges of the whole wave into scratch HBM and
+    .contiguous() slices of every tensor, against (4) one cudaMemcpyAsync of the selected byte count.  CUDA events,
+    VRB_REPS runs each, alternating, best and median, and the host's time inside each call; the three results are
+    compared bitwise.  The same for a selection that enumerates its outer dimension (rows 4..11, columns 2048..3071 of
+    every expert of a [511, 16, 8192] stack: 511 boxes in the wave).  Then arm (a)'s workload
+    as 1-row boxes (load_boxes) next to load_ranges.
+    end to end over loopback: a VRB_E2E_GIB (1 GiB) stack uploaded once; for every rank 0..7, read_safetensors_slices
+    against read_safetensors followed by .contiguous() slices, alternating: host clock, the bytes GET from the server,
+    the peak HBM growth (torch.cuda.max_memory_allocated) and resident-set growth, and a bitwise comparison.
+
+VRB_ARMS (default "abcd") picks the arms.
 
 The card name and power limit are read in the same run.  Needs a GPU: nothing here falls back.
 One JSON line per arm; also written to $VRB_OUT/volume_read_bench.json when set."""
@@ -32,6 +47,7 @@ import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import numpy as np
 import torch
 
 from modal_client_b200 import DeviceFile, _backend, _lib, blob_utils, load_ranges, volume
@@ -273,19 +289,234 @@ async def torch_save_arm(ctx, info, out):
     print(json.dumps(out[-1]), flush=True)
 
 
+LLAMA = {"q_proj": (2048, 2048), "k_proj": (512, 2048), "v_proj": (512, 2048), "o_proj": (2048, 2048),
+         "gate_proj": (5632, 2048), "up_proj": (5632, 2048), "down_proj": (2048, 5632), "input_layernorm": (2048,),
+         "post_attention_layernorm": (2048,)}
+
+
+def llama_shapes(total: int) -> dict:
+    per = sum(2 * (s[0] * (s[1] if len(s) > 1 else 1)) for s in LLAMA.values())
+    return {f"layers.{i}.{k}.weight": s for i in range(max(1, total // per)) for k, s in LLAMA.items()}
+
+
+def tp_index(name: str, shape, rank: int, ranks: int = 8):
+    if len(shape) == 1:
+        return ...
+    d = 1 if ("o_proj" in name or "down_proj" in name) else 0
+    n = shape[d] // ranks
+    return (slice(None),) * d + (slice(rank * n, (rank + 1) * n),)
+
+
+def slices_kernel_arm(ctx, info, out):
+    """The TP slices of a Llama stack (few boxes per wave), then a selection that enumerates its outer dimension: rows
+    4..11 and columns 2048..3071 of every expert of a [511, 16, 8192] stack, 511 boxes in one wave."""
+    rank = int(os.environ.get("VRB_RANK", "3"))
+    wave = 16 * blob_utils.BLOCK_SIZE
+    box_workload(ctx, info, out, "slices_kernel", llama_shapes(2 * wave), lambda n, s: tp_index(n, s, rank))
+    box_workload(ctx, info, out, "slices_kernel_many_boxes", {"experts.weight": (511, 16, 8192)},
+                 lambda n, s: (slice(None), slice(4, 12), slice(2048, 3072)))
+    one_row_boxes_arm(ctx, info, out)
+
+
+def box_workload(ctx, info, out, label: str, shapes: dict, index_of):
+    import ctypes
+
+    from modal_client_b200 import load_boxes
+
+    BS, rank = blob_utils.BLOCK_SIZE, int(os.environ.get("VRB_RANK", "3"))
+    wave = 16 * BS
+    data0 = 8 + 8 * 126  # the data region starts at 8 mod 16
+    # the file's tensors in data order; the wave holds file bytes [0, wave) in consecutive slots
+    runs, tensors, at, dest = [], [], data0, 0
+    for name, shape in shapes.items():
+        nbytes = 2 * int(np.prod(shape))
+        if at >= wave:
+            break
+        bounds, kept = volume._slice_bounds(name, shape, index_of(name, shape))
+        result = [hi - lo for (lo, hi), k in zip(bounds, kept) if k]
+        first = len(runs)
+        for run in volume._slice_runs(shape, bounds, 2, at):
+            runs.append((run, dest))
+            dest += run[1] * run[3]
+        tensors.append((name, shape, at, nbytes, bounds, first, len(runs)))
+        at += nbytes
+    boxes = [(0, *b) for run, d in runs for b in volume._clip_run(run, d, 0, wave, 0)]
+    selected = sum(b[2] * b[3] for b in boxes)
+    # the sliced results of tensors wholly inside the wave (the comparison of route (3) needs whole tensors)
+    whole = [t for t in tensors if t[2] + t[3] <= wave]
+    src = ctx.host_alloc(wave)
+    try:
+        src[:] = torch.randint(0, 256, (wave,), dtype=torch.uint8).numpy()
+        dst = {k: torch.zeros(dest, dtype=torch.uint8, device="cuda") for k in ("load_boxes", "memcpy2d", "slice")}
+        scratch = torch.empty(wave, dtype=torch.uint8, device="cuda")
+        ceiling_dst = torch.empty(selected, dtype=torch.uint8, device="cuda")
+        ceiling_src = torch.from_numpy(src[:selected].copy()).pin_memory()
+        cudart = ctypes.CDLL("libcudart.so.12")
+        cudart.cudaMemcpy2DAsync.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
+                                             ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p]
+        f = DeviceFile(dst["load_boxes"])
+        base, out_ptr = src.ctypes.data, dst["memcpy2d"].data_ptr()
+        stream = torch.cuda.current_stream().cuda_stream
+
+        def memcpy2d():
+            for _, off, w, r, at, pitch in boxes:
+                rc = cudart.cudaMemcpy2DAsync(out_ptr + off, w, base + at, pitch, w, r, 1, stream)
+                assert rc == 0, rc
+
+        def slice_route():
+            load_ranges([DeviceFile(scratch)], [(0, 0, wave)], src, [0], ctx=ctx)
+            for name, shape, at, nbytes, bounds, first, last in whole:
+                if first == last:
+                    continue
+                t = scratch[at : at + nbytes].view(torch.bfloat16).view(shape)
+                part = t[tuple(slice(lo, hi) for lo, hi in bounds)]
+                d0 = runs[first][1]
+                dst["slice"][d0 : d0 + part.numel() * 2].view(torch.bfloat16).view(part.shape).copy_(part)
+
+        cands = {"load_boxes": lambda: load_boxes([f], boxes, src, ctx=ctx), "memcpy2d_per_box": memcpy2d,
+                 "load_ranges_then_slice": slice_route,
+                 "memcpy_ceiling": lambda: ceiling_dst.copy_(ceiling_src, non_blocking=True)}
+        for fn in cands.values():
+            fn()
+        times, enqueue = {k: [] for k in cands}, {k: [] for k in cands}
+
+        def host_timed(k, fn):
+            def run():
+                t0 = time.perf_counter()
+                fn()
+                enqueue[k].append((time.perf_counter() - t0) * 1e3)
+            return run
+
+        for _ in range(int(os.environ.get("VRB_REPS", "5"))):
+            for k, fn in cands.items():
+                times[k].append(events_ms(host_timed(k, fn)))
+        torch.cuda.synchronize()
+        whole_end = runs[whole[-1][6] - 1][1] + runs[whole[-1][6] - 1][0][1] * runs[whole[-1][6] - 1][0][3]
+        equal = {"memcpy2d_equal": torch.equal(dst["load_boxes"], dst["memcpy2d"]),
+                 "slice_equal_on_whole_tensors": torch.equal(dst["load_boxes"][:whole_end], dst["slice"][:whole_end])}
+        best = {k: min(v) for k, v in times.items()}
+        for k, v in times.items():
+            out.append({"arm": f"{label}.{k}", "selected_bytes": selected, "wave_bytes": wave, "boxes": len(boxes),
+                        "tensors": len(tensors), "rank": rank, "best_ms": round(best[k], 3),
+                        "median_ms": round(statistics.median(v), 3), "GB_s": round(selected / best[k] / 1e6, 2),
+                        "host_call_median_ms": round(statistics.median(enqueue[k]), 3),
+                        "share_of_ceiling": round(best["memcpy_ceiling"] / best[k], 3), **equal, **info})
+            print(json.dumps(out[-1]), flush=True)
+    finally:
+        torch.cuda.synchronize()
+        ctx.host_free(src)
+
+
+def one_row_boxes_arm(ctx, info, out):
+    """Arm (a)'s workload (every block of a safetensors image at its slot) as 1-row boxes, next to load_ranges."""
+    from modal_client_b200 import load_boxes
+
+    BS = blob_utils.BLOCK_SIZE
+    sd = state_dict(int(float(os.environ.get("VRB_GIB", "2")) * GiB))
+    f = DeviceFile.safetensors(sd)
+    n = f.nbytes
+    ranges = [(0, o, min(BS, n - o)) for o in range(0, n, BS)]
+    boxes = [(0, o, m, 1, o, m) for _, o, m in ranges]
+    src = ctx.host_alloc(n)
+    try:
+        src[:] = torch.randint(0, 256, (n,), dtype=torch.uint8).numpy()
+        cands = {"load_ranges": lambda: load_ranges([f], ranges, src, [o for _, o, _ in ranges], ctx=ctx),
+                 "load_boxes_1_row": lambda: load_boxes([f], boxes, src, ctx=ctx)}
+        for fn in cands.values():
+            fn()
+        times = {k: [] for k in cands}
+        for _ in range(int(os.environ.get("VRB_REPS", "5"))):
+            for k, fn in cands.items():
+                times[k].append(events_ms(fn))
+        torch.cuda.synchronize()
+        ok = b"".join(s.cpu().numpy().tobytes() for s in f._src.segments) == src.tobytes()
+        for k, v in times.items():
+            out.append({"arm": f"arm_a_workload.{k}", "bytes": n, "ranges": len(ranges), "best_ms": round(min(v), 3),
+                        "median_ms": round(statistics.median(v), 3), "GB_s": round(n / min(v) / 1e6, 2),
+                        "bytes_equal": ok, **info})
+            print(json.dumps(out[-1]), flush=True)
+    finally:
+        torch.cuda.synchronize()
+        ctx.host_free(src)
+    del sd, f
+
+
+async def slices_e2e_arm(info, out):
+    BS = blob_utils.BLOCK_SIZE
+    total = int(float(os.environ.get("VRB_E2E_GIB", "1")) * GiB)
+    g = torch.Generator(device="cuda").manual_seed(7)
+    sd = {k: torch.randn(s, device="cuda", generator=g).to(torch.bfloat16) for k, s in llama_shapes(total).items()}
+    size = sum(t.numel() * 2 for t in sd.values())
+    got_bytes = [0]
+    real_fetch = volume._fetch_block
+
+    async def counting_fetch(url, buf, want, semaphore):
+        got_bytes[0] += want
+        await real_fetch(url, buf, want, semaphore)
+
+    volume._fetch_block = counting_fetch
+    rows = {"slices": [], "full_then_slice": []}
+    try:
+        async with running_volume_server(BS) as (stub, _):
+            client = types.SimpleNamespace(stub=stub)
+            async with volume.VolumeUploadContextManager2("vo-b", client) as batch:
+                batch.put_file(DeviceFile.safetensors(sd), "/tp.safetensors")
+            del sd
+            _, info_hdr = await volume.read_safetensors_header(client, "vo-b", "/tp.safetensors")
+            for rank in range(8):
+                select = {k: tp_index(k, s, rank) for k, (_, s) in info_hdr.items()}
+                results = {}
+                order = ("slices", "full_then_slice") if rank % 2 == 0 else ("full_then_slice", "slices")
+                for route in order:
+                    torch.cuda.synchronize()
+                    got_bytes[0] = 0
+                    hbm = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    with PeakRss() as rss:
+                        t0 = time.perf_counter()
+                        if route == "slices":
+                            res = await volume.read_safetensors_slices(client, "vo-b", "/tp.safetensors", select)
+                        else:
+                            full = await volume.read_safetensors(client, "vo-b", "/tp.safetensors")
+                            res = {k: full[k][i].contiguous() for k, i in select.items()}
+                            del full
+                        torch.cuda.synchronize()
+                        dt = time.perf_counter() - t0
+                    results[route] = res
+                    rows[route].append((dt, got_bytes[0], torch.cuda.max_memory_allocated() - hbm, rss.growth))
+                equal = all(torch.equal(results["slices"][k].view(torch.int16),
+                                        results["full_then_slice"][k].view(torch.int16)) for k in select)
+                rows["slices"][-1] += (equal,)
+                rows["full_then_slice"][-1] += (equal,)
+                del results
+    finally:
+        volume._fetch_block = real_fetch
+    for route, v in rows.items():
+        ts = [x[0] for x in v]
+        out.append({"arm": f"slices_loopback.{route}", "file_bytes": size, "ranks": 8, "median_s": round(statistics.median(ts), 3),
+                    "range_s": [round(min(ts), 3), round(max(ts), 3)],
+                    "bytes_get_per_rank": [x[1] for x in v], "peak_hbm_growth_GB": round(max(x[2] for x in v) / 1e9, 3),
+                    "peak_rss_growth_GB": round(max(x[3] for x in v) / 1e9, 3),
+                    "bitwise_equal": all(x[4] for x in v), **info})
+        print(json.dumps(out[-1]), flush=True)
+
+
 def main():
     if not torch.cuda.is_available():
         raise SystemExit("volume_read_bench needs a GPU")
     info = gpu_info()
     ctx = _lib.Context(0, pinned_bytes=64 << 20, device_bytes=512 << 20)
     _backend.set_context(ctx)
-    out, arms = [], os.environ.get("VRB_ARMS", "abc")
+    out, arms = [], os.environ.get("VRB_ARMS", "abcd")
     if "a" in arms:
         kernel_arm(ctx, info, out)
     if "b" in arms:
         asyncio.run(e2e_arm(info, out))
     if "c" in arms:
         asyncio.run(torch_save_arm(ctx, info, out))
+    if "d" in arms:
+        slices_kernel_arm(ctx, info, out)
+        asyncio.run(slices_e2e_arm(info, out))
     if os.environ.get("VRB_OUT"):
         os.makedirs(os.environ["VRB_OUT"], exist_ok=True)
         with open(os.path.join(os.environ["VRB_OUT"], "volume_read_bench.json"), "w") as fh:
