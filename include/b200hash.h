@@ -260,6 +260,41 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
                                uint64_t nfiles, const b200h_box* boxes, uint64_t nboxes, const void* h_src,
                                uint64_t h_src_bytes, void* cuda_stream);
 
+/* Element types of b200h_cast_box (IEEE binary32, IEEE binary16, bfloat16; all little-endian). */
+#define B200H_DT_F32 1u
+#define B200H_DT_F16 2u
+#define B200H_DT_BF16 3u
+
+/* A box whose elements change type on the way: `box` as in b200h_box, except that `width` and `src_pitch` count SOURCE
+ * bytes, and its rows * width / (source element size) elements are written packed, as `dst_type`, to bytes
+ * [offset, offset + rows * width / (source element size) * (destination element size)) of file `file`. */
+typedef struct b200h_cast_box {
+    b200h_box box;
+    uint64_t src_type, dst_type; /* B200H_DT_* */
+} b200h_cast_box;
+
+/* b200h_copy_boxes_from_host with a conversion: every element of box i of h_src, of type src_type, is converted to
+ * dst_type and written packed to the box's destination run.  Narrowing rounds to nearest even, exactly as the CUDA
+ * intrinsics __float2bfloat16 (F32 -> BF16) and __float2half (F32 -> F16) do, NaN bit patterns included; F16 <-> BF16
+ * widens to F32 exactly and rounds once; widening is exact.
+ * Every argument is checked before any work is enqueued, B200H_E_INVALID otherwise: every rule of
+ * b200h_copy_boxes_from_host (the destination measured in destination bytes), and further: src_type and dst_type are
+ * two different B200H_DT_* codes; width and src_pitch are multiples of the source element size; every row's source
+ * address is a multiple of the source element size; and each box's destination lies in ONE segment, at a device
+ * address that is a multiple of the destination element size.  (Every file written by safetensors.torch.save meets the
+ * alignment rules: the header is padded to a multiple of 8 and tensors are laid out by decreasing element size, so
+ * every tensor starts at a multiple of its element size.)
+ * ONE kernel launch (load_cast_boxes_kernel) per call, none when every box is empty, with tables that grow as those of
+ * b200h_copy_boxes_from_host.  Every source word that holds a selected byte crosses PCIe once, in an aligned 16-byte
+ * load inside its row's hull; device stores are full aligned 16-byte words except at the ends of a box's run and at
+ * one word per 64 KiB tile of source words.  Device bytes outside every box are not written.
+ * The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream), as the range entries do.
+ * Replaces: _read_file_into_fileobj (py/modal/volume.py:923-1000) followed by safetensors.torch.load and a per-tensor
+ * .to(dtype), which holds the stored image and its converted copy at once, to load a checkpoint in a compute dtype. */
+int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                    const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes,
+                                    uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

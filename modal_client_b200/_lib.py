@@ -23,6 +23,7 @@ MD5 = 2
 TRIM_ZEROS = 4
 HEX_OUT = 32  # digest outputs as lowercase ASCII hex rows (64 / 32 chars), formatted on the device
 NO_OUTLIERS = 16  # keep every message on the lane kernel: device batches then only enqueue (include/b200hash.h)
+DT_F32, DT_F16, DT_BF16 = 1, 2, 3  # element types of copy_cast_boxes_from_host (B200H_DT_*)
 
 #: every symbol include/b200hash.h declares (tests check the .so exports all of them)
 ABI_SYMBOLS = (
@@ -35,6 +36,7 @@ ABI_SYMBOLS = (
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
     "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host", "b200h_copy_boxes_from_host",
+    "b200h_copy_cast_boxes_from_host",
 )
 
 
@@ -116,6 +118,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_copy_ranges_from_host.restype = i32
         L.b200h_copy_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
         L.b200h_copy_boxes_from_host.restype = i32
+        L.b200h_copy_cast_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
+        L.b200h_copy_cast_boxes_from_host.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -469,6 +473,21 @@ class Context:
                                                 nfiles, _np_ptr(bx) if len(bx) else None, len(bx),
                                                 ctypes.c_void_p(src.ctypes.data), src.size, stream or None)
         self._check(rc, "b200h_copy_boxes_from_host")
+
+    def copy_cast_boxes_from_host(self, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
+                                  stream: int = 0) -> None:
+        """``copy_boxes_from_host`` with a conversion: box i = ``(file, offset, width, rows, src_offset, src_pitch,
+        src_type, dst_type)`` (``DT_F32`` / ``DT_F16`` / ``DT_BF16``, two different ones) converts its ``rows * width /
+        (source element size)`` elements, ``width`` and ``src_pitch`` counted in source bytes, and writes them packed
+        from byte ``offset`` of its file.  Rows start at a multiple of the source element size; a box's destination lies
+        in one buffer, at a multiple of the destination element size.  One kernel launch, only enqueued on ``stream``."""
+        segs = _segments(seg_ptrs, seg_lens)
+        ffs, nfiles = _segment_args(file_first_seg)
+        bx = np.ascontiguousarray(boxes, dtype=np.uint64).reshape(-1, 8)
+        rc = self._L.b200h_copy_cast_boxes_from_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs),
+                                                     _np_ptr(ffs), nfiles, _np_ptr(bx) if len(bx) else None, len(bx),
+                                                     ctypes.c_void_p(src.ctypes.data), src.size, stream or None)
+        self._check(rc, "b200h_copy_cast_boxes_from_host")
 
     def _copy_ranges(self, entry: str, offsets_name: str, seg_ptrs, seg_lens, file_first_seg, ranges, host: np.ndarray,
                      host_offsets, stream: int) -> None:

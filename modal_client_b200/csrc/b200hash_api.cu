@@ -1557,25 +1557,50 @@ int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint6
                        cuda_stream);
 }
 
-int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
-                               uint64_t nfiles, const b200h_box* boxes, uint64_t nboxes, const void* h_src,
-                               uint64_t h_src_bytes, void* cuda_stream) {
-    if (!ctx) return B200H_E_INVALID;
-    B200H_RANGE("b200h_copy_boxes_from_host");
-    std::lock_guard<std::mutex> lk(ctx->mu);
+// Bytes of one element of a B200H_DT_* type; 0 for an unknown code.
+static uint64_t dt_bytes(uint64_t t) {
+    return t == B200H_DT_F32 ? 4 : t == B200H_DT_F16 || t == B200H_DT_BF16 ? 2 : 0;
+}
+
+// b200h_copy_boxes_from_host (casts == NULL) and b200h_copy_cast_boxes_from_host (boxes == NULL; box i is
+// casts[i].box): box i of h_src to its packed destination run, its elements converted when it is a cast box.
+static int copy_boxes(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                      uint64_t nfiles, const b200h_box* boxes, const b200h_cast_box* casts, uint64_t nboxes,
+                      const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
     std::vector<uint64_t> seg_lens;
     FileTable t;
     if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
-    if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
+    if (nboxes && !boxes && !casts) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
     if (nboxes && !h_src) return fail(ctx, B200H_E_INVALID, "h_src must not be NULL");
+    auto box = [&](uint64_t i) -> const b200h_box& { return casts ? casts[i].box : boxes[i]; };
+    // source and destination element sizes: a plain box copies bytes
+    auto sizes = [&](uint64_t i, uint64_t& ss, uint64_t& ds) {
+        ss = casts ? dt_bytes(casts[i].src_type) : 1;
+        ds = casts ? dt_bytes(casts[i].dst_type) : 1;
+    };
     bool any = false;
     for (uint64_t i = 0; i < nboxes; ++i) {
-        const b200h_box& b = boxes[i];
+        const b200h_box& b = box(i);
         const std::string name = "box " + std::to_string(i);
+        uint64_t ss, ds;
+        sizes(i, ss, ds);
+        if (casts) {
+            if (!ss || !ds) return fail(ctx, B200H_E_INVALID, name + ": unknown element type");
+            if (casts[i].src_type == casts[i].dst_type)
+                return fail(ctx, B200H_E_INVALID, name + ": src_type and dst_type are the same");
+            if (b.width % ss || b.src_pitch % ss)
+                return fail(ctx, B200H_E_INVALID,
+                            name + ": width and src_pitch must be multiples of the source element size");
+            if (((uintptr_t)h_src + b.src_offset) % ss)
+                return fail(ctx, B200H_E_INVALID,
+                            name + ": its rows do not start at a multiple of the source element size");
+        }
         if (b.file >= nfiles) return fail(ctx, B200H_E_INVALID, name + " names a file that does not exist");
         if (b.width && b.rows > ~0ull / b.width) return fail(ctx, B200H_E_INVALID, name + ": rows * width overflows");
         const uint64_t n = b.rows * b.width;
-        if (b.offset > t.size[b.file] || n > t.size[b.file] - b.offset)
+        if (n / ss > ~0ull / ds) return fail(ctx, B200H_E_INVALID, name + ": its destination size overflows");
+        const uint64_t nd = n / ss * ds;  // destination bytes
+        if (b.offset > t.size[b.file] || nd > t.size[b.file] - b.offset)
             return fail(ctx, B200H_E_INVALID, name + " reaches past the end of its file");
         if (b.rows > 1 && b.src_pitch < b.width) return fail(ctx, B200H_E_INVALID, name + ": src_pitch is less than width");
         if (!n) continue;
@@ -1584,6 +1609,16 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
                           b.width <= h_src_bytes - (b.rows - 1) * b.src_pitch &&
                           b.src_offset <= h_src_bytes - (b.rows - 1) * b.src_pitch - b.width;
         if (!fits) return fail(ctx, B200H_E_INVALID, name + ": its source reaches past h_src_bytes");
+        if (casts) {  // one segment, so that every destination word holds whole elements
+            uint64_t npieces = 0, dev = 0;
+            file_pieces(t, b.file, b.offset, nd, [&](uint64_t s, uint64_t in, uint64_t) {
+                if (!npieces++) dev = (uint64_t)(uintptr_t)segs[s].d_ptr + in;
+            });
+            if (npieces != 1) return fail(ctx, B200H_E_INVALID, name + ": its destination crosses a segment edge");
+            if (dev % ds)
+                return fail(ctx, B200H_E_INVALID,
+                            name + ": its destination is not at a multiple of the destination element size");
+        }
         any = true;
     }
     CU_TRY(ctx, cudaSetDevice(ctx->device));
@@ -1602,13 +1637,17 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
     // pieces (box x segment, in destination order within a box; `host` = offset in the box's packed run) and the tiles
     // of every box's virtual source words (see BoxTile): neither grows with the rows
     std::vector<RangePiece> pieces;
-    std::vector<BoxTile> tiles;
+    std::vector<CastTile> tiles;
     std::vector<uint64_t> box_of;  // per piece: the box it belongs to (for the overlap message)
     for (uint64_t i = 0; i < nboxes; ++i) {
-        const b200h_box& bx = boxes[i];
+        const b200h_box& bx = box(i);
+        uint64_t ss, ds;
+        sizes(i, ss, ds);
         const uint64_t n = bx.rows * bx.width;
         if (!n) continue;
-        BoxTile b{};
+        CastTile ct{};
+        if (casts) ct.src_type = (uint32_t)casts[i].src_type, ct.dst_type = (uint32_t)casts[i].dst_type;
+        BoxTile& b = ct.box;
         const bool run = bx.rows == 1 || bx.src_pitch == bx.width;  // one contiguous source run
         b.src = bx.src_offset + phase;
         b.width = run ? n : bx.width;
@@ -1620,7 +1659,7 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
                                    : ((last + b.width - 1) >> 4) - (b.src >> 4) + 1;
         const size_t first = pieces.size();
         uint64_t at = 0;
-        file_pieces(t, bx.file, bx.offset, n, [&](uint64_t s, uint64_t in, uint64_t len) {
+        file_pieces(t, bx.file, bx.offset, n / ss * ds, [&](uint64_t s, uint64_t in, uint64_t len) {
             pieces.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in, at, len});
             box_of.push_back(i);
             at += len;
@@ -1631,12 +1670,13 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
             b.nv = (uint32_t)std::min(kStageTileBytes / 16, nv - v0);
             b.dlo = box_dest_at(b, v0);
             b.dhi = v0 + b.nv == nv ? n : box_dest_at(b, v0 + b.nv);
-            while (pieces[p].host + pieces[p].len <= b.dlo) ++p;
+            // the pieces that hold the tile's destination bytes (dlo and dhi count source bytes)
+            while (pieces[p].host + pieces[p].len <= b.dlo / ss * ds) ++p;
             size_t q = p;
-            while (q + 1 < pieces.size() && pieces[q + 1].host < b.dhi) ++q;
+            while (q + 1 < pieces.size() && pieces[q + 1].host < b.dhi / ss * ds) ++q;
             b.first_piece = p;
             b.npieces = (uint32_t)(q - p + 1);
-            tiles.push_back(b);
+            tiles.push_back(ct);
         }
     }
     // no device byte may be written twice: two files, or two segments of one file, may share a tensor
@@ -1648,9 +1688,35 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
             return fail(ctx, B200H_E_INVALID, "boxes " + std::to_string(box_of[by_dev[k - 1]]) + " and " +
                                                   std::to_string(box_of[by_dev[k]]) + " write the same device bytes");
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    return launch_with_tables(ctx, st, tiles, pieces, [&](const BoxTile* d_tiles, const RangePiece* d_pieces) {
-        return launch_load_boxes(d_tiles, tiles.size(), d_pieces, (const uint8_t*)d_host - phase, st);
+    const void* d_src = (const uint8_t*)d_host - phase;
+    if (casts)
+        return launch_with_tables(ctx, st, tiles, pieces, [&](const CastTile* d_tiles, const RangePiece* d_pieces) {
+            return launch_load_cast_boxes(d_tiles, tiles.size(), d_pieces, d_src, st);
+        });
+    std::vector<BoxTile> plain(tiles.size());
+    for (size_t k = 0; k < tiles.size(); ++k) plain[k] = tiles[k].box;
+    return launch_with_tables(ctx, st, plain, pieces, [&](const BoxTile* d_tiles, const RangePiece* d_pieces) {
+        return launch_load_boxes(d_tiles, plain.size(), d_pieces, d_src, st);
     });
+}
+
+int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                               uint64_t nfiles, const b200h_box* boxes, uint64_t nboxes, const void* h_src,
+                               uint64_t h_src_bytes, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_boxes_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    return copy_boxes(ctx, segs, nsegs, file_first_seg, nfiles, boxes, nullptr, nboxes, h_src, h_src_bytes, cuda_stream);
+}
+
+int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                    const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes,
+                                    uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_cast_boxes_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
+    return copy_boxes(ctx, segs, nsegs, file_first_seg, nfiles, nullptr, boxes, nboxes, h_src, h_src_bytes, cuda_stream);
 }
 
 // ---------------------------------------------------------------------------------------------- files

@@ -21,9 +21,12 @@
 // Loads never leave the 16-byte aligned hull of a piece: the aligned words that hold a piece's first and last byte.
 // Those words lie in the same allocation granule as the bytes themselves (device allocations are at least 256-byte
 // aligned and sized in multiples of that), which the lane kernel's misaligned-start reads rely on as well.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/b200hash.h"
 #include "b200hash_kernels.cuh"
 
 namespace b200h {
@@ -323,6 +326,32 @@ __device__ __forceinline__ void box_words_out(const BoxTile& b, const RangePiece
     }
 }
 
+// One warp's pass over tile b: the loads run two chunks ahead in registers, a chunk goes to the warp's ring when its
+// turn comes, and out(from, upto) stores the packed destination bytes [from, upto) (in source bytes) whose source has
+// arrived.  The ring's other half still holds the chunk before, which a destination word may need.
+template <class Out>
+__device__ __forceinline__ void box_tile_steps(const BoxTile& b, const uint4* words, uint4* ring, uint32_t lane,
+                                               Out&& out) {
+    uint64_t from = b.dlo;
+    uint4 v[kLoadChunks], u[kLoadChunks];  // chunks c and c + 1, loaded
+    box_load_chunk(b, words, 0, lane, v);
+    box_load_chunk(b, words, kBoxChunk, lane, u);
+    for (uint32_t c = 0; c < b.nv; c += kBoxChunk) {
+        // the ring's other half holds chunk c - 1, which this step's words may still need
+#pragma unroll
+        for (int i = 0; i < kLoadChunks; ++i) {
+            ring[(c + i * 32 + lane) % kBoxRing] = v[i];
+            v[i] = u[i];
+        }
+        __syncwarp();
+        box_load_chunk(b, words, c + 2 * kBoxChunk, lane, u);
+        const uint64_t upto = c + kBoxChunk >= b.nv ? b.dhi : box_dest_at(b, b.v0 + c + kBoxChunk);
+        out(from, upto);
+        __syncwarp();
+        from = upto;
+    }
+}
+
 __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
     load_boxes_kernel(const BoxTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
                       const uint8_t* __restrict__ src) {
@@ -334,24 +363,135 @@ __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
     for (uint64_t t = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; t < ntiles; t += nwarps) {
         const BoxTile b = tiles[t];
         const RangePiece* __restrict__ pc = pieces + b.first_piece;
-        uint64_t from = b.dlo;
-        uint4 v[kLoadChunks], u[kLoadChunks];  // chunks c and c + 1, loaded
-        box_load_chunk(b, words, 0, lane, v);
-        box_load_chunk(b, words, kBoxChunk, lane, u);
-        for (uint32_t c = 0; c < b.nv; c += kBoxChunk) {
-            // the ring's other half holds chunk c - 1, which this step's words may still need
-#pragma unroll
-            for (int i = 0; i < kLoadChunks; ++i) {
-                ring[(c + i * 32 + lane) % kBoxRing] = v[i];
-                v[i] = u[i];
-            }
-            __syncwarp();
-            box_load_chunk(b, words, c + 2 * kBoxChunk, lane, u);
-            const uint64_t upto = c + kBoxChunk >= b.nv ? b.dhi : box_dest_at(b, b.v0 + c + kBoxChunk);
+        box_tile_steps(b, words, ring, lane, [&](uint64_t from, uint64_t upto) {
             for (uint32_t q = 0; q < b.npieces; ++q) box_words_out(b, pc[q], ring, from, upto, lane);
-            __syncwarp();
-            from = upto;
+        });
+    }
+}
+
+// ---- boxes whose elements change type on the way (F32, F16, BF16; b200h_copy_cast_boxes_from_host)
+//
+//   load_cast_boxes_kernel   load_boxes_kernel's tiles, loads and ring, with a destination word built from elements
+//                        instead of bytes.  Every element of a box lies whole in one aligned source word (rows start at
+//                        a multiple of the element size), and the box's destination is one piece at a multiple of the
+//                        destination element size, so every destination word holds whole elements.  A word of 16 / ds
+//                        elements takes 16 / ds * ss source bytes: 32 when narrowing F32 (two or three ring words), 16
+//                        between F16 and BF16 (one or two), 8 when widening (one or two).  When they are one run of one
+//                        row they come from the ring with shift_bytes; otherwise (a word across rows, a box's ends) element
+//                        by element.  The conversion then takes pairs of elements with the paired sm_90 intrinsics.
+
+constexpr uint32_t kDtF32 = B200H_DT_F32, kDtF16 = B200H_DT_F16;
+
+__device__ __forceinline__ uint32_t dt_bytes(uint32_t t) { return t == kDtF32 ? 4u : 2u; }
+
+// two 16-bit elements (F16 or BF16), widened exactly
+__device__ __forceinline__ float2 widen_pair(uint32_t x, uint32_t t) {
+    if (t == kDtF16) {
+        __half2 h;
+        memcpy(&h, &x, 4);
+        return __half22float2(h);
+    }
+    __nv_bfloat162 h;
+    memcpy(&h, &x, 4);
+    return __bfloat1622float2(h);
+}
+
+// two floats rounded to nearest even, as F16 or BF16
+__device__ __forceinline__ uint32_t narrow_pair(float a, float b, uint32_t t) {
+    uint32_t x;
+    if (t == kDtF16) {
+        const __half2 h = __float22half2_rn(make_float2(a, b));
+        memcpy(&x, &h, 4);
+    } else {
+        const __nv_bfloat162 h = __float22bfloat162_rn(make_float2(a, b));
+        memcpy(&x, &h, 4);
+    }
+    return x;
+}
+
+// The destination word of the source bytes lo || hi (32 of them from F32, 16 between F16 and BF16, 8 widening).
+__device__ __forceinline__ uint4 cast_word(uint4 lo, uint4 hi, uint32_t st, uint32_t dt) {
+    if (st == kDtF32)
+        return make_uint4(narrow_pair(__uint_as_float(lo.x), __uint_as_float(lo.y), dt),
+                          narrow_pair(__uint_as_float(lo.z), __uint_as_float(lo.w), dt),
+                          narrow_pair(__uint_as_float(hi.x), __uint_as_float(hi.y), dt),
+                          narrow_pair(__uint_as_float(hi.z), __uint_as_float(hi.w), dt));
+    if (dt == kDtF32) {
+        const float2 a = widen_pair(lo.x, st), b = widen_pair(lo.y, st);
+        return make_uint4(__float_as_uint(a.x), __float_as_uint(a.y), __float_as_uint(b.x), __float_as_uint(b.y));
+    }
+    const float2 a = widen_pair(lo.x, st), b = widen_pair(lo.y, st), c = widen_pair(lo.z, st), d = widen_pair(lo.w, st);
+    return make_uint4(narrow_pair(a.x, a.y, dt), narrow_pair(b.x, b.y, dt), narrow_pair(c.x, c.y, dt),
+                      narrow_pair(d.x, d.y, dt));
+}
+
+// Destination words of the box (one piece at device address `dev`) whose elements have packed source bytes in
+// [from, upto) (clipped to [b.dlo, b.dhi)) and whose last element's source lies before `upto`.
+__device__ __forceinline__ void cast_words_out(const BoxTile& b, uint32_t st, uint32_t dt, uint64_t dev,
+                                               const uint4* ring, uint64_t from, uint64_t upto, uint32_t lane) {
+    const uint32_t ss = dt_bytes(st), ds = dt_bytes(dt);
+    const uint64_t qhi = b.dhi / ss * ds, lo = from / ss * ds, hi = upto / ss * ds;
+    if (lo >= hi) return;
+    const uint64_t qa = dev + b.dlo / ss * ds, qe = dev + qhi, ha = dev + hi, welems = b.width / ss;
+    // a word whose elements go on past `hi` waits for the next step
+    const uint64_t w1 = hi < qhi ? ha >> 4 : ((ha - 1) >> 4) + 1;
+    for (uint64_t w = ((dev + lo) >> 4) + lane; w < w1; w += 32) {
+        const uint64_t ws = w * 16, aa = max(ws, qa), ea = min(ws + 16, qe);
+        const uint32_t jlo = (uint32_t)(aa - ws), jhi = (uint32_t)(ea - ws);
+        const uint64_t e = (aa - dev) / ds;  // the word's first element, counted in the box's packed run
+        uint64_t r = e / welems, c = e % welems;
+        uint4 s0, s1 = make_uint4(0, 0, 0, 0);
+        if (jhi - jlo == 16 && c + 16 / ds <= welems) {
+            const uint64_t s = b.src + r * b.pitch + c * ss;
+            const uint32_t slot = (uint32_t)(box_virtual(b, r, s) - b.v0), sh = (uint32_t)s & 15u;
+            const uint4 w0 = ring[slot % kBoxRing];
+            if (ss * 16 / ds == 32) {
+                const uint4 n1 = ring[(slot + 1) % kBoxRing];
+                s0 = sh ? shift_bytes(w0, n1, sh) : w0;
+                s1 = sh ? shift_bytes(n1, ring[(slot + 2) % kBoxRing], sh) : n1;
+            } else if (ss == ds) {
+                s0 = sh ? shift_bytes(w0, ring[(slot + 1) % kBoxRing], sh) : w0;
+            } else {
+                s0 = sh > 8 ? shift_bytes(w0, ring[(slot + 1) % kBoxRing], sh) : shift_bytes(w0, w0, sh);
+            }
+        } else {
+            uint64_t x[4] = {0, 0, 0, 0};  // the source bytes, element k at byte k * ss
+#pragma unroll 1
+            for (uint32_t j = jlo; j < jhi; j += ds) {
+                const uint64_t s = b.src + r * b.pitch + c * ss;
+                const uint8_t* word =
+                    reinterpret_cast<const uint8_t*>(ring + (uint32_t)(box_virtual(b, r, s) - b.v0) % kBoxRing);
+                const uint32_t p = j / ds * ss;
+                const uint64_t val = (ss == 4 ? (uint64_t)*reinterpret_cast<const uint32_t*>(word + (s & 15u))
+                                              : (uint64_t)*reinterpret_cast<const uint16_t*>(word + (s & 15u)))
+                                     << (8 * (p & 7));
+                if (p < 8) x[0] |= val;
+                else if (p < 16) x[1] |= val;
+                else if (p < 24) x[2] |= val;
+                else x[3] |= val;
+                if (++c == welems) c = 0, ++r;
+            }
+            s0 = make_uint4((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
+            s1 = make_uint4((uint32_t)x[2], (uint32_t)(x[2] >> 32), (uint32_t)x[3], (uint32_t)(x[3] >> 32));
         }
+        store_bytes(reinterpret_cast<uint8_t*>(ws), cast_word(s0, s1, st, dt), jlo, jhi);
+    }
+}
+
+__global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
+    load_cast_boxes_kernel(const CastTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
+                           const uint8_t* __restrict__ src) {
+    __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
+    const uint32_t lane = threadIdx.x & 31u;
+    uint4* ring = rings[threadIdx.x >> 5];
+    const uint4* words = reinterpret_cast<const uint4*>(src);
+    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
+    for (uint64_t t = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; t < ntiles; t += nwarps) {
+        const CastTile ct = tiles[t];
+        const uint64_t dev = pieces[ct.box.first_piece].dev;
+        box_tile_steps(ct.box, words, ring, lane, [&](uint64_t from, uint64_t upto) {
+            cast_words_out(ct.box, ct.src_type, ct.dst_type, dev, ring, from, upto, lane);
+        });
     }
 }
 
@@ -362,6 +502,15 @@ int launch_load_boxes(const BoxTile* tiles, uint64_t ntiles, const RangePiece* p
     const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
     load_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
                                                                                    static_cast<const uint8_t*>(src));
+    return 1;
+}
+
+int launch_load_cast_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
+                           cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
+    load_cast_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
+        tiles, ntiles, pieces, static_cast<const uint8_t*>(src));
     return 1;
 }
 

@@ -26,6 +26,8 @@ needed for those bytes.  The volumefs2 uploader uses it for the missing blocks w
 buffer into the files' tensors with ONE ``b200h_copy_ranges_from_host`` call (``volume.read_file_into_device``), and
 ``load_boxes(files, boxes, src)`` the strided form: rows of a page-locked buffer, any distance apart and at any phase,
 packed into the files with ONE ``b200h_copy_boxes_from_host`` call (``volume.read_safetensors_slices``).
+``load_cast_boxes(files, boxes, src)`` is ``load_boxes`` whose elements change type on the way (F32, F16, BF16), with
+ONE ``b200h_copy_cast_boxes_from_host`` call (``volume.read_safetensors(..., dtype=...)``).
 """
 from __future__ import annotations
 
@@ -355,6 +357,43 @@ def load_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> L
     ptrs, lens, first = _file_table(sources)
     with lead._on_stream():
         ctx.copy_boxes_from_host(ptrs, lens, first, boxes, src, lead.stream_handle)
+    return Loaded(lead._publish())
+
+
+def cast_dtypes() -> dict:
+    """The torch dtypes ``load_cast_boxes`` converts between, with their ``_lib.DT_*`` codes."""
+    import torch
+
+    return {torch.float32: _lib.DT_F32, torch.float16: _lib.DT_F16, torch.bfloat16: _lib.DT_BF16}
+
+
+def load_cast_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> Loaded:
+    """``load_boxes`` with a conversion: box i = ``(index into files, offset, width, rows, src_offset, src_pitch,
+    src_dtype, dst_dtype)``, two different torch dtypes of ``cast_dtypes()``, converts the ``rows * width / itemsize``
+    elements of type ``src_dtype`` (``width`` and ``src_pitch`` count source bytes) to ``dst_dtype`` -- rounding to
+    nearest even exactly as torch's CUDA ``.to()`` does -- and writes them packed from byte ``offset`` of its file.
+    Every row must start at a multiple of the source itemsize in ``src``'s memory, and a box's destination must lie in
+    one tensor of its file at a multiple of the destination itemsize.  ONE ``b200h_copy_cast_boxes_from_host`` call,
+    ordered exactly as ``load_boxes``."""
+    ctx = ctx or get_context()
+    sources = [f._src for f in files]
+    if any(len(b) != 8 for b in boxes):
+        raise ValueError("a box is (file, offset, width, rows, src_offset, src_pitch, src_dtype, dst_dtype)")
+    codes = cast_dtypes()
+    for b in boxes:
+        for dt in b[6:]:
+            if dt not in codes:
+                raise ValueError(f"load_cast_boxes converts between {', '.join(map(str, codes))}, not {dt}")
+    boxes = [tuple(int(x) for x in b[:6]) + (codes[b[6]], codes[b[7]]) for b in boxes]
+    if boxes and not sources:
+        raise ValueError("boxes without files")
+    if not sources:
+        return Loaded(None)
+    lead = sources[0]
+    lead._after_current()
+    ptrs, lens, first = _file_table(sources)
+    with lead._on_stream():
+        ctx.copy_cast_boxes_from_host(ptrs, lens, first, boxes, src, lead.stream_handle)
     return Loaded(lead._publish())
 
 
@@ -866,5 +905,6 @@ class DeviceFile(io.RawIOBase):
         return f"<DeviceFile {self._src.nbytes} bytes in {len(segs)} segments on {segs[0].device}>"
 
 
-__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "Staged", "hash_parts_many", "load_boxes", "load_ranges",
+__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "Staged", "hash_parts_many", "load_boxes", "load_cast_boxes",
+           "load_ranges",
            "safetensors_layout", "stage_ranges"]

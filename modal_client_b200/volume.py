@@ -39,7 +39,8 @@ from . import _wire, blob_utils, device_file
 from ._logging import logger
 from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
-from .device_file import BOUNCE_BYTES, DeviceFile, _st_dtypes, load_boxes, load_ranges, stage_ranges
+from .device_file import (BOUNCE_BYTES, DeviceFile, _st_dtypes, cast_dtypes, load_boxes, load_cast_boxes, load_ranges,
+                          stage_ranges)
 from .exception import ExecutionError, ServiceError
 from .http_utils import ClientSessionRegistry
 
@@ -623,11 +624,13 @@ def _safetensors_entries(header: bytes, data_len: int):
     return extra, entries
 
 
-def _check_into(into: Mapping, entries, ctx, sliced: bool = False) -> None:
+def _check_into(into: Mapping, entries, ctx, sliced: bool = False, stored: Mapping | None = None) -> None:
     """Every mismatch between ``into`` and the header's tensors (``sliced``: the selected slices, for
-    ``read_safetensors_slices``), in one ``ValueError``."""
+    ``read_safetensors_slices``), in one ``ValueError``.  ``stored``: {name: the file's dtype} of the tensors that are
+    converted to the dtype ``entries`` gives them."""
     problems = []
     want = {name: (dtype, shape) for name, dtype, shape, _, _ in entries}
+    stored = stored or {}
     there, what, holds = ("selected", "read_safetensors_slices", "the slice is") if sliced else \
         ("in the file", "read_safetensors", "the file holds")
     for name in sorted(set(want) - set(into)):
@@ -638,7 +641,11 @@ def _check_into(into: Mapping, entries, ctx, sliced: bool = False) -> None:
     for name in sorted(set(want) & set(into)):
         t, (dtype, shape) = into[name], want[name]
         if t.dtype != dtype or list(t.shape) != shape:
-            problems.append(f"{name!r}: {holds} {dtype} {shape}, into has {t.dtype} {list(t.shape)}")
+            if name in stored:
+                problems.append(f"{name!r}: {holds} {stored[name]} {shape}, converted to {dtype}, into has {t.dtype} "
+                                f"{list(t.shape)}")
+            else:
+                problems.append(f"{name!r}: {holds} {dtype} {shape}, into has {t.dtype} {list(t.shape)}")
             continue
         try:
             DeviceFile._Source._check_tensor(t, ctx, f"into[{name!r}]")
@@ -655,7 +662,90 @@ def _check_into(into: Mapping, entries, ctx, sliced: bool = False) -> None:
         raise ValueError(f"{what}(into=...): " + "; ".join(problems))
 
 
-async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping | None = None,
+def _cast_targets(path: str, dtype, entries, data_start: int, sliced: bool = False) -> dict:
+    """{name: target dtype} of the tensors of ``entries`` (``_safetensors_entries``; the selected ones for
+    ``read_safetensors_slices``) that ``dtype`` converts: ``None``; one of float32, float16 and bfloat16 for every
+    F32 / F16 / BF16 tensor of another dtype, integer and bool tensors unchanged; or ``{name: such a dtype}``.  Every
+    problem in one ``ValueError``: another floating dtype under a single dtype, a mapped name that is not there, an
+    unsupported target or source, and a tensor to convert whose file offset (``data_start`` + its data offset) is not a
+    multiple of its element size."""
+    if dtype is None:
+        return {}
+    import torch
+
+    codes, tags = cast_dtypes(), _st_dtypes()
+    by_name = {e[0]: e for e in entries}
+    problems, want = [], {}
+    supported = "float32, float16 or bfloat16"
+    if isinstance(dtype, Mapping):
+        for name, target in dtype.items():
+            if name not in by_name:
+                problems.append(f"{name!r} is in dtype but not {'selected' if sliced else 'in the file'}")
+            else:
+                want[name] = target
+    elif not isinstance(dtype, torch.dtype) or dtype not in codes:
+        problems.append(f"{dtype} is not a supported target ({supported})")
+    else:
+        for name, src, *_ in entries:
+            if src in codes:
+                want[name] = dtype
+            elif tags[src][0][0] in "FC":  # F64, F8_*, F4, C64: floating, but not converted
+                problems.append(f"{name!r} is {tags[src][0]}, which does not convert to {dtype}")
+    out = {}
+    for name, target in want.items():
+        _, src, _, lo, _ = by_name[name]
+        if not isinstance(target, torch.dtype) or target not in codes:
+            problems.append(f"{name!r}: {target} is not a supported target ({supported})")
+        elif src not in codes:
+            problems.append(f"{name!r} is {tags[src][0]}; only F32, F16 and BF16 tensors convert")
+        elif src != target:
+            if (data_start + lo) % src.itemsize:
+                problems.append(f"{name!r} starts at file offset {data_start + lo}, not a multiple of its element size "
+                                f"{src.itemsize}")
+            out[name] = target
+    if problems:
+        raise ValueError(f"{path}: dtype: " + "; ".join(problems))
+    return out
+
+
+async def _load_runs(client, volume_id: str, path: str, runs, dst: DeviceFile, start: int, end: int,
+                     staging_bytes: int) -> None:
+    """Load ``runs`` -- ``[((F, W, P, R) as _slice_runs gives it, packed offset in dst, (stored dtype, target dtype) or
+    None)]`` -- into ``dst``: ONE ``VolumeGetFile2`` call over file bytes [start, end), then exactly the blocks that
+    hold a byte of a run, once each, into the page-locked waves of ``_load_in_waves``.  Each complete wave makes at most
+    one ``load_boxes`` call (the unconverted runs; one also when nothing converts) and at most one ``load_cast_boxes``
+    call: every run is cut into boxes, split where the staging stops being contiguous, at a wave's edge or a skipped
+    block.  A converted run's packed offsets count target bytes."""
+    BS = blob_utils.BLOCK_SIZE
+    touched = _touched_blocks([r for r, _, _ in runs], BS)
+    if not touched:
+        return
+    slices = [s for s in await _block_slices(client, volume_id, path, start, end - start)
+              if (start + s[1]) // BS in touched]
+
+    def load(wave, at, buf, ctx):
+        plain, cast, k = [], [], 0
+        while k < len(wave):  # a stretch: blocks adjacent in the file and in the buffer
+            e = k + 1
+            while e < len(wave) and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and at[e] == at[e - 1] + wave[e - 1][2]:
+                e += 1
+            s0, s1 = start + wave[k][1], start + wave[e - 1][1] + wave[e - 1][2]
+            for run, d, conv in runs:
+                for b in _clip_run(run, 0, s0, s1, at[k]):
+                    if conv is None:
+                        plain.append((0, d + b[0], *b[1:]))
+                    else:  # the box's offset in the run, in source bytes, to target bytes
+                        cast.append((0, d + b[0] // conv[0].itemsize * conv[1].itemsize, *b[1:], *conv))
+            k = e
+        loaded = load_boxes([dst], plain, buf, ctx=ctx) if plain or not cast else None
+        if cast:  # on the same stream as the plain boxes: its completion implies theirs
+            loaded = load_cast_boxes([dst], cast, buf, ctx=ctx)
+        return loaded
+
+    await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
+
+
+async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping | None = None, dtype=None,
                            staging_bytes: int = 256 << 20) -> dict:
     """The safetensors file at ``path`` as ``{name: tensor}`` on the context's device, equal to what
     ``safetensors.torch.load`` gives for the file's bytes (same names, dtypes, shapes and values; keys in data order).
@@ -665,17 +755,37 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
     the context's device, or with ``into=`` the caller's tensors, filled in place: names, dtypes and shapes must match
     exactly and the tensors must be contiguous, on the context's device and not overlap; every mismatch is listed in one
     ``ValueError`` before any block GET.  The data region then arrives with one ``read_file_into_device`` into a
-    ``DeviceFile`` over the tensors in data order (``staging_bytes`` as there)."""
+    ``DeviceFile`` over the tensors in data order (``staging_bytes`` as there).
+
+    ``dtype`` converts tensors as they land, each result equal bit for bit to ``full.to(dtype)`` on the device: a torch
+    dtype (float32, float16 or bfloat16) for every F32 / F16 / BF16 tensor, integer and bool tensors unchanged, or
+    ``{name: dtype}`` for the tensors it names.  ``_cast_targets`` lists what it refuses, in one ``ValueError`` before
+    any data GET (a file not written by ``safetensors.torch.save`` may hold a tensor that cannot convert in place).
+    With ``into=`` each tensor must have its target dtype.  When something converts, the same ``VolumeGetFile2`` call
+    and block GETs as without ``dtype`` feed the waves of ``_load_runs``: HBM holds only the results, never the stored
+    image; when nothing converts, the call is the one without ``dtype``."""
     ctx = blob_utils.get_context()
     size, n, _, entries = await _read_safetensors_header(client, volume_id, path)
+    targets = _cast_targets(path, dtype, entries, 8 + n)
+    if targets and staging_bytes < 2 * blob_utils.BLOCK_SIZE:
+        raise ValueError(f"staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), got {staging_bytes}")
+    result = [(name, targets.get(name, dt), shape, lo, hi) for name, dt, shape, lo, hi in entries]
     if into is not None:
-        _check_into(into, entries, ctx)
+        _check_into(into, result, ctx, stored={name: dt for name, dt, *_ in entries if name in targets})
         tensors = [into[name] for name, *_ in entries]
     else:
-        tensors = [DeviceFile._Source._new_tensor(shape, dtype, ctx) for _, dtype, shape, _, _ in entries]
+        tensors = [DeviceFile._Source._new_tensor(shape, dt, ctx) for _, dt, shape, _, _ in result]
     if entries and size - 8 - n:
         dst = DeviceFile._over(DeviceFile._Source(tensors, BOUNCE_BYTES))
-        await read_file_into_device(client, volume_id, path, dst, start=8 + n, staging_bytes=staging_bytes)
+        if not targets:
+            await read_file_into_device(client, volume_id, path, dst, start=8 + n, staging_bytes=staging_bytes)
+        else:
+            runs, dest = [], 0
+            for (name, dt, _, lo, hi), t in zip(entries, tensors):
+                if hi > lo:
+                    runs.append(((8 + n + lo, hi - lo, hi - lo, 1), dest, (dt, t.dtype) if name in targets else None))
+                dest += t.numel() * t.element_size()
+            await _load_runs(client, volume_id, path, runs, dst, 8 + n, size, staging_bytes)
     return {name: t for (name, *_), t in zip(entries, tensors)}
 
 
@@ -816,7 +926,7 @@ def _clip_run(run, dest: int, s0: int, s1: int, at: int):
 
 
 async def read_safetensors_slices(client, volume_id: str, path: str, select: Mapping, *, into: Mapping | None = None,
-                                  staging_bytes: int = 256 << 20) -> dict:
+                                  dtype=None, staging_bytes: int = 256 << 20) -> dict:
     """Slices of tensors of the safetensors file at ``path``: ``{name: full[index]}`` for every ``name: index`` of
     ``select``, in its order, each a new contiguous tensor on the context's device (``full`` as ``read_safetensors``
     returns it; for these index forms also what ``safe_open(...).get_slice(name)[index]`` gives).  An index is an int
@@ -833,7 +943,9 @@ async def read_safetensors_slices(client, volume_id: str, path: str, select: Map
     skipped block.  Of HBM, the call allocates only the results and the copy's small stream-ordered tables.  With ``into=`` the caller's tensors are filled
     in place: the sliced shapes and the dtypes must match, and the tensors must be contiguous, on the context's device
     and not overlap, every mismatch in one ``ValueError`` before any data GET.  On return and on error, ordering and
-    partial content are as for ``read_safetensors``."""
+    partial content are as for ``read_safetensors``.  ``dtype`` converts the slices as they land, as
+    ``read_safetensors`` does (a mapping names selected tensors); each result equals ``full[index].to(dtype)`` bit for
+    bit, and the requests are those of the call without ``dtype``."""
     BS = blob_utils.BLOCK_SIZE
     if staging_bytes < 2 * BS:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
@@ -845,43 +957,29 @@ async def read_safetensors_slices(client, volume_id: str, path: str, select: Map
         raise ValueError(f"{path}: no tensors named {', '.join(repr(u) for u in unknown)}")
     plans = []  # (name, dtype, result shape, runs)
     for name, index in select.items():
-        _, dtype, shape, lo, _ = by_name[name]
+        _, dt, shape, lo, _ = by_name[name]
         bounds, kept = _slice_bounds(name, shape, index)
         result = [hi - b for (b, hi), k in zip(bounds, kept) if k]
-        plans.append((name, dtype, result, _slice_runs(shape, bounds, dtype.itemsize, 8 + n + lo)))
+        plans.append((name, dt, result, _slice_runs(shape, bounds, dt.itemsize, 8 + n + lo)))
+    targets = _cast_targets(path, dtype, [by_name[name] for name in select], 8 + n, sliced=True)
     if into is not None:
-        _check_into(into, [(name, dtype, result, 0, 0) for name, dtype, result, _ in plans], ctx, sliced=True)
+        _check_into(into, [(name, targets.get(name, dt), result, 0, 0) for name, dt, result, _ in plans], ctx,
+                    sliced=True, stored={name: dt for name, dt, *_ in plans if name in targets})
         tensors = [into[name] for name, *_ in plans]
     else:
-        tensors = [DeviceFile._Source._new_tensor(result, dtype, ctx) for _, dtype, result, _ in plans]
-    runs, base = [], 0  # (run, its packed offset in the one file over every result tensor)
-    for (_, _, _, rs), t in zip(plans, tensors):
-        dest = base
+        tensors = [DeviceFile._Source._new_tensor(result, targets.get(name, dt), ctx) for name, dt, result, _ in plans]
+    runs, base = [], 0  # (run, its packed offset in the one file over every result tensor, conversion)
+    for (name, dt, _, rs), t in zip(plans, tensors):
+        dest, conv = base, (dt, t.dtype) if name in targets else None
         for run in rs:
-            runs.append((run, dest))
-            dest += run[1] * run[3]
+            runs.append((run, dest, conv))
+            dest += run[1] * run[3] // dt.itemsize * t.element_size()
         base += t.numel() * t.element_size()
-    touched = _touched_blocks([r for r, _ in runs], BS)
-    if touched:
-        first = min(touched) * BS
-        end = max(F + (R - 1) * P + W for (F, W, P, R), _ in runs)
-        slices = [s for s in await _block_slices(client, volume_id, path, first, end - first)
-                  if (first + s[1]) // BS in touched]
+    if runs:
+        first = min(_touched_blocks([r for r, _, _ in runs], BS)) * BS
+        end = max(F + (R - 1) * P + W for (F, W, P, R), _, _ in runs)
         dst = DeviceFile._over(DeviceFile._Source(tensors, BOUNCE_BYTES))
-
-        def load(wave, at, buf, ctx):
-            boxes, k = [], 0
-            while k < len(wave):  # a stretch: blocks adjacent in the file and in the buffer
-                e = k + 1
-                while e < len(wave) and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and at[e] == at[e - 1] + wave[e - 1][2]:
-                    e += 1
-                s0, s1 = first + wave[k][1], first + wave[e - 1][1] + wave[e - 1][2]
-                for run, d in runs:
-                    boxes += [(0, *b) for b in _clip_run(run, d, s0, s1, at[k])]
-                k = e
-            return load_boxes([dst], boxes, buf, ctx=ctx)
-
-        await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
+        await _load_runs(client, volume_id, path, runs, dst, first, end, staging_bytes)
     return {name: t for (name, *_), t in zip(plans, tensors)}
 
 

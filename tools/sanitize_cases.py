@@ -9,6 +9,9 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
   stage        ranges of segmented device files into page-locked host memory: every source phase, segments that start
                at the first and end at the last byte of their allocation (the aligned-hull loads), ranges across tiny
                and empty segments, partial last words
+  cast boxes   load_cast_boxes_kernel: every conversion between F32, F16 and BF16, boxes that end at the last byte of
+               their exact-size destination allocation and of the page-locked source, every element phase, rows that
+               cross destination words, 1-element rows
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -112,5 +115,28 @@ for (_, off, n), o in zip(ranges, offsets):
 assert (dst[clean] == 0xC3).all()
 ctx.host_free(dst)
 print("stage ranges ok", flush=True)
+
+# 7. load_cast_boxes_kernel: each box fills an exact-size allocation; the last box reads the source's last bytes
+names = {_lib.DT_F32: torch.float32, _lib.DT_F16: torch.float16, _lib.DT_BF16: torch.bfloat16}
+src = ctx.host_alloc(1 << 20)
+src[:] = synth_array(7, 1 << 20)
+boxes, outs, at = [], [], 0
+for st, dt in [(a, b) for a in names for b in names if a != b]:
+    ss, ds = names[st].itemsize, names[dt].itemsize
+    for w, rows, gap, ph in ((1, 9, 0, 0), (3, 7, 1, 1), (37, 5, 2, 2), (9000, 2, 5, 3), (8, 1, 0, 0)):
+        at = -(-at // 16) * 16 + ph * ss
+        outs.append(torch.empty(w * rows * ds, dtype=torch.uint8, device="cuda"))
+        boxes.append((len(outs) - 1, 0, w * ss, rows, at, (w + gap) * ss, st, dt))
+        at += ((rows - 1) * (w + gap) + w) * ss
+boxes[-1] = boxes[-1][:4] + (src.size - 8 * names[boxes[-1][6]].itemsize,) + boxes[-1][5:]
+ctx.copy_cast_boxes_from_host([t.data_ptr() for t in outs], [t.numel() for t in outs], list(range(len(outs) + 1)),
+                              boxes, src)
+torch.cuda.synchronize()
+for (f, _, w, rows, a, pitch, st, dt), t in zip(boxes, outs):
+    rows_ = np.concatenate([src[a + r * pitch : a + r * pitch + w] for r in range(rows)])
+    want = torch.from_numpy(rows_).cuda().view(names[st]).to(names[dt]).view(torch.uint8)
+    assert torch.equal(t, want), (st, dt, w, rows)
+ctx.host_free(src)
+print("cast boxes ok", flush=True)
 ctx.close()
 print("ALL OK")

@@ -32,7 +32,19 @@
     against read_safetensors followed by .contiguous() slices, alternating: host clock, the bytes GET from the server,
     the peak HBM growth (torch.cuda.max_memory_allocated) and resident-set growth, and a bitwise comparison.
 
-VRB_ARMS (default "abcd") picks the arms.
+(e) loading converted to another dtype (F32 <-> BF16).
+    kernel: a VRB_GIB (2 GiB) image of F32 (then of BF16) in one page-locked buffer, as 1-row boxes of one 8 MiB block
+    each, the data region starting at 0 and at 8 mod 16 (a safetensors data region starts at either): (1) ONE
+    load_cast_boxes call (F32 -> BF16, BF16 -> F32), (2) ONE load_boxes call of the same source bytes, unconverted, and
+    (3) the unfused route: that load_boxes call into scratch HBM followed by torch's .to() into the result.  CUDA
+    events, VRB_REPS runs each, alternating, best and median; GB/s of source bytes and the share of load_boxes' rate.
+    The converted results are compared bitwise with torch's cast.
+    end to end over loopback: a VRB_E2E_GIB (1 GiB) F32 Llama-shaped file uploaded once; read_safetensors(dtype=
+    torch.bfloat16) against read_safetensors followed by .to(torch.bfloat16), alternating, VRB_E2E_REPS (2) runs each:
+    host clock, peak HBM growth (torch.cuda.max_memory_allocated) and a bitwise comparison.  The same for rank
+    VRB_RANK's TP slices: read_safetensors_slices(dtype=torch.bfloat16) against the slices followed by .to().
+
+VRB_ARMS (default "abcd") picks the arms; "e" is run only when named.
 
 The card name and power limit are read in the same run.  Needs a GPU: nothing here falls back.
 One JSON line per arm; also written to $VRB_OUT/volume_read_bench.json when set."""
@@ -501,6 +513,121 @@ async def slices_e2e_arm(info, out):
         print(json.dumps(out[-1]), flush=True)
 
 
+def cast_kernel_arm(ctx, info, out):
+    from modal_client_b200 import load_boxes, load_cast_boxes
+
+    BS = blob_utils.BLOCK_SIZE
+    n = int(float(os.environ.get("VRB_GIB", "2")) * GiB) // BS * BS
+    src = ctx.host_alloc(n + 16)
+    try:
+        torch.from_numpy(src).random_(0, 256)
+        for stored, target in ((torch.float32, torch.bfloat16), (torch.bfloat16, torch.float32)):
+            ss, ds = stored.itemsize, target.itemsize
+            plain = torch.empty(n, dtype=torch.uint8, device="cuda")  # the unconverted bytes / the unfused scratch
+            conv = torch.empty(n // ss, dtype=target, device="cuda")
+            fp, fc = DeviceFile(plain), DeviceFile(conv)
+            for phase in (0, 8):
+                # one 1-row box per 8 MiB block slot; the data region starts at `phase`
+                blocks = [(max(phase, o), o + BS - max(phase, o)) for o in range(0, n, BS)]
+                plain_boxes = [(0, a - phase, m, 1, a, m) for a, m in blocks]
+                cast_boxes = [(0, (a - phase) // ss * ds, m, 1, a, m, stored, target) for a, m in blocks]
+                nbytes = sum(m for _, m in blocks)
+                view, head = plain[: nbytes].view(stored), conv[: nbytes // ss]
+
+                def unfused():
+                    load_boxes([fp], plain_boxes, src, ctx=ctx)
+                    head.copy_(view)
+
+                cands = {"load_cast_boxes": lambda: load_cast_boxes([fc], cast_boxes, src, ctx=ctx),
+                         "load_boxes": lambda: load_boxes([fp], plain_boxes, src, ctx=ctx),
+                         "load_boxes_then_to": unfused}
+                for fn in cands.values():
+                    fn()
+                times = {k: [] for k in cands}
+                for _ in range(int(os.environ.get("VRB_REPS", "5"))):
+                    for k, fn in cands.items():
+                        times[k].append(events_ms(fn))
+                load_cast_boxes([fc], cast_boxes, src, ctx=ctx)
+                load_boxes([fp], plain_boxes, src, ctx=ctx)
+                torch.cuda.synchronize()
+                iv = torch.int16 if ds == 2 else torch.int32
+                equal = torch.equal(conv[: nbytes // ss].view(iv), view.to(target).view(iv))
+                best = {k: min(v) for k, v in times.items()}
+                for k, v in times.items():
+                    out.append({"arm": f"cast_kernel.{stored}_to_{target}.phase{phase}.{k}", "source_bytes": nbytes,
+                                "boxes": len(blocks), "best_ms": round(best[k], 3),
+                                "median_ms": round(statistics.median(v), 3), "GB_s": round(nbytes / best[k] / 1e6, 2),
+                                "share_of_load_boxes": round(best["load_boxes"] / best[k], 3), "bitwise_equal": equal,
+                                **info})
+                    print(json.dumps(out[-1]), flush=True)
+            del fp, fc, plain, conv, view, head
+    finally:
+        torch.cuda.synchronize()
+        ctx.host_free(src)
+
+
+async def cast_e2e_arm(info, out):
+    BS = blob_utils.BLOCK_SIZE
+    total = int(float(os.environ.get("VRB_E2E_GIB", "1")) * GiB)
+    rank = int(os.environ.get("VRB_RANK", "3"))
+    g = torch.Generator(device="cuda").manual_seed(8)
+    sd = {k: torch.randn(s, device="cuda", generator=g) for k, s in llama_shapes(total // 2).items()}  # F32
+    size = sum(t.numel() * 4 for t in sd.values())
+    bf16 = torch.bfloat16
+    rows = {}
+    async with running_volume_server(BS) as (stub, _):
+        client = types.SimpleNamespace(stub=stub)
+        async with volume.VolumeUploadContextManager2("vo-e", client) as batch:
+            batch.put_file(DeviceFile.safetensors(sd), "/f32.safetensors")
+        shapes = {k: tuple(t.shape) for k, t in sd.items()}
+        del sd
+        select = {k: tp_index(k, s, rank) for k, s in shapes.items()}
+
+        async def read(converted: bool, sliced: bool):
+            if sliced:
+                if converted:
+                    return await volume.read_safetensors_slices(client, "vo-e", "/f32.safetensors", select, dtype=bf16)
+                res = await volume.read_safetensors_slices(client, "vo-e", "/f32.safetensors", select)
+            else:
+                if converted:
+                    return await volume.read_safetensors(client, "vo-e", "/f32.safetensors", dtype=bf16)
+                res = await volume.read_safetensors(client, "vo-e", "/f32.safetensors")
+            out_ = {}
+            for k in list(res):
+                out_[k] = res.pop(k).to(bf16)
+            return out_
+
+        for sliced in (False, True):
+            label = "slices_rank" if sliced else "full"
+            for rep in range(int(os.environ.get("VRB_E2E_REPS", "2"))):
+                results = {}
+                order = (True, False) if rep % 2 == 0 else (False, True)
+                for converted in order:
+                    route = f"{label}.{'dtype_bf16' if converted else 'read_then_to_bf16'}"
+                    torch.cuda.synchronize()
+                    hbm = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    t0 = time.perf_counter()
+                    res = await read(converted, sliced)
+                    torch.cuda.synchronize()
+                    dt = time.perf_counter() - t0
+                    rows.setdefault(route, []).append((dt, torch.cuda.max_memory_allocated() - hbm))
+                    results[converted] = res
+                equal = all(torch.equal(results[True][k].view(torch.int16), results[False][k].view(torch.int16))
+                            for k in results[True])
+                for converted in order:
+                    route = f"{label}.{'dtype_bf16' if converted else 'read_then_to_bf16'}"
+                    rows[route][-1] += (equal,)
+                del results
+    for route, v in rows.items():
+        ts = [x[0] for x in v]
+        out.append({"arm": f"cast_loopback.{route}", "file_bytes": size, "rank": rank if "slices" in route else None,
+                    "median_s": round(statistics.median(ts), 3), "range_s": [round(min(ts), 3), round(max(ts), 3)],
+                    "peak_hbm_growth_GB": round(max(x[1] for x in v) / 1e9, 3),
+                    "bitwise_equal": all(x[2] for x in v), **info})
+        print(json.dumps(out[-1]), flush=True)
+
+
 def main():
     if not torch.cuda.is_available():
         raise SystemExit("volume_read_bench needs a GPU")
@@ -517,6 +644,9 @@ def main():
     if "d" in arms:
         slices_kernel_arm(ctx, info, out)
         asyncio.run(slices_e2e_arm(info, out))
+    if "e" in arms:
+        cast_kernel_arm(ctx, info, out)
+        asyncio.run(cast_e2e_arm(info, out))
     if os.environ.get("VRB_OUT"):
         os.makedirs(os.environ["VRB_OUT"], exist_ok=True)
         with open(os.path.join(os.environ["VRB_OUT"], "volume_read_bench.json"), "w") as fh:
