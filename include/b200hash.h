@@ -295,6 +295,45 @@ int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, u
                                     const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes,
                                     uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream);
 
+/* A segment of a file whose elements may change type on the way out: len SOURCE bytes at d_ptr (device memory on ctx's
+ * device).  src_type == dst_type: the bytes as they are (0 or a B200H_DT_* code).  Otherwise two different B200H_DT_*
+ * codes, and the segment contributes its len / (source element size) elements converted to dst_type, packed:
+ * len / ss * ds bytes of its file's image. */
+typedef struct b200h_cast_segment {
+    const void* d_ptr;
+    uint64_t len;                /* source bytes */
+    uint64_t src_type, dst_type; /* equal: the bytes as they are; else two different B200H_DT_* codes */
+} b200h_cast_segment;
+
+/* b200h_copy_ranges_to_host over files made of cast segments: range i (a b200h_file_range of the file's IMAGE, any start
+ * byte, mid-element included) of the converted images lands at dst + dst_offsets[i].  Conversion is that of
+ * b200h_copy_cast_boxes_from_host: exactly torch's CUDA .to(), NaN bit patterns included.
+ * Every argument is checked before anything is enqueued, B200H_E_INVALID otherwise: the rules of
+ * b200h_copy_ranges_to_host (file table, ranges within their files, dst_offsets multiples of 16, destinations in bounds
+ * and disjoint, segments device memory on ctx's device), and for a converting segment: d_ptr and len multiples of the
+ * source element size, and its image offset in its file a multiple of the destination element size (every file written
+ * by safetensors.torch.save meets this).  dst is 16-byte aligned page-locked host memory the device can reach, or
+ * memory of ctx's device (cudaPointerGetAttributes).
+ * ONE kernel launch (stage_cast_ranges_kernel) per call, none when every range is empty; its tables live in a
+ * stream-ordered allocation, so the call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream).  Every
+ * store is a full aligned 16-byte word except the bytes behind a range's last whole word; bytes of dst outside the
+ * destinations are not written.
+ * Replaces: safetensors.torch.save({k: v.to(dtype)}) followed by the reads of _put_missing_blocks
+ * (py/modal/volume.py:1500-1574), which holds the converted copy of every tensor in memory at once. */
+int b200h_copy_cast_ranges(b200h_ctx* ctx, const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                           uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* dst,
+                           uint64_t dst_bytes, const uint64_t* dst_offsets, void* cuda_stream);
+
+/* b200h_hash_segment_parts_device over files made of cast segments (the rules of b200h_copy_cast_ranges for them): the
+ * parts are cut from the converted images, with the same rows, flags, outputs and synchronisation rules.  A part is
+ * hashed in place only when it lies in one segment that converts nothing; every other part is gathered into a wave
+ * slot by stage_cast_ranges_kernel (one launch per wave), so the converted bytes never exist in HBM outside the wave
+ * slots.  b200h_cast_segment_parts_preview shows the split. */
+int b200h_hash_cast_segment_parts_device(b200h_ctx* ctx, const b200h_cast_segment* segs, uint64_t nsegs,
+                                         const uint64_t* file_first_seg, uint64_t nfiles, uint64_t part_len,
+                                         uint32_t flags, void* d_sha256, void* d_md5, uint64_t* d_trimmed_len,
+                                         uint64_t* nparts_out, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.
@@ -373,6 +412,11 @@ int b200h_plan_preview(const uint64_t* lengths, uint64_t n, uint32_t flags, uint
 int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
                                 uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out, uint64_t* nwaves_out,
                                 uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap);
+/* The same for b200h_hash_cast_segment_parts_device: segments as b200h_cast_segment (their pointers unused, every other
+ * rule checked); a part is in place only in a segment that converts nothing. */
+int b200h_cast_segment_parts_preview(const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                     uint64_t nfiles, uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out,
+                                     uint64_t* nwaves_out, uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap);
 /* Kernels launched by this context so far (all kinds). */
 uint64_t b200h_launch_count(b200h_ctx* ctx);
 /* Combining queue of b200h_hash_batch_host: GPU batches issued for, and caller requests served by, the small-request

@@ -36,7 +36,8 @@ ABI_SYMBOLS = (
     "b200h_stream_copy", "b200h_stream_copy_isa", "b200h_plan_preview", "b200h_pack_preview",
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
     "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host", "b200h_copy_boxes_from_host",
-    "b200h_copy_cast_boxes_from_host",
+    "b200h_copy_cast_boxes_from_host", "b200h_copy_cast_ranges", "b200h_hash_cast_segment_parts_device",
+    "b200h_cast_segment_parts_preview",
 )
 
 
@@ -120,6 +121,14 @@ def load_library() -> ctypes.CDLL:
         L.b200h_copy_boxes_from_host.restype = i32
         L.b200h_copy_cast_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
         L.b200h_copy_cast_boxes_from_host.restype = i32
+        L.b200h_copy_cast_ranges.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
+        L.b200h_copy_cast_ranges.restype = i32
+        L.b200h_hash_cast_segment_parts_device.argtypes = [vp, vp, u64, vp, u64, u64, u32, vp, vp, vp,
+                                                           ctypes.POINTER(u64), vp]
+        L.b200h_hash_cast_segment_parts_device.restype = i32
+        L.b200h_cast_segment_parts_preview.argtypes = [vp, u64, vp, u64, u64, u64, ctypes.POINTER(u64),
+                                                       ctypes.POINTER(u64), vp, vp, u64]
+        L.b200h_cast_segment_parts_preview.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -227,20 +236,50 @@ def segment_parts_preview(seg_lens, file_first_seg, part_len: int, wave_bytes: i
     """How ``Context.hash_segment_parts_device`` splits these files (file f = segments file_first_seg[f] ..
     file_first_seg[f+1]) for wave slots of ``wave_bytes``: -> (seg uint64[nparts]: the segment each part is hashed in
     place in, or ``GATHERED``; wave uint32[nparts]; number of waves).  The library's own host code; no GPU."""
-    L = load_library()
     ln = np.ascontiguousarray(seg_lens, dtype=np.uint64)
+    return _preview("b200h_segment_parts_preview", _np_ptr(ln), ln.size, file_first_seg, part_len, wave_bytes)
+
+
+def cast_segment_parts_preview(seg_lens, src_types, dst_types, file_first_seg, part_len: int, wave_bytes: int):
+    """``segment_parts_preview`` for ``Context.hash_cast_segment_parts_device``: segment s holds seg_lens[s] SOURCE
+    bytes of type src_types[s], converted to dst_types[s] (equal types: the bytes as they are).  A part is in place
+    only in a segment that converts nothing.  The library's own host code and argument rules; no GPU."""
+    segs = _cast_segments(np.zeros(len(seg_lens), np.uint64), seg_lens, src_types, dst_types)
+    return _preview("b200h_cast_segment_parts_preview", _np_ptr(segs) if len(segs) else None, len(segs), file_first_seg,
+                    part_len, wave_bytes)
+
+
+def _preview(entry: str, segs, nsegs: int, file_first_seg, part_len: int, wave_bytes: int):
+    fn = getattr(load_library(), entry)
     ffs, nfiles = _segment_args(file_first_seg)
     n, w = ctypes.c_uint64(), ctypes.c_uint64()
-    rc = L.b200h_segment_parts_preview(_np_ptr(ln), ln.size, _np_ptr(ffs), nfiles, part_len, wave_bytes, ctypes.byref(n),
-                                       ctypes.byref(w), None, None, 0)
+    rc = fn(segs, nsegs, _np_ptr(ffs), nfiles, part_len, wave_bytes, ctypes.byref(n), ctypes.byref(w), None, None, 0)
     if rc != 0:
-        raise B200HashError(f"b200h_segment_parts_preview failed ({rc})")
+        raise B200HashError(f"{entry} failed ({rc})")
     seg, wave = np.empty(n.value, np.uint64), np.empty(n.value, np.uint32)
     if n.value:
-        rc = L.b200h_segment_parts_preview(_np_ptr(ln), ln.size, _np_ptr(ffs), nfiles, part_len, wave_bytes, None, None,
-                                           _np_ptr(seg), _np_ptr(wave), n.value)
+        rc = fn(segs, nsegs, _np_ptr(ffs), nfiles, part_len, wave_bytes, None, None, _np_ptr(seg), _np_ptr(wave), n.value)
         assert rc == 0
     return seg, wave, int(w.value)
+
+
+def _cast_segments(ptrs, lens, src_types, dst_types) -> np.ndarray:
+    """The b200h_cast_segment {d_ptr, len, src_type, dst_type} array, as uint64[n, 4]."""
+    segs = np.empty((len(lens), 4), np.uint64)
+    segs[:, :2] = _segments(ptrs, lens)
+    for col, types in ((2, src_types), (3, dst_types)):
+        t = np.ascontiguousarray(types, dtype=np.uint64)
+        if t.shape != (len(segs),):
+            raise ValueError("src_types and dst_types need one entry per segment")
+        segs[:, col] = t
+    return segs
+
+
+def _dst_buffer(dst) -> tuple[int, int]:
+    """(address, bytes) of a uint8 numpy array (page-locked host memory) or a CUDA tensor."""
+    if isinstance(dst, np.ndarray):
+        return dst.ctypes.data, dst.size
+    return dst.data_ptr(), dst.numel() * dst.element_size()
 
 
 class Context:
@@ -433,6 +472,22 @@ class Context:
         self._check(rc, "b200h_hash_segment_parts_device")
         return int(got.value)
 
+    def hash_cast_segment_parts_device(self, seg_ptrs, seg_lens, src_types, dst_types, file_first_seg, part_len: int,
+                                       flags: int, d_sha: int = 0, d_md5: int = 0, d_trimmed: int = 0,
+                                       stream: int = 0) -> int:
+        """``hash_segment_parts_device`` over the converted images of files made of device buffers: segment s holds
+        seg_lens[s] source bytes of type src_types[s] at seg_ptrs[s], converted to dst_types[s] (``DT_*``; equal
+        types: the bytes as they are).  Returns the row count."""
+        segs = _cast_segments(seg_ptrs, seg_lens, src_types, dst_types)
+        ffs, nfiles = _segment_args(file_first_seg)
+        got = ctypes.c_uint64()
+        rc = self._L.b200h_hash_cast_segment_parts_device(self._h, _np_ptr(segs) if len(segs) else None, len(segs),
+                                                          _np_ptr(ffs), nfiles, part_len, flags, d_sha or None,
+                                                          d_md5 or None, d_trimmed or None, ctypes.byref(got),
+                                                          stream or None)
+        self._check(rc, "b200h_hash_cast_segment_parts_device")
+        return int(got.value)
+
     def crc32_device(self, ptrs, lens, d_out: int, stream: int = 0) -> None:
         """zlib.crc32 of every device range (lens[i] bytes at device address ptrs[i]) into the device uint32 array at
         ``d_out``, computed on the device; the work is only enqueued on ``stream``."""
@@ -449,6 +504,25 @@ class Context:
         ``stream``: ``dst`` holds the bytes once that stream's work has completed."""
         self._copy_ranges("b200h_copy_ranges_to_host", "dst_offsets", seg_ptrs, seg_lens, file_first_seg, ranges, dst,
                           dst_offsets, stream)
+
+    def copy_cast_ranges(self, seg_ptrs, seg_lens, src_types, dst_types, file_first_seg, ranges, dst, dst_offsets,
+                         stream: int = 0) -> None:
+        """``copy_ranges_to_host`` over the converted images of files made of device buffers (segments as for
+        ``hash_cast_segment_parts_device``): range i = ``(file, offset, len)`` of a file's image, any start byte, lands
+        at ``dst_offsets[i]`` of ``dst`` -- a uint8 array over page-locked memory from ``host_alloc``, or a CUDA tensor
+        on the context's device (offsets multiples of 16, destinations disjoint).  One kernel launch, only enqueued on
+        ``stream``."""
+        segs = _cast_segments(seg_ptrs, seg_lens, src_types, dst_types)
+        ffs, nfiles = _segment_args(file_first_seg)
+        rg = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 3)
+        offs = np.ascontiguousarray(dst_offsets, dtype=np.uint64)
+        if offs.shape != (len(rg),):
+            raise ValueError("dst_offsets needs one entry per range")
+        addr, nbytes = _dst_buffer(dst)
+        rc = self._L.b200h_copy_cast_ranges(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
+                                            nfiles, _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(addr),
+                                            nbytes, _np_ptr(offs) if len(rg) else None, stream or None)
+        self._check(rc, "b200h_copy_cast_ranges")
 
     def copy_ranges_from_host(self, seg_ptrs, seg_lens, file_first_seg, ranges, src: np.ndarray, src_offsets,
                               stream: int = 0) -> None:

@@ -839,6 +839,50 @@ void file_pieces(const FileTable& t, uint64_t file, uint64_t offset, uint64_t le
     }
 }
 
+// Bytes of one element of a B200H_DT_* type; 0 for an unknown code.
+static uint64_t dt_bytes(uint64_t t) {
+    return t == B200H_DT_F32 ? 4 : t == B200H_DT_F16 || t == B200H_DT_BF16 ? 2 : 0;
+}
+
+static bool converts(const b200h_cast_segment& c) { return c.src_type != c.dst_type; }
+static const b200h_cast_segment kNoSegment{};  // what the cast entries pass as their segments when nsegs == 0
+
+// The file table of cast segments (file_table over their image lengths, which `seg_lens` receives) and their source
+// ranges as plain segments in `plain` (for segments_on_device).  Checks every rule of a cast segment: known type codes
+// (equal codes are 0 or a B200H_DT_* code), a converting segment's length and, with check_ptrs, its address multiples
+// of the source element size, and its image offset in its file a multiple of the destination element size.
+static int cast_file_table(const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                           uint64_t nfiles, bool check_ptrs, std::vector<uint64_t>& seg_lens,
+                           std::vector<b200h_segment>& plain, FileTable& t, std::string& err) {
+    if (nsegs && !segs) return err = "segments must not be NULL", B200H_E_INVALID;
+    seg_lens.assign(nsegs, 0);
+    plain.assign(nsegs, b200h_segment{nullptr, 0});
+    for (uint64_t s = 0; s < nsegs; ++s) {
+        const b200h_cast_segment& c = segs[s];
+        const std::string name = "segment " + std::to_string(s);
+        const uint64_t ss = dt_bytes(c.src_type), ds = dt_bytes(c.dst_type);
+        plain[s] = {c.d_ptr, c.len};
+        seg_lens[s] = c.len;
+        if (!converts(c)) {
+            if (c.src_type && !ss) return err = name + ": unknown element type", B200H_E_INVALID;
+            continue;
+        }
+        if (!ss || !ds) return err = name + ": unknown element type", B200H_E_INVALID;
+        if (c.len % ss) return err = name + ": its length is not a multiple of the source element size", B200H_E_INVALID;
+        if (check_ptrs && (uintptr_t)c.d_ptr % ss)
+            return err = name + ": its address is not a multiple of the source element size", B200H_E_INVALID;
+        if (c.len / ss > ~0ull / ds) return err = name + ": its image is larger than 2^64 - 1 bytes", B200H_E_INVALID;
+        seg_lens[s] = c.len / ss * ds;
+    }
+    if (int rc = file_table(segs ? seg_lens.data() : nullptr, nsegs, file_first_seg, nfiles, t, err)) return rc;
+    for (uint64_t s = 0; s < nsegs; ++s)
+        if (converts(segs[s]) && t.seg_start[s] % dt_bytes(segs[s].dst_type))
+            return err = "segment " + std::to_string(s) + ": its image starts at file offset " +
+                         std::to_string(t.seg_start[s]) + ", not a multiple of the destination element size",
+                   B200H_E_INVALID;
+    return 0;
+}
+
 constexpr uint64_t kInPlace = ~0ull;
 
 // Where every part of a segmented batch is hashed: b200h_segment_parts_preview reports it, and
@@ -859,8 +903,10 @@ struct SegmentParts {
     std::vector<uint64_t> wave_bytes;  // staged bytes of every wave
 };
 
-// Fills `p`; returns 0, or B200H_E_INVALID with the reason in `err`.
-int layout_segment_parts(const FileTable& t, uint64_t part_len, uint64_t wave_cap, SegmentParts& p, std::string& err) {
+// Fills `p`; returns 0, or B200H_E_INVALID with the reason in `err`.  With `casts` (the segments of
+// b200h_hash_cast_segment_parts_device), a part is hashed in place only when its segment converts nothing.
+int layout_segment_parts(const FileTable& t, uint64_t part_len, uint64_t wave_cap, SegmentParts& p, std::string& err,
+                         const b200h_cast_segment* casts = nullptr) {
     if (part_len == 0) return err = "part_len must be > 0", B200H_E_INVALID;
     if (wave_cap == 0) return err = "wave_bytes must be > 0", B200H_E_INVALID;
     for (uint64_t f = 0; f < t.size.size(); ++f) {
@@ -874,7 +920,7 @@ int layout_segment_parts(const FileTable& t, uint64_t part_len, uint64_t wave_ca
                 p.seg_off.push_back(in);
             });
             p.file.push_back(f);
-            p.stage.push_back(npieces == 1 ? kInPlace : 0);
+            p.stage.push_back(npieces == 1 && !(casts && converts(casts[p.seg.back()])) ? kInPlace : 0);
         }
     }
     const uint64_t nparts = p.off.size();
@@ -961,24 +1007,64 @@ int launch_with_tables(b200h_ctx* ctx, cudaStream_t st, const std::vector<A>& a,
     return 0;
 }
 
+// The piece of segment s (bytes [in, in + n) of its image) that lands at destination offset `at`: `segs` are the
+// source ranges, `casts` (may be NULL) the segments' types.
+static CastPiece cast_piece(const b200h_segment* segs, const b200h_cast_segment* casts, uint64_t s, uint64_t in,
+                            uint64_t n, uint64_t at) {
+    const uint64_t dev = (uint64_t)(uintptr_t)segs[s].d_ptr;
+    if (!casts || !converts(casts[s])) return {{dev + in, at, n}, 0, 0, 0, 0};
+    const uint64_t ss = dt_bytes(casts[s].src_type), ds = dt_bytes(casts[s].dst_type);
+    return {{dev + in / ds * ss, at, n}, (uint32_t)casts[s].src_type, (uint32_t)casts[s].dst_type, (uint32_t)(in % ds), 0};
+}
+
+// Appends the pieces of bytes [offset, offset + len) of file `file` (len > 0) landing at destination offset `at`, in
+// file order, and the tiles of their destination bytes (kStageTileBytes each, the last one shorter), which use them.
+static void range_tables(const FileTable& t, const b200h_segment* segs, const b200h_cast_segment* casts, uint64_t file,
+                         uint64_t offset, uint64_t len, uint64_t at, std::vector<CastPiece>& pieces,
+                         std::vector<RangeTile>& tiles) {
+    const size_t first = pieces.size();
+    uint64_t h = at;
+    file_pieces(t, file, offset, len, [&](uint64_t s, uint64_t in, uint64_t n) {
+        pieces.push_back(cast_piece(segs, casts, s, in, n, h));
+        h += n;
+    });
+    size_t p = first;
+    for (uint64_t o = 0; o < len; o += kStageTileBytes) {
+        const uint64_t n = std::min(kStageTileBytes, len - o), d = at + o;
+        while (pieces[p].r.host + pieces[p].r.len <= d) ++p;
+        size_t q = p;
+        while (q + 1 < pieces.size() && pieces[q + 1].r.host < d + n) ++q;
+        tiles.push_back({d, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
+    }
+}
+
 // b200h_hash_segment_parts_device with ctx->mu held, on stream `st`.  d_etag_msg != NULL (b200h_hash_fixed_parts_device):
 // two more words, the ETag message {0, nparts * 16}, ride the part-table upload, even when there are no parts, and
-// *d_etag_msg points at them.
+// *d_etag_msg points at them.  With `casts` (b200h_hash_cast_segment_parts_device; segs is then NULL), the files are
+// the cast segments' images, and the parts that are not hashed in place are gathered by stage_cast_ranges_kernel.
 int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
                               uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
-                              uint64_t* d_trimmed_len, uint64_t* nparts_out, cudaStream_t st, const uint64_t** d_etag_msg) {
+                              uint64_t* d_trimmed_len, uint64_t* nparts_out, cudaStream_t st, const uint64_t** d_etag_msg,
+                              const b200h_cast_segment* casts = nullptr) {
     if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
     if (((uintptr_t)d_sha256 | (uintptr_t)d_md5) & 15u)
         return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
     std::vector<uint64_t> seg_lens;
+    std::vector<b200h_segment> plain;
     FileTable t;
-    if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
+    std::string err;
+    if (casts) {
+        if (int rc = cast_file_table(casts, nsegs, file_first_seg, nfiles, true, seg_lens, plain, t, err))
+            return fail(ctx, rc, err);
+        segs = plain.data();
+    } else if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) {
+        return rc;
+    }
     // before the layout, whose part list the segments' lengths size
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
     SegmentParts p;
-    std::string err;
-    if (int rc = layout_segment_parts(t, part_len, std::max(ctx->dwave_cap, ctx->dwave_want), p, err))
+    if (int rc = layout_segment_parts(t, part_len, std::max(ctx->dwave_cap, ctx->dwave_want), p, err, casts))
         return fail(ctx, rc, err);
     const uint64_t nparts = p.off.size();
     if (nparts && !(flags & (B200H_SHA256 | B200H_MD5)))
@@ -997,6 +1083,9 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     if (d_etag_msg) table.insert(table.end(), {0, nparts * 16});
     std::vector<uint64_t> wave_tiles(nwaves + 1, 0);  // tiles of wave w: [wave_tiles[w], wave_tiles[w + 1])
     std::vector<GatherTile> tiles;
+    // with casts: the tables of every wave's stage_cast_ranges_kernel launch (destination offsets in the wave's slot)
+    std::vector<std::vector<CastPiece>> cast_pieces(casts ? nwaves : 0);
+    std::vector<std::vector<RangeTile>> cast_tiles(casts ? nwaves : 0);
     for (size_t w = 0; w < nwaves; ++w) {
         uint8_t* slot = ctx->dwave[w & 1];
         for (uint64_t i = p.wave_first[w]; i < p.wave_first[w + 1]; ++i) {
@@ -1006,6 +1095,10 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
                 continue;
             }
             table[i] = (uint64_t)(uintptr_t)(slot + p.stage[i]);
+            if (casts) {
+                range_tables(t, segs, casts, p.file[i], p.off[i], p.len[i], p.stage[i], cast_pieces[w], cast_tiles[w]);
+                continue;
+            }
             uint64_t at = table[i];
             file_pieces(t, p.file[i], p.off[i], p.len[i], [&](uint64_t s, uint64_t in, uint64_t n) {
                 for (uint64_t k = 0; k < n; k += kGatherTileBytes)
@@ -1030,12 +1123,21 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     for (size_t w = 0; w < nwaves; ++w) {
         const uint64_t i0 = p.wave_first[w], cnt = p.wave_first[w + 1] - i0;
         const int slot = (int)(w & 1);
-        const bool staged = wave_tiles[w + 1] > wave_tiles[w];
+        const bool staged = casts ? !cast_tiles[w].empty() : wave_tiles[w + 1] > wave_tiles[w];
         if (staged) {
             // the slot is shared with the *_host entry points and the previous waves: wait for its last reader
             CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_consumed[slot], 0));
-            ctx->launches += launch_gather_segments(d_tiles + wave_tiles[w], wave_tiles[w + 1] - wave_tiles[w], st);
-            CU_TRY(ctx, cudaGetLastError());
+            if (casts) {
+                if (int rc = launch_with_tables(ctx, st, cast_tiles[w], cast_pieces[w],
+                                                [&](const RangeTile* d_ct, const CastPiece* d_cp) {
+                                                    return launch_stage_cast_ranges(d_ct, cast_tiles[w].size(), d_cp,
+                                                                                    ctx->dwave[slot], st);
+                                                }))
+                    return rc;
+            } else {
+                ctx->launches += launch_gather_segments(d_tiles + wave_tiles[w], wave_tiles[w + 1] - wave_tiles[w], st);
+                CU_TRY(ctx, cudaGetLastError());
+            }
         }
         if (int rc = enqueue_device_batch(ctx, nullptr, d_table + i0, d_table + nparts + i0, cnt, flags & kPublicFlags,
                                           o_sha ? o_sha + 32 * i0 : nullptr, o_md5 ? o_md5 + 16 * i0 : nullptr,
@@ -1412,6 +1514,19 @@ int b200h_hash_segment_parts_device(b200h_ctx* ctx, const b200h_segment* segs, u
                                      nullptr);
 }
 
+int b200h_hash_cast_segment_parts_device(b200h_ctx* ctx, const b200h_cast_segment* segs, uint64_t nsegs,
+                                         const uint64_t* file_first_seg, uint64_t nfiles, uint64_t part_len,
+                                         uint32_t flags, void* d_sha256, void* d_md5, uint64_t* d_trimmed_len,
+                                         uint64_t* nparts_out, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_hash_cast_segment_parts_device");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segments must not be NULL");
+    return hash_segment_parts_locked(ctx, nullptr, nsegs, file_first_seg, nfiles, part_len, flags, d_sha256, d_md5,
+                                     d_trimmed_len, nparts_out, cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp,
+                                     nullptr, segs ? segs : &kNoSegment);
+}
+
 int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, uint32_t* d_crc_out, void* cuda_stream) {
     if (!ctx) return B200H_E_INVALID;
     B200H_RANGE("b200h_crc32_device");
@@ -1457,14 +1572,25 @@ static void* pinned_device_pointer(b200h_ctx* ctx, const void* h, uint64_t bytes
 
 // b200h_copy_ranges_to_host (to_host) and b200h_copy_ranges_from_host: range i of the segmented files and bytes
 // [host_offsets[i], host_offsets[i] + len) of the page-locked buffer `host` are copied one way or the other.
+// b200h_copy_cast_ranges (casts != NULL, segs NULL, to_host): the files are the cast segments' images, and `host` is
+// page-locked host memory or memory of ctx's device.
 static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, uint64_t nsegs,
                        const uint64_t* file_first_seg, uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges,
-                       const void* host, uint64_t host_bytes, const uint64_t* host_offsets, void* cuda_stream) {
-    const std::string buf = to_host ? "h_dst" : "h_src", offsets = to_host ? "dst_offsets" : "src_offsets",
+                       const void* host, uint64_t host_bytes, const uint64_t* host_offsets, void* cuda_stream,
+                       const b200h_cast_segment* casts = nullptr) {
+    const std::string buf = casts ? "dst" : to_host ? "h_dst" : "h_src", offsets = to_host ? "dst_offsets" : "src_offsets",
                       noun = to_host ? "destination" : "source";
     std::vector<uint64_t> seg_lens;
+    std::vector<b200h_segment> plain;
     FileTable t;
-    if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
+    if (casts) {
+        std::string err;
+        if (int rc = cast_file_table(casts, nsegs, file_first_seg, nfiles, true, seg_lens, plain, t, err))
+            return fail(ctx, rc, err);
+        segs = plain.data();
+    } else if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) {
+        return rc;
+    }
     if (nranges && (!ranges || !host_offsets))
         return fail(ctx, B200H_E_INVALID, "ranges and " + offsets + " must not be NULL");
     if (nranges && !host) return fail(ctx, B200H_E_INVALID, buf + " must not be NULL");
@@ -1492,46 +1618,43 @@ static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, 
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
     if (nranges == 0) return 0;
-    void* d_host = pinned_device_pointer(ctx, host, host_bytes);
+    void* d_host = casts && device_range_ok(ctx, host, host_bytes) ? const_cast<void*>(host)
+                                                                   : pinned_device_pointer(ctx, host, host_bytes);
     if (!d_host)
         return fail(ctx, B200H_E_INVALID,
-                    buf + " is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
+                    buf + (casts ? " is neither device memory on cuda:" + std::to_string(ctx->device) +
+                                       " nor page-locked host memory it can reach"
+                                 : " is not page-locked host memory reachable from cuda:" +
+                                       std::to_string(ctx->device)));
     if (order.empty()) return 0;
 
     // pieces (range x segment, in file order within a range) and the tiles of host bytes that use them
-    std::vector<RangePiece> pieces;
+    std::vector<CastPiece> pieces;
     std::vector<RangeTile> tiles;
     std::vector<uint64_t> range_of;  // per piece: the range it belongs to (for the overlap message)
     for (uint64_t i = 0; i < nranges; ++i) {
         const b200h_file_range& r = ranges[i];
         if (!r.len) continue;
-        const size_t first = pieces.size();
-        uint64_t at = host_offsets[i];
-        file_pieces(t, r.file, r.offset, r.len, [&](uint64_t s, uint64_t in, uint64_t n) {
-            pieces.push_back({(uint64_t)(uintptr_t)segs[s].d_ptr + in, at, n});
-            range_of.push_back(i);
-            at += n;
-        });
-        size_t p = first;
-        for (uint64_t o = 0; o < r.len; o += kStageTileBytes) {
-            const uint64_t n = std::min(kStageTileBytes, r.len - o), h = host_offsets[i] + o;
-            while (pieces[p].host + pieces[p].len <= h) ++p;
-            size_t q = p;
-            while (q + 1 < pieces.size() && pieces[q + 1].host < h + n) ++q;
-            tiles.push_back({h, (uint32_t)n, (uint32_t)(q - p + 1), (uint64_t)p});
-        }
+        range_tables(t, segs, casts, r.file, r.offset, r.len, host_offsets[i], pieces, tiles);
+        range_of.resize(pieces.size(), i);
     }
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    if (casts)
+        return launch_with_tables(ctx, st, tiles, pieces, [&](const RangeTile* d_tiles, const CastPiece* d_pieces) {
+            return launch_stage_cast_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
+        });
+    std::vector<RangePiece> bytes(pieces.size());
+    for (size_t k = 0; k < pieces.size(); ++k) bytes[k] = pieces[k].r;
     if (!to_host) {  // no device byte may be written twice: two files, or two segments of one file, may share a tensor
-        std::vector<size_t> by_dev(pieces.size());
+        std::vector<size_t> by_dev(bytes.size());
         for (size_t k = 0; k < by_dev.size(); ++k) by_dev[k] = k;
-        std::sort(by_dev.begin(), by_dev.end(), [&](size_t a, size_t b) { return pieces[a].dev < pieces[b].dev; });
+        std::sort(by_dev.begin(), by_dev.end(), [&](size_t a, size_t b) { return bytes[a].dev < bytes[b].dev; });
         for (size_t k = 1; k < by_dev.size(); ++k)
-            if (pieces[by_dev[k - 1]].dev + pieces[by_dev[k - 1]].len > pieces[by_dev[k]].dev)
+            if (bytes[by_dev[k - 1]].dev + bytes[by_dev[k - 1]].len > bytes[by_dev[k]].dev)
                 return fail(ctx, B200H_E_INVALID, "ranges " + std::to_string(range_of[by_dev[k - 1]]) + " and " +
                                                       std::to_string(range_of[by_dev[k]]) + " write the same device bytes");
     }
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    return launch_with_tables(ctx, st, tiles, pieces, [&](const RangeTile* d_tiles, const RangePiece* d_pieces) {
+    return launch_with_tables(ctx, st, tiles, bytes, [&](const RangeTile* d_tiles, const RangePiece* d_pieces) {
         return to_host ? launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_host, st)
                        : launch_load_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
     });
@@ -1557,9 +1680,15 @@ int b200h_copy_ranges_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint6
                        cuda_stream);
 }
 
-// Bytes of one element of a B200H_DT_* type; 0 for an unknown code.
-static uint64_t dt_bytes(uint64_t t) {
-    return t == B200H_DT_F32 ? 4 : t == B200H_DT_F16 || t == B200H_DT_BF16 ? 2 : 0;
+int b200h_copy_cast_ranges(b200h_ctx* ctx, const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                           uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges, void* dst,
+                           uint64_t dst_bytes, const uint64_t* dst_offsets, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_cast_ranges");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segments must not be NULL");
+    return copy_ranges(ctx, true, nullptr, nsegs, file_first_seg, nfiles, ranges, nranges, dst, dst_bytes, dst_offsets,
+                       cuda_stream, segs ? segs : &kNoSegment);
 }
 
 // b200h_copy_boxes_from_host (casts == NULL) and b200h_copy_cast_boxes_from_host (boxes == NULL; box i is
@@ -2093,6 +2222,18 @@ int b200h_plan_preview(const uint64_t* lengths, uint64_t n, uint32_t flags, uint
     return 0;
 }
 
+// The outputs of the two previews.
+static void report_segment_parts(const SegmentParts& p, uint64_t* nparts_out, uint64_t* nwaves_out, uint64_t* seg_out,
+                                 uint32_t* wave_out, uint64_t out_cap) {
+    const uint64_t nparts = p.off.size();
+    if (nparts_out) *nparts_out = nparts;
+    if (nwaves_out) *nwaves_out = p.wave_bytes.size();
+    for (uint64_t i = 0; i < std::min(nparts, out_cap); ++i) {
+        if (seg_out) seg_out[i] = p.stage[i] == kInPlace ? p.seg[i] : kInPlace;
+        if (wave_out) wave_out[i] = p.wave[i];
+    }
+}
+
 int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const uint64_t* file_first_seg, uint64_t nfiles,
                                 uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out, uint64_t* nwaves_out,
                                 uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap) {
@@ -2101,13 +2242,21 @@ int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const 
     std::string err;
     if (int rc = file_table(seg_lens, nsegs, file_first_seg, nfiles, t, err)) return rc;
     if (int rc = layout_segment_parts(t, part_len, wave_bytes, p, err)) return rc;
-    const uint64_t nparts = p.off.size();
-    if (nparts_out) *nparts_out = nparts;
-    if (nwaves_out) *nwaves_out = p.wave_bytes.size();
-    for (uint64_t i = 0; i < std::min(nparts, out_cap); ++i) {
-        if (seg_out) seg_out[i] = p.stage[i] == kInPlace ? p.seg[i] : kInPlace;
-        if (wave_out) wave_out[i] = p.wave[i];
-    }
+    report_segment_parts(p, nparts_out, nwaves_out, seg_out, wave_out, out_cap);
+    return 0;
+}
+
+int b200h_cast_segment_parts_preview(const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                     uint64_t nfiles, uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out,
+                                     uint64_t* nwaves_out, uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap) {
+    std::vector<uint64_t> seg_lens;
+    std::vector<b200h_segment> plain;
+    FileTable t;
+    SegmentParts p;
+    std::string err;
+    if (int rc = cast_file_table(segs, nsegs, file_first_seg, nfiles, false, seg_lens, plain, t, err)) return rc;
+    if (int rc = layout_segment_parts(t, part_len, wave_bytes, p, err, segs ? segs : &kNoSegment)) return rc;
+    report_segment_parts(p, nparts_out, nwaves_out, seg_out, wave_out, out_cap);
     return 0;
 }
 

@@ -122,6 +122,19 @@ constexpr uint64_t kStageTileBytes = 64 << 10;
 int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, void* dst, cudaStream_t st);
 // The inverse, host -> device; `src` is 16-byte aligned memory the device can load from.
 int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
+// A piece of a range whose segment may convert its elements on the way out (stage_cast_ranges_kernel).  src_type ==
+// dst_type: `r` as in RangePiece, the bytes as they are, phase 0.  Otherwise the piece's bytes are its segment's image
+// (the source elements converted, the B200H_DT_* codes of b200hash.h): r.dev is the source address of the element that
+// holds the piece's first image byte, which is byte `phase` of that element's converted value; r.host and r.len count
+// image bytes.
+struct CastPiece {
+    RangePiece r;
+    uint32_t src_type, dst_type, phase, pad;
+};
+// Every tile's copy of the pieces' images, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the
+// device can store to (page-locked host memory or device memory).
+int launch_stage_cast_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces, void* dst,
+                             cudaStream_t st);
 
 // Boxes of a host buffer copied into segmented device files (load_boxes_kernel, b200hash_stage.cu).  A box is `rows`
 // rows of `width` bytes, row r at byte src + r * pitch of the host buffer, packed into one destination run.  Its source

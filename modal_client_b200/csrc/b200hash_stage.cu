@@ -55,15 +55,50 @@ __device__ __forceinline__ uint4 load_word(const uint8_t* src) {
     return sh ? shift_bytes(lo, __ldg(a + 1), sh) : lo;
 }
 
+__device__ __forceinline__ const RangePiece& range_of(const RangePiece& p) { return p; }
+__device__ __forceinline__ const RangePiece& range_of(const CastPiece& p) { return p.r; }
+
 // the piece of pc[lo .. n) that holds destination offset d (the pieces of a range tile its destination without gaps)
-__device__ __forceinline__ uint32_t find_piece(const RangePiece* __restrict__ pc, uint32_t lo, uint32_t n, uint64_t d) {
+template <class Piece>
+__device__ __forceinline__ uint32_t find_piece(const Piece* __restrict__ pc, uint32_t lo, uint32_t n, uint64_t d) {
     uint32_t hi = n - 1;
     while (lo < hi) {
         const uint32_t mid = (lo + hi + 1) >> 1;
-        if (pc[mid].host <= d) lo = mid;
+        if (range_of(pc[mid]).host <= d) lo = mid;
         else hi = mid - 1;
     }
     return lo;
+}
+
+// A tile whose bytes all come, as they are, from one piece at `src`: one phase, no lookups.
+__device__ __forceinline__ void stage_one_piece(const uint8_t* src, uint8_t* out, uint32_t words, uint32_t tail) {
+    const uint32_t sh = (uint32_t)((uintptr_t)src & 15u);
+    const uint4* a = reinterpret_cast<const uint4*>(src - sh);
+    uint4* o = reinterpret_cast<uint4*>(out);
+    uint32_t w = threadIdx.x;
+    if (sh == 0) {
+        for (; w + 3 * kStageThreads < words; w += 4 * kStageThreads) {
+            uint4 v[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) v[i] = __ldg(a + w + i * kStageThreads);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) o[w + i * kStageThreads] = v[i];
+        }
+        for (; w < words; w += kStageThreads) o[w] = __ldg(a + w);
+    } else {
+        for (; w + 3 * kStageThreads < words; w += 4 * kStageThreads) {
+            uint4 lo[4], hi[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                lo[i] = __ldg(a + w + i * kStageThreads);
+                hi[i] = __ldg(a + w + i * kStageThreads + 1);
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) o[w + i * kStageThreads] = shift_bytes(lo[i], hi[i], sh);
+        }
+        for (; w < words; w += kStageThreads) o[w] = shift_bytes(__ldg(a + w), __ldg(a + w + 1), sh);
+    }
+    if (threadIdx.x < tail) out[(uint64_t)words * 16 + threadIdx.x] = src[(uint64_t)words * 16 + threadIdx.x];
 }
 
 __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
@@ -75,35 +110,8 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
         uint8_t* out = dst + tile.host;
         const uint32_t words = tile.len >> 4, tail = tile.len & 15u;
         if (tile.npieces == 1) {
-            // the whole tile comes from one segment: one phase, no lookups
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(pc->dev) + (tile.host - pc->host);
-            const uint32_t sh = (uint32_t)((uintptr_t)src & 15u);
-            const uint4* a = reinterpret_cast<const uint4*>(src - sh);
-            uint4* o = reinterpret_cast<uint4*>(out);
-            uint32_t w = threadIdx.x;
-            if (sh == 0) {
-                for (; w + 3 * kStageThreads < words; w += 4 * kStageThreads) {
-                    uint4 v[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) v[i] = __ldg(a + w + i * kStageThreads);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) o[w + i * kStageThreads] = v[i];
-                }
-                for (; w < words; w += kStageThreads) o[w] = __ldg(a + w);
-            } else {
-                for (; w + 3 * kStageThreads < words; w += 4 * kStageThreads) {
-                    uint4 lo[4], hi[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        lo[i] = __ldg(a + w + i * kStageThreads);
-                        hi[i] = __ldg(a + w + i * kStageThreads + 1);
-                    }
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) o[w + i * kStageThreads] = shift_bytes(lo[i], hi[i], sh);
-                }
-                for (; w < words; w += kStageThreads) o[w] = shift_bytes(__ldg(a + w), __ldg(a + w + 1), sh);
-            }
-            if (threadIdx.x < tail) out[(uint64_t)words * 16 + threadIdx.x] = src[(uint64_t)words * 16 + threadIdx.x];
+            // the whole tile comes from one segment
+            stage_one_piece(reinterpret_cast<const uint8_t*>(pc->dev) + (tile.host - pc->host), out, words, tail);
             continue;
         }
         uint32_t cur = 0;
@@ -495,6 +503,114 @@ __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
     }
 }
 
+// ---- ranges of files whose segments may change type on the way out (b200h_copy_cast_ranges, and the gather of
+//      b200h_hash_cast_segment_parts_device)
+//
+//   stage_cast_ranges_kernel   stage_ranges_kernel's tiles and destination words over CastPieces.  A converting
+//                        piece's image is its source elements converted, element k at image byte k * ds; a range may
+//                        start at any image byte, so a piece records the element that holds its first byte and that
+//                        byte's place in it (`phase`).
+//   * a tile that lies in one piece that converts nothing is stage_ranges_kernel's (stage_one_piece);
+//   * a destination word inside one converting piece whose first byte starts an element takes its 16 / ds * ss source
+//     bytes with aligned 16-byte loads inside the piece's 16-byte hull (two or three narrowing F32, one or two between
+//     F16 and BF16, one widening unless the 8 bytes cross a word), joined with shift_bytes and converted by cast_word;
+//   * a word inside one piece that converts nothing is stage_ranges_kernel's (load_word);
+//   * any other word (across pieces, or holding part of an element) is assembled element by element, one byte at a
+//     time, and still stored as one word;
+//   * only the bytes behind a range's last whole word are stored singly.
+// A single element converts through the paired intrinsics too (the other half of the pair unused), so every path gives
+// the same bits.
+
+// one element of type st (in the low bits of x) as type dt
+__device__ __forceinline__ uint32_t cast_one(uint32_t x, uint32_t st, uint32_t dt) {
+    if (st == kDtF32) return narrow_pair(__uint_as_float(x), 0.f, dt) & 0xffffu;
+    const float2 f = widen_pair(x & 0xffffu, st);
+    return dt == kDtF32 ? __float_as_uint(f.x) : narrow_pair(f.x, 0.f, dt) & 0xffffu;
+}
+
+// byte d (a destination offset inside piece p) of the piece's image
+__device__ __forceinline__ uint32_t image_byte(const CastPiece& p, uint64_t d) {
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(p.r.dev);
+    if (p.src_type == p.dst_type) return s[d - p.r.host];
+    const uint32_t ss = dt_bytes(p.src_type), ds = dt_bytes(p.dst_type);
+    const uint64_t rel = d - p.r.host + p.phase, e = ds == 4 ? rel >> 2 : rel >> 1;
+    const uint32_t x = ss == 4 ? *reinterpret_cast<const uint32_t*>(s + e * 4)
+                               : (uint32_t)*reinterpret_cast<const uint16_t*>(s + e * 2);
+    return (cast_one(x, p.src_type, p.dst_type) >> (8 * (uint32_t)(rel & (ds - 1)))) & 0xffu;
+}
+
+// the destination word at d, byte by byte from pieces pc[i ..] (pc[i] holds d; the word lies in the range)
+__device__ __forceinline__ uint4 image_word(const CastPiece* __restrict__ pc, uint32_t i, uint64_t d) {
+    uint64_t x[2] = {0, 0};
+    uint64_t end = pc[i].r.host + pc[i].r.len;
+#pragma unroll 1
+    for (uint32_t j = 0; j < 16; ++j) {
+        while (d + j >= end) {
+            ++i;
+            end = pc[i].r.host + pc[i].r.len;
+        }
+        const uint64_t b = (uint64_t)image_byte(pc[i], d + j) << (8 * (j & 7));
+        if (j < 8) x[0] |= b;
+        else x[1] |= b;
+    }
+    return make_uint4((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
+}
+
+// the destination word of the 16 / ds elements at s (a multiple of ss), inside one converting piece
+__device__ __forceinline__ uint4 cast_load_word(const uint8_t* s, uint32_t st, uint32_t dt) {
+    const uint32_t sh = (uint32_t)((uintptr_t)s & 15u);
+    const uint4* a = reinterpret_cast<const uint4*>(s - sh);
+    const uint4 w0 = __ldg(a);
+    uint4 lo, hi = make_uint4(0, 0, 0, 0);
+    if (st == kDtF32) {  // 32 source bytes
+        const uint4 w1 = __ldg(a + 1);
+        lo = sh ? shift_bytes(w0, w1, sh) : w0;
+        hi = sh ? shift_bytes(w1, __ldg(a + 2), sh) : w1;
+    } else if (dt != kDtF32) {  // 16
+        lo = sh ? shift_bytes(w0, __ldg(a + 1), sh) : w0;
+    } else {  // 8
+        lo = sh > 8 ? shift_bytes(w0, __ldg(a + 1), sh) : shift_bytes(w0, w0, sh);
+    }
+    return cast_word(lo, hi, st, dt);
+}
+
+__global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
+    stage_cast_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles, const CastPiece* __restrict__ pieces,
+                             uint8_t* __restrict__ dst) {
+    for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const RangeTile tile = tiles[t];
+        const CastPiece* __restrict__ pc = pieces + tile.first_piece;
+        uint8_t* out = dst + tile.host;
+        const uint32_t words = tile.len >> 4, tail = tile.len & 15u;
+        if (tile.npieces == 1 && pc->src_type == pc->dst_type) {
+            stage_one_piece(reinterpret_cast<const uint8_t*>(pc->r.dev) + (tile.host - pc->r.host), out, words, tail);
+            continue;
+        }
+        uint32_t cur = 0;
+        for (uint32_t w = threadIdx.x; w < words; w += kStageThreads) {
+            const uint64_t d = tile.host + (uint64_t)w * 16;
+            if (d >= pc[cur].r.host + pc[cur].r.len) cur = find_piece(pc, cur + 1, tile.npieces, d);
+            const CastPiece p = pc[cur];
+            const uint64_t in = d - p.r.host, left = p.r.len - in;
+            const uint8_t* s = reinterpret_cast<const uint8_t*>(p.r.dev);
+            uint4 v;
+            if (left >= 16 && p.src_type == p.dst_type) {
+                v = load_word(s + in);
+            } else if (left >= 16 && ((in + p.phase) & (dt_bytes(p.dst_type) - 1)) == 0) {
+                const uint64_t e = (in + p.phase) / dt_bytes(p.dst_type);
+                v = cast_load_word(s + e * dt_bytes(p.src_type), p.src_type, p.dst_type);
+            } else {
+                v = image_word(pc, cur, d);
+            }
+            *reinterpret_cast<uint4*>(dst + d) = v;
+        }
+        if (threadIdx.x < tail) {
+            const uint64_t d = tile.host + (uint64_t)words * 16 + threadIdx.x;
+            dst[d] = (uint8_t)image_byte(pc[find_piece(pc, 0, tile.npieces, d)], d);
+        }
+    }
+}
+
 }  // namespace
 
 int launch_load_boxes(const BoxTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
@@ -528,6 +644,15 @@ int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiec
     const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
     stage_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
                                                                                       static_cast<uint8_t*>(dst));
+    return 1;
+}
+
+int launch_stage_cast_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces, void* dst,
+                             cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
+    stage_cast_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
+        tiles, ntiles, pieces, static_cast<uint8_t*>(dst));
     return 1;
 }
 

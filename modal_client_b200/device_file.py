@@ -49,29 +49,37 @@ BOUNCE_BYTES = 16 << 20  # page-locked host memory per DeviceFile (shared by its
 class _TensorBytes:
     """The bytes of an ordered list of contiguous CUDA tensors (the segments), read as one file, plus what reading them
     needs: a side stream ordered after the stream that was current when the DeviceFile was made, a lazily allocated
-    pinned bounce buffer, a lock, a byte counter."""
+    pinned bounce buffer, a lock, a byte counter.
+
+    With ``casts`` -- ``(src_type, dst_type)`` ``_lib.DT_*`` codes per segment, equal (0, 0) for one that converts
+    nothing -- the file is the segments' converted images: segment s contributes its elements as ``dst_type``, and
+    every offset and count (``seg_start``, ``nbytes``, ``bytes_to_host``) is in image bytes.  The converted bytes are
+    made on the way out, by the context ``ctx``, and never held in HBM."""
 
     device_type = "cuda"
 
-    def __init__(self, tensors, bounce_bytes: int):
+    def __init__(self, tensors, bounce_bytes: int, casts=None, ctx=None):
         import torch
 
-        self._attach(tensors, bounce_bytes)
+        self._attach(tensors, bounce_bytes, casts, ctx)
         device = self.segments[0].device
         self.stream = torch.cuda.Stream(device)
         # everything already queued on the caller's stream (the kernels that produced the tensors) runs first
         self.stream.wait_stream(torch.cuda.current_stream(device))
         self.stream_handle = self.stream.cuda_stream
 
-    def _attach(self, tensors, bounce_bytes: int):
+    def _attach(self, tensors, bounce_bytes: int, casts=None, ctx=None):
         """``tensors``: one tensor, or a non-empty list of them in file order."""
         import torch
 
         self.tensors = list(tensors) if isinstance(tensors, (list, tuple)) else [tensors]  # keep the storages alive
         self.segments = [t.reshape(-1).view(torch.uint8) for t in self.tensors]
+        self.casts, self.ctx = casts, ctx
+        size = {_lib.DT_F32: 4, _lib.DT_F16: 2, _lib.DT_BF16: 2}
         self.seg_start = [0]  # file offset of every segment, then the size
-        for s in self.segments:
-            self.seg_start.append(self.seg_start[-1] + s.numel())
+        for i, s in enumerate(self.segments):
+            st, dt = casts[i] if casts else (0, 0)
+            self.seg_start.append(self.seg_start[-1] + (s.numel() // size[st] * size[dt] if st != dt else s.numel()))
         self.nbytes = self.seg_start[-1]
         self.lock = threading.Lock()
         self.bytes_to_host = 0
@@ -168,7 +176,7 @@ class _TensorBytes:
 
     def copy_out(self, pos: int, dst: np.ndarray) -> None:
         """dst[:] = bytes [pos, pos + dst.size) of the file, one bounce buffer at a time (a bounce buffer may be filled
-        from several segments)."""
+        from several segments; with casts, by one ``copy_cast_ranges`` call)."""
         n = int(dst.size)
         with self.lock:
             if self._bounce is None:
@@ -180,6 +188,11 @@ class _TensorBytes:
                 k = min(n - done, self._bounce_bytes)
                 filled = 0
                 with self._on_stream():
+                    if self.casts:
+                        ptrs, lens, first = _file_table([self])
+                        self.ctx.copy_cast_ranges(ptrs, lens, *_types([self]), first, [(0, pos + done, k)], bounce, [0],
+                                                  self.stream_handle)
+                        filled = k
                     while filled < k:
                         at = pos + done + filled
                         while self.seg_start[seg + 1] <= at:  # skips empty segments
@@ -221,8 +234,12 @@ def _hash_sources(sources: list[_TensorBytes], ctx, part_len: int, flags: int):
     n = sum(-(-src.nbytes // part_len) for src in sources)
     with lead._on_stream():
         d_sha, d_md5, d_trim = _outputs(n, flags, lead.segments[0].device)
-        got = ctx.hash_segment_parts_device(ptrs, lens, first, part_len, flags, _ptr(d_sha), _ptr(d_md5), _ptr(d_trim),
-                                            lead.stream_handle)
+        if any(src.casts for src in sources):
+            got = ctx.hash_cast_segment_parts_device(ptrs, lens, *_types(sources), first, part_len, flags, _ptr(d_sha),
+                                                     _ptr(d_md5), _ptr(d_trim), lead.stream_handle)
+        else:
+            got = ctx.hash_segment_parts_device(ptrs, lens, first, part_len, flags, _ptr(d_sha), _ptr(d_md5),
+                                                _ptr(d_trim), lead.stream_handle)
         assert got == n
         return _fetch(d_sha, d_md5, d_trim)
 
@@ -230,7 +247,7 @@ def _hash_sources(sources: list[_TensorBytes], ctx, part_len: int, flags: int):
 def hash_parts_many(files: list["DeviceFile"], part_len: int, flags: int = _lib.SHA256 | _lib.MD5, ctx=None):
     """``DeviceFile.hash_parts`` of several files at once: every file's parts (one or more segments each), file-major,
     digested by ONE ``b200h_hash_segment_parts_device`` call on the first file's stream, which is ordered after every
-    file's stream.  -> (sha uint8[n,32] | None, md5 uint8[n,16] | None, trimmed uint64[n])."""
+    file's stream (``b200h_hash_cast_segment_parts_device`` when any of the files converts its tensors).  -> (sha uint8[n,32] | None, md5 uint8[n,16] | None, trimmed uint64[n])."""
     return _hash_sources([f._src for f in files], ctx or get_context(), part_len, flags)
 
 
@@ -257,7 +274,8 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
     """Copy ``ranges`` -- ``(index into files, offset, length)`` each -- of device files into ``dst``, a uint8 array
     over page-locked memory from ``ctx.host_alloc``; range i lands at ``dst[dst_offsets[i]:]`` (offsets multiples of
     16, destinations disjoint; the layout is the caller's).  ONE ``b200h_copy_ranges_to_host`` call (one kernel launch)
-    whatever the files are made of, enqueued on the first file's stream, which is ordered after every file's stream.
+    whatever the files are made of, enqueued on the first file's stream, which is ordered after every file's stream;
+    ONE ``b200h_copy_cast_ranges`` call instead when any of the files converts its tensors.
     Returns at once; ``wait()`` on the result blocks until the bytes are in ``dst``.  Every file's ``bytes_to_host``
     grows by the bytes of its ranges."""
     ctx = ctx or get_context()
@@ -267,7 +285,10 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
     lead = sources[0]
     ptrs, lens, first = _file_table(sources)
     with lead._on_stream():
-        ctx.copy_ranges_to_host(ptrs, lens, first, ranges, dst, offsets, lead.stream_handle)
+        if any(src.casts for src in sources):
+            ctx.copy_cast_ranges(ptrs, lens, *_types(sources), first, ranges, dst, offsets, lead.stream_handle)
+        else:
+            ctx.copy_ranges_to_host(ptrs, lens, first, ranges, dst, offsets, lead.stream_handle)
         done = lead._mark()
     for f, _, n in ranges:
         with sources[f].lock:
@@ -286,6 +307,13 @@ def _file_table(sources: list[_TensorBytes]):
         lens += [s.numel() for s in src.segments]
         first.append(len(lens))
     return ptrs, lens, first
+
+
+def _types(sources: list[_TensorBytes]):
+    """(src_types, dst_types) of every segment of ``sources``, in ``_file_table`` order ((0, 0): the bytes as they
+    are)."""
+    pairs = [pair for src in sources for pair in (src.casts or [(0, 0)] * len(src.segments))]
+    return [st for st, _ in pairs], [dt for _, dt in pairs]
 
 
 def _range_args(files: list["DeviceFile"], ranges, offsets, offsets_name: str):
@@ -365,6 +393,54 @@ def cast_dtypes() -> dict:
     import torch
 
     return {torch.float32: _lib.DT_F32, torch.float16: _lib.DT_F16, torch.bfloat16: _lib.DT_BF16}
+
+
+def cast_targets(path: str, dtype, entries, data_start: int, sliced: bool = False) -> dict:
+    """{name: target dtype} of the tensors of ``entries`` -- ``(name, dtype, shape, data offset, end)`` each, as
+    ``volume._safetensors_entries`` gives them (the selected ones for ``read_safetensors_slices``; a state dict's tensors
+    for ``DeviceFile.safetensors``) -- that ``dtype`` converts: ``None``; one of float32, float16 and bfloat16 for every
+    F32 / F16 / BF16 tensor of another dtype, integer and bool tensors unchanged; or ``{name: such a dtype}``.  Every
+    problem in one ``ValueError``: another floating dtype under a single dtype, a mapped name that is not there, an
+    unsupported target or source, and a tensor to convert whose file offset (``data_start`` + its data offset) is not a
+    multiple of its element size."""
+    if dtype is None:
+        return {}
+    import torch
+
+    codes, tags = cast_dtypes(), _st_dtypes()
+    by_name = {e[0]: e for e in entries}
+    problems, want = [], {}
+    supported = "float32, float16 or bfloat16"
+    if isinstance(dtype, Mapping):
+        for name, target in dtype.items():
+            if name not in by_name:
+                problems.append(f"{name!r} is in dtype but not {'selected' if sliced else 'in the file'}")
+            else:
+                want[name] = target
+    elif not isinstance(dtype, torch.dtype) or dtype not in codes:
+        problems.append(f"{dtype} is not a supported target ({supported})")
+    else:
+        for name, src, *_ in entries:
+            if src in codes:
+                want[name] = dtype
+            elif tags[src][0][0] in "FC":  # F64, F8_*, F4, C64: floating, but not converted
+                problems.append(f"{name!r} is {tags[src][0]}, which does not convert to {dtype}")
+    out = {}
+    for name, target in want.items():
+        _, src, _, lo, _ = by_name[name]
+        if not isinstance(target, torch.dtype) or target not in codes:
+            problems.append(f"{name!r}: {target} is not a supported target ({supported})")
+        elif src not in codes:
+            problems.append(f"{name!r} is {tags[src][0]}; only F32, F16 and BF16 tensors convert")
+        elif src != target:
+            if (data_start + lo) % src.itemsize:
+                problems.append(f"{name!r} starts at file offset {data_start + lo}, not a multiple of its element size "
+                                f"{src.itemsize}")
+            out[name] = target
+    if problems:
+        raise ValueError(f"{path}: dtype: " + "; ".join(problems))
+    return out
+
 
 
 def load_cast_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> Loaded:
@@ -721,18 +797,54 @@ class DeviceFile(io.RawIOBase):
         self._pos = 0
 
     @classmethod
-    def safetensors(cls, tensors: Mapping, metadata: Mapping | None = None, *, ctx=None,
+    def safetensors(cls, tensors: Mapping, metadata: Mapping | None = None, *, dtype=None, ctx=None,
                     bounce_bytes: int = BOUNCE_BYTES) -> "DeviceFile":
         """A file whose bytes are the safetensors image of ``tensors`` (``safetensors.torch.save(tensors, metadata)``),
         made of the tensors where they are: the header is built on the host and copied to the device once, every tensor
         is one segment of the file.  Tensors must be contiguous, on the context's device, of a dtype safetensors stores;
         zero-size, 0-d and storage-sharing tensors are fine.  The metadata entries keep the mapping's order (the
-        library writes them in no fixed order when there are several)."""
+        library writes them in no fixed order when there are several).
+
+        ``dtype`` exports the tensors in another dtype, as ``volume.read_safetensors(dtype=...)`` reads them: one of
+        torch.float32, float16 and bfloat16 for every F32 / F16 / BF16 tensor (integer and bool tensors unchanged), or
+        ``{name: dtype}``.  The file is then exactly ``safetensors.torch.save({k: v.to(target)}, metadata)``, header
+        dtypes and data order included, but no converted copy is made: the elements are converted on the device as
+        the file's blocks are hashed, staged or read (``b200h_hash_cast_segment_parts_device``,
+        ``b200h_copy_cast_ranges``), so HBM holds only the tensors, the header and the digest tables.  A tensor
+        already in its target dtype is taken as it is.  Every problem (another floating dtype under a single
+        ``dtype``, names not in ``tensors``, unsupported sources or targets) is reported in one ``ValueError`` before
+        anything is copied to the device."""
+        if dtype is not None:
+            safetensors_layout(tensors, metadata)  # the names, metadata and dtypes, checked before the targets
+            targets = cast_targets("DeviceFile.safetensors", dtype,
+                                   [(name, t.dtype, t.shape, 0, None) for name, t in tensors.items()], 0)
+            if targets:
+                return cls._safetensors_cast(tensors, metadata, targets, ctx, bounce_bytes)
         header, ordered = safetensors_layout(tensors, metadata)
         for name, t in ordered:
             ctx = cls._Source._check_tensor(t, ctx, f"DeviceFile.safetensors[{name!r}]")
         head = cls._Source._to_device(header, ctx or get_context())
         return cls._over(cls._Source([head] + [t for _, t in ordered], bounce_bytes))
+
+    @classmethod
+    def _safetensors_cast(cls, tensors: Mapping, metadata, targets: dict, ctx, bounce_bytes: int) -> "DeviceFile":
+        """``safetensors`` with ``{name: target dtype}`` for the tensors that convert: the layout is that of ``meta``
+        stand-ins in the targets, and each converting tensor is a segment of the file that converts."""
+        import torch
+
+        for name, t in tensors.items():
+            ctx = cls._Source._check_tensor(t, ctx, f"DeviceFile.safetensors[{name!r}]")
+        ctx = ctx or get_context()
+        stand_ins = {name: torch.empty(t.shape, dtype=targets[name], device="meta") if name in targets else t
+                     for name, t in tensors.items()}
+        header, ordered = safetensors_layout(stand_ins, metadata)
+        codes = cast_dtypes()
+        segments, casts = [cls._Source._to_device(header, ctx)], [(0, 0)]
+        for name, _ in ordered:
+            t = tensors[name]
+            segments.append(t)
+            casts.append((codes[t.dtype], codes[targets[name]]) if name in targets else (0, 0))
+        return cls._over(cls._Source(segments, bounce_bytes, casts, ctx))
 
     @classmethod
     def torch_save(cls, obj, *, ctx=None, bounce_bytes: int = BOUNCE_BYTES) -> "DeviceFile":

@@ -39,7 +39,7 @@ from . import _wire, blob_utils, device_file
 from ._logging import logger
 from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
-from .device_file import (BOUNCE_BYTES, DeviceFile, _st_dtypes, cast_dtypes, load_boxes, load_cast_boxes, load_ranges,
+from .device_file import (BOUNCE_BYTES, DeviceFile, _st_dtypes, cast_targets, load_boxes, load_cast_boxes, load_ranges,
                           stage_ranges)
 from .exception import ExecutionError, ServiceError
 from .http_utils import ClientSessionRegistry
@@ -662,52 +662,6 @@ def _check_into(into: Mapping, entries, ctx, sliced: bool = False, stored: Mappi
         raise ValueError(f"{what}(into=...): " + "; ".join(problems))
 
 
-def _cast_targets(path: str, dtype, entries, data_start: int, sliced: bool = False) -> dict:
-    """{name: target dtype} of the tensors of ``entries`` (``_safetensors_entries``; the selected ones for
-    ``read_safetensors_slices``) that ``dtype`` converts: ``None``; one of float32, float16 and bfloat16 for every
-    F32 / F16 / BF16 tensor of another dtype, integer and bool tensors unchanged; or ``{name: such a dtype}``.  Every
-    problem in one ``ValueError``: another floating dtype under a single dtype, a mapped name that is not there, an
-    unsupported target or source, and a tensor to convert whose file offset (``data_start`` + its data offset) is not a
-    multiple of its element size."""
-    if dtype is None:
-        return {}
-    import torch
-
-    codes, tags = cast_dtypes(), _st_dtypes()
-    by_name = {e[0]: e for e in entries}
-    problems, want = [], {}
-    supported = "float32, float16 or bfloat16"
-    if isinstance(dtype, Mapping):
-        for name, target in dtype.items():
-            if name not in by_name:
-                problems.append(f"{name!r} is in dtype but not {'selected' if sliced else 'in the file'}")
-            else:
-                want[name] = target
-    elif not isinstance(dtype, torch.dtype) or dtype not in codes:
-        problems.append(f"{dtype} is not a supported target ({supported})")
-    else:
-        for name, src, *_ in entries:
-            if src in codes:
-                want[name] = dtype
-            elif tags[src][0][0] in "FC":  # F64, F8_*, F4, C64: floating, but not converted
-                problems.append(f"{name!r} is {tags[src][0]}, which does not convert to {dtype}")
-    out = {}
-    for name, target in want.items():
-        _, src, _, lo, _ = by_name[name]
-        if not isinstance(target, torch.dtype) or target not in codes:
-            problems.append(f"{name!r}: {target} is not a supported target ({supported})")
-        elif src not in codes:
-            problems.append(f"{name!r} is {tags[src][0]}; only F32, F16 and BF16 tensors convert")
-        elif src != target:
-            if (data_start + lo) % src.itemsize:
-                problems.append(f"{name!r} starts at file offset {data_start + lo}, not a multiple of its element size "
-                                f"{src.itemsize}")
-            out[name] = target
-    if problems:
-        raise ValueError(f"{path}: dtype: " + "; ".join(problems))
-    return out
-
-
 async def _load_runs(client, volume_id: str, path: str, runs, dst: DeviceFile, start: int, end: int,
                      staging_bytes: int) -> None:
     """Load ``runs`` -- ``[((F, W, P, R) as _slice_runs gives it, packed offset in dst, (stored dtype, target dtype) or
@@ -759,14 +713,14 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
 
     ``dtype`` converts tensors as they land, each result equal bit for bit to ``full.to(dtype)`` on the device: a torch
     dtype (float32, float16 or bfloat16) for every F32 / F16 / BF16 tensor, integer and bool tensors unchanged, or
-    ``{name: dtype}`` for the tensors it names.  ``_cast_targets`` lists what it refuses, in one ``ValueError`` before
+    ``{name: dtype}`` for the tensors it names.  ``cast_targets`` lists what it refuses, in one ``ValueError`` before
     any data GET (a file not written by ``safetensors.torch.save`` may hold a tensor that cannot convert in place).
     With ``into=`` each tensor must have its target dtype.  When something converts, the same ``VolumeGetFile2`` call
     and block GETs as without ``dtype`` feed the waves of ``_load_runs``: HBM holds only the results, never the stored
     image; when nothing converts, the call is the one without ``dtype``."""
     ctx = blob_utils.get_context()
     size, n, _, entries = await _read_safetensors_header(client, volume_id, path)
-    targets = _cast_targets(path, dtype, entries, 8 + n)
+    targets = cast_targets(path, dtype, entries, 8 + n)
     if targets and staging_bytes < 2 * blob_utils.BLOCK_SIZE:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), got {staging_bytes}")
     result = [(name, targets.get(name, dt), shape, lo, hi) for name, dt, shape, lo, hi in entries]
@@ -961,7 +915,7 @@ async def read_safetensors_slices(client, volume_id: str, path: str, select: Map
         bounds, kept = _slice_bounds(name, shape, index)
         result = [hi - b for (b, hi), k in zip(bounds, kept) if k]
         plans.append((name, dt, result, _slice_runs(shape, bounds, dt.itemsize, 8 + n + lo)))
-    targets = _cast_targets(path, dtype, [by_name[name] for name in select], 8 + n, sliced=True)
+    targets = cast_targets(path, dtype, [by_name[name] for name in select], 8 + n, sliced=True)
     if into is not None:
         _check_into(into, [(name, targets.get(name, dt), result, 0, 0) for name, dt, result, _ in plans], ctx,
                     sliced=True, stored={name: dt for name, dt, *_ in plans if name in targets})

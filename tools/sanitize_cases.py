@@ -12,6 +12,8 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
   cast boxes   load_cast_boxes_kernel: every conversion between F32, F16 and BF16, boxes that end at the last byte of
                their exact-size destination allocation and of the page-locked source, every element phase, rows that
                cross destination words, 1-element rows
+  cast ranges  stage_cast_ranges_kernel: every conversion, segments that are exact-size allocations, ranges at odd image
+               offsets into page-locked host memory and into device memory
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -138,5 +140,38 @@ for (f, _, w, rows, a, pitch, st, dt), t in zip(boxes, outs):
     assert torch.equal(t, want), (st, dt, w, rows)
 ctx.host_free(src)
 print("cast boxes ok", flush=True)
+
+# 8. stage_cast_ranges_kernel: every conversion, each segment an exact-size allocation (its first and last bytes are
+#    those of the allocation), plain bytes between them, ranges at odd image offsets into host and device memory
+segs, casts, at = [], [], 0
+for st, dt in [(a, b) for a in names for b in names if a != b] + [(0, 0)]:
+    ss, ds = (names[st].itemsize, names[dt].itemsize) if st else (1, 1)
+    if at % ds:
+        segs.append(torch.randint(0, 256, (ds - at % ds,), dtype=torch.uint8, device="cuda"))
+        casts.append((0, 0))
+        at += ds - at % ds
+    n = 4099 * ss if st else 37
+    segs.append(torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda"))
+    casts.append((st, dt))
+    at += n // ss * ds
+image = torch.cat([t.view(names[st]).to(names[dt]).view(torch.uint8) if st else t
+                   for t, (st, dt) in zip(segs, casts)]).cpu().numpy()
+ranges = [(0, 0, image.size), (0, 1, image.size - 2), (0, image.size - 3, 3), (0, 8199, 5000)]
+offsets, at = [], 128
+for _, _, n in ranges:
+    offsets.append(at)
+    at += -(-n // 128) * 128 + 128
+args = ([t.data_ptr() for t in segs], [t.numel() for t in segs], [c[0] for c in casts], [c[1] for c in casts],
+        [0, len(segs)], ranges)
+host = ctx.host_alloc(at)
+dev = torch.empty(at, dtype=torch.uint8, device="cuda")
+for dst in (host, dev):
+    ctx.copy_cast_ranges(*args, dst, offsets, 1)  # after the fills on torch's (legacy) default stream
+    torch.cuda.synchronize()
+    got = dst if dst is host else dst.cpu().numpy()
+    for (_, off, n), o in zip(ranges, offsets):
+        assert np.array_equal(got[o : o + n], image[off : off + n]), (off, n)
+ctx.host_free(host)
+print("cast ranges ok", flush=True)
 ctx.close()
 print("ALL OK")
