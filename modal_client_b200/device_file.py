@@ -28,6 +28,9 @@ buffer into the files' tensors with ONE ``b200h_copy_ranges_from_host`` call (``
 packed into the files with ONE ``b200h_copy_boxes_from_host`` call (``volume.read_safetensors_slices``).
 ``load_cast_boxes(files, boxes, src)`` is ``load_boxes`` whose elements change type on the way (F32, F16, BF16), with
 ONE ``b200h_copy_cast_boxes_from_host`` call (``volume.read_safetensors(..., dtype=...)``).
+
+``safetensors_shards(state_dict, max_shard_size=...)`` is a checkpoint in the Hugging Face Hub's sharded layout: the
+files ``huggingface_hub.save_torch_state_dict`` writes, each shard a ``DeviceFile.safetensors``, plus the index.
 """
 from __future__ import annotations
 
@@ -781,6 +784,117 @@ def torch_save_layout(obj):
     return sk, storages, size, records, compute_crc
 
 
+# ------------------------------------------------------------------------------- sharded safetensors
+#
+# The Hugging Face Hub's sharded layout, as ``huggingface_hub.save_torch_state_dict`` writes it: names that share a
+# storage are reduced to one (``_hub_duplicates``), the rest split greedily in key order on storage sizes
+# (``_hub_split``), every shard a safetensors file with ``{"format": "pt"}`` metadata, and with more than one shard a
+# ``<pattern>.index.json`` that maps every name to its shard.  The rules are restated here (the library is not a
+# dependency); tests/test_safetensors_shards_cpu.py compares the files with the library's.
+
+_SIZE_UNITS = {"TB": 10**12, "GB": 10**9, "MB": 10**6, "KB": 10**3}
+
+
+def parse_size_to_int(size) -> int:
+    """``"5GB"`` -> 5 * 10**9 (units TB, GB, MB, KB, decimal, any case, a fractional value allowed), an int as it is:
+    what the Hub takes as ``max_shard_size``."""
+    if not isinstance(size, str):
+        return size
+    text = size.strip()
+    unit = text[-2:].upper()
+    if unit not in _SIZE_UNITS:
+        raise ValueError(f"Unit '{unit}' not supported. Supported units are TB, GB, MB, KB. Got '{text}'.")
+    try:
+        value = float(text[:-2].strip())
+    except ValueError as exc:
+        raise ValueError(f"Could not parse the size value from '{text}': {exc}") from None
+    return int(value * _SIZE_UNITS[unit])
+
+
+def _hub_duplicates(tensors: Mapping, discard) -> tuple[dict, list]:
+    """({kept name: [removed names]}, [names of every storage no name covers]) of ``tensors``: names whose bytes
+    overlap in one storage form a group, and of the names that cover the whole storage the first by name that is not in
+    ``discard`` is kept (the first by name when all are).  Every tensor is contiguous."""
+    groups: dict = {}
+    for name, t in tensors.items():
+        st = t.untyped_storage()
+        if st.data_ptr() and st.nbytes():
+            groups.setdefault((t.device, st.data_ptr(), st.nbytes()), set()).add(name)
+    shared = []
+    for names in sorted(groups.values()):  # sets sort by inclusion, as the Hub sorts them
+        areas = sorted((tensors[n].data_ptr(), tensors[n].data_ptr() + tensors[n].nbytes, n) for n in names)
+        _, last_stop, first = areas[0]
+        shared.append({first})
+        for lo, hi, n in areas[1:]:
+            if lo >= last_stop:
+                shared.append({n})
+            else:
+                shared[-1].add(n)
+            last_stop = hi
+    remove, uncovered = {}, []
+    discard = set(discard or ())
+    for names in shared:
+        complete = {n for n in names if tensors[n].data_ptr() == tensors[n].untyped_storage().data_ptr() and
+                    tensors[n].nbytes == tensors[n].untyped_storage().nbytes()}
+        if not complete:
+            uncovered.append(sorted(names))
+            continue
+        keep = sorted(complete - discard or complete)[0]
+        for n in sorted(names):
+            if n != keep:
+                remove.setdefault(keep, []).append(n)
+    return remove, uncovered
+
+
+def _hub_split(sizes: Mapping, ids: Mapping, pattern: str, max_size: int) -> tuple[dict, int]:
+    """({file name: [tensor names]} in shard order, total size) of the greedy split: in key order, a name whose storage
+    id was seen joins that storage's shard at no cost; a storage larger than ``max_size`` is a shard of its own; else
+    the current shard is closed when the storage would tip it over ``max_size``."""
+    by_id, shards, current, used, total = {}, [], [], 0, 0
+    for name, size in sizes.items():
+        if ids[name] in by_id:
+            by_id[ids[name]].append(name)
+            continue
+        by_id[ids[name]] = [name]
+        total += size
+        if size > max_size:
+            shards.append([name])
+            continue
+        if used + size > max_size:
+            shards.append(current)
+            current, used = [], 0
+        current.append(name)
+        used += size
+    if current:
+        shards.append(current)
+    for names in by_id.values():
+        for shard in shards:
+            if names[0] in shard:
+                shard += names[1:]
+                break
+    if len(shards) == 1:
+        return {pattern.format(suffix=""): list(sizes)}, total
+    return {pattern.format(suffix=f"-{i + 1:05d}-of-{len(shards):05d}"): shard for i, shard in enumerate(shards)}, total
+
+
+class SafetensorsShards:
+    """The files of a sharded safetensors checkpoint (``DeviceFile.safetensors_shards``): ``files``, {file name:
+    DeviceFile} in shard order, and ``index``, (file name, bytes) of the index, or None for a single file."""
+
+    def __init__(self, files: dict, index):
+        self.files, self.index = files, index
+
+    def put(self, batch, remote_dir) -> None:
+        """Queue every shard and the index under ``remote_dir`` on a volumefs2 ``VolumeUploadContextManager2``: the
+        batch hashes the blocks of every shard in its one device call, and stages them as it stages any DeviceFile."""
+        from pathlib import PurePosixPath
+
+        for name, f in self.files.items():
+            batch.put_file(f, PurePosixPath(remote_dir) / name)
+        if self.index is not None:
+            batch.put_file(io.BytesIO(self.index[1]), PurePosixPath(remote_dir) / self.index[0])
+
+
 class DeviceFile(io.RawIOBase):
     """Read-only, seekable ``BinaryIO`` over the raw bytes of one contiguous CUDA tensor (any dtype), in memory order,
     or (``DeviceFile.safetensors``) over the safetensors image of many.
@@ -845,6 +959,97 @@ class DeviceFile(io.RawIOBase):
             segments.append(t)
             casts.append((codes[t.dtype], codes[targets[name]]) if name in targets else (0, 0))
         return cls._over(cls._Source(segments, bounce_bytes, casts, ctx))
+
+    @classmethod
+    def safetensors_shards(cls, state_dict: Mapping, *, filename_pattern: str = "model{suffix}.safetensors",
+                           max_shard_size="5GB", metadata: Mapping | None = None, dtype=None,
+                           shared_tensors_to_discard=None, ctx=None) -> SafetensorsShards:
+        """A checkpoint in the Hugging Face Hub's sharded layout, made of the tensors where they are: every file's
+        bytes are exactly what ``huggingface_hub.save_torch_state_dict(state_dict, d, filename_pattern=...,
+        max_shard_size=..., metadata=..., shared_tensors_to_discard=...)`` writes into ``d``.
+
+        * Of names that share a storage only one is written, the first by name of those covering the storage that is
+          not in ``shared_tensors_to_discard``; every removed name is recorded in the metadata as ``{removed: kept}``
+          unless ``metadata`` has that key already.
+        * The rest are split in key order: a shard is closed before a storage that would take it over
+          ``max_shard_size`` (an int, or ``"5GB"``, ``"512MB"``, ...; decimal units), and a storage larger than that is a
+          shard of its own.  One shard is ``filename_pattern.format(suffix="")``; n > 1 are named with the suffix
+          ``-0000k-of-0000n`` and come with ``filename_pattern.format(suffix="") + ".index.json"``, ``{"metadata":
+          {"total_size": ..., **metadata}, "weight_map": {name: file}}`` as ``json.dump(..., indent=2)`` writes it.
+        * Every file is a ``DeviceFile.safetensors`` with metadata ``{"format": "pt"}``, plus ``metadata`` when there
+          is a single file (the library writes several entries in no fixed order).
+
+        ``dtype`` is ``DeviceFile.safetensors``'s: the files are then the Hub's of the converted checkpoint -- every
+        storage converted once, so tensors that share one still do, as in ``model.to(dtype).state_dict()`` -- split
+        on the converted sizes, and every shard converts its elements on the device as it is read, never making a
+        converted copy.  Names that share a storage must convert to one dtype.
+
+        Every problem is reported in one ``ValueError`` before anything is copied to the device: a pattern without
+        ``{suffix}``, a bad ``max_shard_size``, non-contiguous tensors (the Hub copies them; this call makes no copies
+        in HBM), storages that no name covers (the Hub refuses them too), and whatever ``DeviceFile.safetensors``
+        refuses."""
+        if not isinstance(state_dict, Mapping):
+            raise ValueError(f"expected a mapping of str -> torch.Tensor, got {type(state_dict).__name__}")
+        problems, valid = [], {}
+        try:
+            if "{suffix}" not in filename_pattern:
+                raise ValueError
+            filename_pattern.format(suffix="")
+        except (ValueError, KeyError, IndexError, TypeError):
+            problems.append(f"filename_pattern {filename_pattern!r} needs exactly one field, {{suffix}}")
+        try:
+            max_size = parse_size_to_int(max_shard_size)
+        except ValueError as exc:
+            problems.append(f"max_shard_size: {exc}")
+        try:
+            safetensors_layout({}, metadata)
+        except ValueError as exc:
+            problems.append(str(exc))
+        for name, t in state_dict.items():
+            try:
+                safetensors_layout({name: t})
+                ctx = cls._Source._check_tensor(t, ctx, f"safetensors_shards[{name!r}]")
+                valid[name] = t
+            except ValueError as exc:
+                problems.append(str(exc))
+        targets = {}
+        if dtype is not None and len(valid) == len(state_dict):
+            try:
+                targets = cast_targets("safetensors_shards", dtype,
+                                       [(name, t.dtype, t.shape, 0, None) for name, t in state_dict.items()], 0)
+            except ValueError as exc:
+                problems.append(str(exc))
+        remove, uncovered = _hub_duplicates(valid, shared_tensors_to_discard)
+        for names in uncovered:
+            problems.append(f"no name covers the whole storage of {', '.join(map(repr, names))}")
+        for keep, gone in remove.items():
+            if len({targets.get(n, valid[n].dtype) for n in [keep] + gone}) > 1:
+                problems.append(f"{', '.join(map(repr, [keep] + gone))} share a storage but convert to different "
+                                f"dtypes")
+        if problems:
+            raise ValueError("safetensors_shards: " + "; ".join(problems))
+        ctx = ctx or get_context()
+        meta = dict(metadata or {})
+        for keep, gone in remove.items():
+            for n in gone:
+                meta.setdefault(n, keep)
+        removed = {n for gone in remove.values() for n in gone}
+        kept = {n: t for n, t in state_dict.items() if n not in removed}
+        sizes = {n: t.untyped_storage().nbytes() // t.element_size() * targets[n].itemsize if n in targets else
+                 t.untyped_storage().nbytes() for n, t in kept.items()}
+        ids = {n: (t.device, t.untyped_storage().data_ptr(), sizes[n]) for n, t in kept.items()}
+        split, total = _hub_split(sizes, ids, filename_pattern, max_size)
+        file_meta = {"format": "pt", **meta} if len(split) == 1 else {"format": "pt"}
+        files = {}
+        for fname, names in split.items():
+            conv = {n: targets[n] for n in names if n in targets}
+            files[fname] = cls.safetensors({n: kept[n] for n in names}, file_meta, dtype=conv or None, ctx=ctx)
+        index = None
+        if len(split) > 1:
+            body = {"metadata": {"total_size": total, **meta},
+                    "weight_map": {n: fname for fname, names in split.items() for n in names}}
+            index = (filename_pattern.format(suffix="") + ".index.json", json.dumps(body, indent=2).encode())
+        return SafetensorsShards(files, index)
 
     @classmethod
     def torch_save(cls, obj, *, ctx=None, bounce_bytes: int = BOUNCE_BYTES) -> "DeviceFile":
@@ -1017,6 +1222,8 @@ class DeviceFile(io.RawIOBase):
         return f"<DeviceFile {self._src.nbytes} bytes in {len(segs)} segments on {segs[0].device}>"
 
 
-__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "Staged", "hash_parts_many", "load_boxes", "load_cast_boxes",
-           "load_ranges",
-           "safetensors_layout", "stage_ranges"]
+safetensors_shards = DeviceFile.safetensors_shards
+
+__all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "SafetensorsShards", "Staged", "hash_parts_many", "load_boxes",
+           "load_cast_boxes", "load_ranges", "parse_size_to_int", "safetensors_layout", "safetensors_shards",
+           "stage_ranges"]

@@ -19,7 +19,9 @@ The way back (counterparts of ``Volume.read_file`` / ``read_file_into_fileobj``,
 of a ``DeviceFile`` (blocks downloaded into page-locked memory, a wave per ``load_ranges`` call), and
 ``read_safetensors``, a safetensors checkpoint back into CUDA tensors without a host copy of the file,
 ``read_safetensors_slices``, slices of its tensors (a tensor-parallel rank's rows or columns) downloading only the blocks
-they touch, and ``read_torch_save``, a torch.save checkpoint back into CUDA storages, its zip CRC-32s checked on the device.
+they touch, ``read_torch_save``, a torch.save checkpoint back into CUDA storages, its zip CRC-32s checked on the device,
+and ``read_safetensors_sharded``, a checkpoint in the Hugging Face Hub's sharded layout (``model.safetensors.index.json``)
+through one wave loop over the blocks of all its shards.
 """
 from __future__ import annotations
 
@@ -544,8 +546,9 @@ async def read_file_into_device(client, volume_id: str, path: str, dst: DeviceFi
 
 async def _load_in_waves(slices, load, staging_bytes: int, concurrency: int | None,
                          progress_cb: Callable[..., Any]) -> None:
-    """Download ``slices`` (``_block_slices``) to the device: every block goes to its own ``BLOCK_SIZE`` slot of a
-    page-locked buffer (``ctx.host_alloc``) of two halves, a wave per half; when a wave is complete,
+    """Download ``slices`` (``_block_slices``, each possibly followed by more fields that ``load`` reads) to the device:
+    every block goes to its own ``BLOCK_SIZE`` slot of a page-locked buffer (``ctx.host_alloc``) of two halves, a wave
+    per half; when a wave is complete,
     ``load(wave, at, buf, ctx)`` -- the wave's slices, their offsets in the buffer, the buffer and the context -- makes
     its one copy (``load_ranges`` or ``load_boxes``) and returns the ``Loaded``.  A half is refilled only after its
     previous copy has read it, so ``load`` may still read the previous wave's slots; every copy has read the buffer
@@ -568,7 +571,7 @@ async def _load_in_waves(slices, load, staging_bytes: int, concurrency: int | No
                 await _fetch_block(url, buf[a : a + m], m, semaphore)
                 progress_cb(advance=m)
 
-            await gather_cancel_on_error(*[fetch(url, m, a) for (url, _, m), a in zip(wave, at)])
+            await gather_cancel_on_error(*[fetch(url, m, a) for (url, _, m, *_), a in zip(wave, at)])
             loaded[half] = load(wave, at, buf, ctx)
     finally:
         for pending in loaded:  # the copies must have read the buffer before it is freed
@@ -662,38 +665,46 @@ def _check_into(into: Mapping, entries, ctx, sliced: bool = False, stored: Mappi
         raise ValueError(f"{what}(into=...): " + "; ".join(problems))
 
 
-async def _load_runs(client, volume_id: str, path: str, runs, dst: DeviceFile, start: int, end: int,
-                     staging_bytes: int) -> None:
-    """Load ``runs`` -- ``[((F, W, P, R) as _slice_runs gives it, packed offset in dst, (stored dtype, target dtype) or
-    None)]`` -- into ``dst``: ONE ``VolumeGetFile2`` call over file bytes [start, end), then exactly the blocks that
-    hold a byte of a run, once each, into the page-locked waves of ``_load_in_waves``.  Each complete wave makes at most
-    one ``load_boxes`` call (the unconverted runs; one also when nothing converts) and at most one ``load_cast_boxes``
-    call: every run is cut into boxes, split where the staging stops being contiguous, at a wave's edge or a skipped
-    block.  A converted run's packed offsets count target bytes."""
+async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
+    """Load ``files`` -- ``(path, runs, dst, start, end)`` each, ``runs`` ``[((F, W, P, R) as _slice_runs gives it,
+    packed offset in dst, (stored dtype, target dtype) or None)]`` -- into their ``dst``: ONE ``VolumeGetFile2`` call per
+    file that has a touched block, over its bytes [start, end), all made concurrently, then exactly the blocks that
+    hold a byte of a run, once each, into the page-locked waves of ONE ``_load_in_waves``, so a wave may hold the blocks
+    of several files.  Each complete wave makes at most one ``load_boxes`` call (the unconverted runs; one also when
+    nothing converts) and at most one ``load_cast_boxes`` call, over every file's ``dst``: every run is cut into boxes,
+    split where the staging stops being contiguous, at a wave's edge, a skipped block or the next file.  A converted
+    run's packed offsets count target bytes."""
     BS = blob_utils.BLOCK_SIZE
-    touched = _touched_blocks([r for r, _, _ in runs], BS)
-    if not touched:
+    touched = [_touched_blocks([r for r, _, _ in runs], BS) for _, runs, _, _, _ in files]
+    live = [files[k] for k, t in enumerate(touched) if t]
+    touched = [t for t in touched if t]
+    if not live:
         return
-    slices = [s for s in await _block_slices(client, volume_id, path, start, end - start)
-              if (start + s[1]) // BS in touched]
+    answers = await gather_cancel_on_error(*[_block_slices(client, volume_id, path, start, end - start)
+                                             for path, _, _, start, end in live])
+    slices = [(url, off, m, i) for i, ((_, _, _, start, _), got) in enumerate(zip(live, answers))
+              for url, off, m in got if (start + off) // BS in touched[i]]
+    dsts = [dst for _, _, dst, _, _ in live]
 
     def load(wave, at, buf, ctx):
         plain, cast, k = [], [], 0
-        while k < len(wave):  # a stretch: blocks adjacent in the file and in the buffer
-            e = k + 1
-            while e < len(wave) and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and at[e] == at[e - 1] + wave[e - 1][2]:
+        while k < len(wave):  # a stretch: blocks of one file, adjacent in the file and in the buffer
+            e, i = k + 1, wave[k][3]
+            while e < len(wave) and wave[e][3] == i and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and \
+                    at[e] == at[e - 1] + wave[e - 1][2]:
                 e += 1
+            _, runs, _, start, _ = live[i]
             s0, s1 = start + wave[k][1], start + wave[e - 1][1] + wave[e - 1][2]
             for run, d, conv in runs:
                 for b in _clip_run(run, 0, s0, s1, at[k]):
                     if conv is None:
-                        plain.append((0, d + b[0], *b[1:]))
+                        plain.append((i, d + b[0], *b[1:]))
                     else:  # the box's offset in the run, in source bytes, to target bytes
-                        cast.append((0, d + b[0] // conv[0].itemsize * conv[1].itemsize, *b[1:], *conv))
+                        cast.append((i, d + b[0] // conv[0].itemsize * conv[1].itemsize, *b[1:], *conv))
             k = e
-        loaded = load_boxes([dst], plain, buf, ctx=ctx) if plain or not cast else None
+        loaded = load_boxes(dsts, plain, buf, ctx=ctx) if plain or not cast else None
         if cast:  # on the same stream as the plain boxes: its completion implies theirs
-            loaded = load_cast_boxes([dst], cast, buf, ctx=ctx)
+            loaded = load_cast_boxes(dsts, cast, buf, ctx=ctx)
         return loaded
 
     await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
@@ -739,7 +750,7 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
                 if hi > lo:
                     runs.append(((8 + n + lo, hi - lo, hi - lo, 1), dest, (dt, t.dtype) if name in targets else None))
                 dest += t.numel() * t.element_size()
-            await _load_runs(client, volume_id, path, runs, dst, 8 + n, size, staging_bytes)
+            await _load_runs(client, volume_id, [(path, runs, dst, 8 + n, size)], staging_bytes)
     return {name: t for (name, *_), t in zip(entries, tensors)}
 
 
@@ -933,8 +944,126 @@ async def read_safetensors_slices(client, volume_id: str, path: str, select: Map
         first = min(_touched_blocks([r for r, _, _ in runs], BS)) * BS
         end = max(F + (R - 1) * P + W for (F, W, P, R), _, _ in runs)
         dst = DeviceFile._over(DeviceFile._Source(tensors, BOUNCE_BYTES))
-        await _load_runs(client, volume_id, path, runs, dst, first, end, staging_bytes)
+        await _load_runs(client, volume_id, [(path, runs, dst, first, end)], staging_bytes)
     return {name: t for (name, *_), t in zip(plans, tensors)}
+
+
+async def _read_index(client, volume_id: str, index_path: str):
+    """(index metadata or None, [(shard path, header length, entries)] in shard order) of the sharded safetensors
+    checkpoint whose ``model.safetensors.index.json`` is at ``index_path``: the index through host memory (one
+    ``VolumeGetFile2`` call), then every shard's header concurrently (three each, as ``read_safetensors`` reads one).
+    The shards are the index's file names, sorted, each relative to the index's directory; every disagreement between
+    ``weight_map`` and the shards' headers is listed in one ``ValueError`` before any data GET."""
+    raw = b"".join([body async for body in read_file(client, volume_id, index_path)])
+    try:
+        index = json.loads(raw.decode("utf-8"))
+    except (UnicodeDecodeError, ValueError) as exc:
+        raise ValueError(f"{index_path} is not a valid JSON index: {exc}") from None
+    weight_map = index.get("weight_map") if isinstance(index, dict) else None
+    if not isinstance(weight_map, dict) or not all(isinstance(v, str) for v in weight_map.values()):
+        raise ValueError(f"{index_path}: the index needs a weight_map of tensor name -> shard file name")
+    names = sorted(set(weight_map.values()))
+    bad = [f for f in names if not f or PurePosixPath(f).is_absolute() or ".." in PurePosixPath(f).parts]
+    if bad:
+        raise ValueError(f"{index_path}: shard names must be relative to the index's directory without '..': "
+                         f"{', '.join(map(repr, bad))}")
+    base = PurePosixPath(index_path).parent
+    paths = [(base / f).as_posix() for f in names]
+    headers = await gather_cancel_on_error(*[_read_safetensors_header(client, volume_id, p) for p in paths])
+    problems, holder = [], {}
+    for f, (_, _, _, entries) in zip(names, headers):
+        held = {e[0] for e in entries}
+        for name in held:
+            if name in holder:
+                problems.append(f"{name!r} is in both {holder[name]} and {f}")
+            holder.setdefault(name, f)
+            if name not in weight_map:
+                problems.append(f"{f} holds {name!r}, which weight_map does not name")
+            elif weight_map[name] != f:
+                problems.append(f"{f} holds {name!r}, which weight_map maps to {weight_map[name]}")
+    held_by = {f: {e[0] for e in h[3]} for f, h in zip(names, headers)}
+    for name, f in weight_map.items():
+        if name not in held_by[f]:
+            problems.append(f"weight_map maps {name!r} to {f}, which does not hold it")
+    if problems:
+        raise ValueError(f"{index_path}: " + "; ".join(sorted(problems)))
+    metadata = index.get("metadata")
+    return metadata, [(p, n, entries) for p, (_, n, _, entries) in zip(paths, headers)]
+
+
+async def read_safetensors_index(client, volume_id: str, index_path: str):
+    """(the index's ``metadata``, {name: (shard path, torch dtype, shape tuple)} in shard order, then data order) of
+    the sharded safetensors checkpoint whose index (``model.safetensors.index.json``) is at ``index_path``: the index
+    through host memory, then every shard's header, concurrently.  Shard names are resolved against the index's
+    directory; absolute names and names with ``..`` are refused.  A name of ``weight_map`` that its shard does not hold,
+    a tensor a shard holds that ``weight_map`` maps elsewhere (or not at all), and a name two shards hold are all
+    reported in one ``ValueError``, before any data GET."""
+    metadata, shards = await _read_index(client, volume_id, index_path)
+    return metadata, {name: (path, dtype, tuple(shape)) for path, _, entries in shards
+                      for name, dtype, shape, _, _ in entries}
+
+
+async def read_safetensors_sharded(client, volume_id: str, index_path: str, *, select: Mapping | None = None,
+                                   into: Mapping | None = None, dtype=None, staging_bytes: int = 256 << 20) -> dict:
+    """A sharded safetensors checkpoint (the index at ``index_path``, read as ``read_safetensors_index`` reads it) as
+    ``{name: tensor}`` on the context's device: what merging ``read_safetensors`` over every shard returns, keys in
+    shard order, then data order.  With ``select={name: index}`` it is what ``read_safetensors_slices`` returns for
+    those names instead, in ``select``'s order.  ``into=`` and ``dtype=`` mean what they mean there, with the same
+    messages, every problem in one ``ValueError`` before any data GET.
+
+    Every shard's data comes through one wave loop: ONE ``VolumeGetFile2`` call per shard with a touched byte, all
+    made concurrently, then every touched block once (untouched blocks of a selection never), the blocks of all shards
+    in one sequence of page-locked waves (``staging_bytes`` as in ``read_file_into_device``), so a wave may hold blocks
+    of several shards and the pipeline does not drain between shards.  Each complete wave makes at most one
+    ``load_boxes`` and one ``load_cast_boxes`` call, over a ``DeviceFile`` per shard.  Of HBM, the call allocates only
+    the results and the copies' small tables.  Ordering and partial content on return and on error are as for
+    ``read_safetensors``."""
+    BS = blob_utils.BLOCK_SIZE
+    if staging_bytes < 2 * BS:
+        raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
+    ctx = blob_utils.get_context()
+    _, shards = await _read_index(client, volume_id, index_path)
+    by_name = {e[0]: (k, 8 + n + e[3], e) for k, (_, n, entries) in enumerate(shards) for e in entries}
+    plans = []  # (shard, name, stored dtype, result shape, runs)
+    if select is None:
+        for name, (k, at, (_, dt, shape, lo, hi)) in by_name.items():
+            plans.append((k, name, dt, shape, [(at, hi - lo, hi - lo, 1)] if hi > lo else []))
+    else:
+        unknown = [name for name in select if name not in by_name]
+        if unknown:
+            raise ValueError(f"{index_path}: no tensors named {', '.join(repr(u) for u in unknown)}")
+        for name, index in select.items():
+            k, at, (_, dt, shape, _, _) = by_name[name]
+            bounds, kept = _slice_bounds(name, shape, index)
+            result = [hi - b for (b, hi), keep in zip(bounds, kept) if keep]
+            plans.append((k, name, dt, result, _slice_runs(shape, bounds, dt.itemsize, at)))
+    sliced = select is not None
+    targets = cast_targets(index_path, dtype, [(name, dt, shape, by_name[name][1], None)
+                                               for _, name, dt, shape, _ in plans], 0, sliced=sliced)
+    if into is not None:
+        _check_into(into, [(name, targets.get(name, dt), shape, 0, 0) for _, name, dt, shape, _ in plans], ctx,
+                    sliced=sliced, stored={name: dt for _, name, dt, *_ in plans if name in targets})
+        tensors = [into[name] for _, name, *_ in plans]
+    else:
+        tensors = [DeviceFile._Source._new_tensor(shape, targets.get(name, dt), ctx) for _, name, dt, shape, _ in plans]
+    per = {}  # shard -> [its result tensors, runs, packed bytes so far]
+    for (k, name, dt, _, rs), t in zip(plans, tensors):
+        ts, runs, base = per.setdefault(k, [[], [], 0])
+        dest, conv = base, (dt, t.dtype) if name in targets else None
+        for run in rs:
+            runs.append((run, dest, conv))
+            dest += run[1] * run[3] // dt.itemsize * t.element_size()
+        ts.append(t)
+        per[k][2] = base + t.numel() * t.element_size()
+    files = []
+    for k in sorted(per):
+        ts, runs, _ = per[k]
+        if runs:
+            start = min(F for (F, _, _, _), _, _ in runs)
+            end = max(F + (R - 1) * P + W for (F, W, P, R), _, _ in runs)
+            files.append((shards[k][0], runs, DeviceFile._over(DeviceFile._Source(ts, BOUNCE_BYTES)), start, end))
+    await _load_runs(client, volume_id, files, staging_bytes)
+    return {name: t for (_, name, *_), t in zip(plans, tensors)}
 
 
 _ZIP_TAIL = 1 << 16  # the end of a torch.save file read first: its end records and, usually, its central directory
