@@ -314,7 +314,7 @@ typedef struct b200h_cast_segment {
  * source element size, and its image offset in its file a multiple of the destination element size (every file written
  * by safetensors.torch.save meets this).  dst is 16-byte aligned page-locked host memory the device can reach, or
  * memory of ctx's device (cudaPointerGetAttributes).
- * ONE kernel launch (stage_cast_ranges_kernel) per call, none when every range is empty; its tables live in a
+ * ONE kernel launch (stage_ranges_kernel) per call, none when every range is empty; its tables live in a
  * stream-ordered allocation, so the call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream).  Every
  * store is a full aligned 16-byte word except the bytes behind a range's last whole word; bytes of dst outside the
  * destinations are not written.
@@ -327,7 +327,7 @@ int b200h_copy_cast_ranges(b200h_ctx* ctx, const b200h_cast_segment* segs, uint6
 /* b200h_hash_segment_parts_device over files made of cast segments (the rules of b200h_copy_cast_ranges for them): the
  * parts are cut from the converted images, with the same rows, flags, outputs and synchronisation rules.  A part is
  * hashed in place only when it lies in one segment that converts nothing; every other part is gathered into a wave
- * slot by stage_cast_ranges_kernel (one launch per wave), so the converted bytes never exist in HBM outside the wave
+ * slot by stage_ranges_kernel (one launch per wave), so the converted bytes never exist in HBM outside the wave
  * slots.  b200h_cast_segment_parts_preview shows the split. */
 int b200h_hash_cast_segment_parts_device(b200h_ctx* ctx, const b200h_cast_segment* segs, uint64_t nsegs,
                                          const uint64_t* file_first_seg, uint64_t nfiles, uint64_t part_len,

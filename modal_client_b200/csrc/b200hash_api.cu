@@ -1041,7 +1041,7 @@ static void range_tables(const FileTable& t, const b200h_segment* segs, const b2
 // b200h_hash_segment_parts_device with ctx->mu held, on stream `st`.  d_etag_msg != NULL (b200h_hash_fixed_parts_device):
 // two more words, the ETag message {0, nparts * 16}, ride the part-table upload, even when there are no parts, and
 // *d_etag_msg points at them.  With `casts` (b200h_hash_cast_segment_parts_device; segs is then NULL), the files are
-// the cast segments' images, and the parts that are not hashed in place are gathered by stage_cast_ranges_kernel.
+// the cast segments' images, and the parts that are not hashed in place are gathered by stage_ranges_kernel.
 int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
                               uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
                               uint64_t* d_trimmed_len, uint64_t* nparts_out, cudaStream_t st, const uint64_t** d_etag_msg,
@@ -1083,7 +1083,7 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     if (d_etag_msg) table.insert(table.end(), {0, nparts * 16});
     std::vector<uint64_t> wave_tiles(nwaves + 1, 0);  // tiles of wave w: [wave_tiles[w], wave_tiles[w + 1])
     std::vector<GatherTile> tiles;
-    // with casts: the tables of every wave's stage_cast_ranges_kernel launch (destination offsets in the wave's slot)
+    // with casts: the tables of every wave's stage_ranges_kernel launch (destination offsets in the wave's slot)
     std::vector<std::vector<CastPiece>> cast_pieces(casts ? nwaves : 0);
     std::vector<std::vector<RangeTile>> cast_tiles(casts ? nwaves : 0);
     for (size_t w = 0; w < nwaves; ++w) {
@@ -1130,8 +1130,8 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
             if (casts) {
                 if (int rc = launch_with_tables(ctx, st, cast_tiles[w], cast_pieces[w],
                                                 [&](const RangeTile* d_ct, const CastPiece* d_cp) {
-                                                    return launch_stage_cast_ranges(d_ct, cast_tiles[w].size(), d_cp,
-                                                                                    ctx->dwave[slot], st);
+                                                    return launch_stage_ranges(d_ct, cast_tiles[w].size(), d_cp,
+                                                                               ctx->dwave[slot], st);
                                                 }))
                     return rc;
             } else {
@@ -1639,24 +1639,22 @@ static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, 
         range_of.resize(pieces.size(), i);
     }
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
-    if (casts)
+    if (to_host)
         return launch_with_tables(ctx, st, tiles, pieces, [&](const RangeTile* d_tiles, const CastPiece* d_pieces) {
-            return launch_stage_cast_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
+            return launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
         });
     std::vector<RangePiece> bytes(pieces.size());
     for (size_t k = 0; k < pieces.size(); ++k) bytes[k] = pieces[k].r;
-    if (!to_host) {  // no device byte may be written twice: two files, or two segments of one file, may share a tensor
-        std::vector<size_t> by_dev(bytes.size());
-        for (size_t k = 0; k < by_dev.size(); ++k) by_dev[k] = k;
-        std::sort(by_dev.begin(), by_dev.end(), [&](size_t a, size_t b) { return bytes[a].dev < bytes[b].dev; });
-        for (size_t k = 1; k < by_dev.size(); ++k)
-            if (bytes[by_dev[k - 1]].dev + bytes[by_dev[k - 1]].len > bytes[by_dev[k]].dev)
-                return fail(ctx, B200H_E_INVALID, "ranges " + std::to_string(range_of[by_dev[k - 1]]) + " and " +
-                                                      std::to_string(range_of[by_dev[k]]) + " write the same device bytes");
-    }
+    // no device byte may be written twice: two files, or two segments of one file, may share a tensor
+    std::vector<size_t> by_dev(bytes.size());
+    for (size_t k = 0; k < by_dev.size(); ++k) by_dev[k] = k;
+    std::sort(by_dev.begin(), by_dev.end(), [&](size_t a, size_t b) { return bytes[a].dev < bytes[b].dev; });
+    for (size_t k = 1; k < by_dev.size(); ++k)
+        if (bytes[by_dev[k - 1]].dev + bytes[by_dev[k - 1]].len > bytes[by_dev[k]].dev)
+            return fail(ctx, B200H_E_INVALID, "ranges " + std::to_string(range_of[by_dev[k - 1]]) + " and " +
+                                                  std::to_string(range_of[by_dev[k]]) + " write the same device bytes");
     return launch_with_tables(ctx, st, tiles, bytes, [&](const RangeTile* d_tiles, const RangePiece* d_pieces) {
-        return to_host ? launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_host, st)
-                       : launch_load_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
+        return launch_load_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
     });
 }
 

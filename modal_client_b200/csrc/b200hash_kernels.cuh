@@ -104,10 +104,11 @@ int launch_crc32(const CrcRange* ranges, const uint64_t* first, uint64_t n, uint
 // (host arithmetic on CRC values; no data involved)
 uint32_t crc32_length_term(uint64_t len);
 
-// Ranges of segmented device files copied to or from one host buffer (b200hash_stage.cu).  A piece is the part of a
-// range that lies in one segment (len > 0); the pieces of a range are listed in file order and cover its bytes of the
-// host buffer without gaps.  A tile is up to kStageTileBytes of one range's bytes of the host buffer, starting at a
-// multiple of 16; it uses pieces [first_piece, first_piece + npieces), every piece that holds one of its bytes.
+// Ranges of segmented device files copied to or from one host buffer (b200hash_stage.cu; a copy out of the device may
+// also go to a device buffer, which `host` offsets then count in).  A piece is the part of a range that lies in one
+// segment (len > 0); the pieces of a range are listed in file order and cover its bytes of the host buffer without
+// gaps.  A tile is up to kStageTileBytes of one range's bytes of the host buffer, starting at a multiple of 16; it uses
+// pieces [first_piece, first_piece + npieces), every piece that holds one of its bytes.
 struct RangePiece {
     uint64_t dev, host, len;  // device address; byte offset in the host buffer
 };
@@ -117,12 +118,10 @@ struct RangeTile {
     uint64_t first_piece;
 };
 constexpr uint64_t kStageTileBytes = 64 << 10;
-// Every tile's copy device -> host, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the device
-// can store to.
-int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, void* dst, cudaStream_t st);
-// The inverse, host -> device; `src` is 16-byte aligned memory the device can load from.
+// Every tile's copy host -> device, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device
+// can load from.
 int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
-// A piece of a range whose segment may convert its elements on the way out (stage_cast_ranges_kernel).  src_type ==
+// A piece of a range copied out of the device, whose segment may convert its elements on the way.  src_type ==
 // dst_type: `r` as in RangePiece, the bytes as they are, phase 0.  Otherwise the piece's bytes are its segment's image
 // (the source elements converted, the B200H_DT_* codes of b200hash.h): r.dev is the source address of the element that
 // holds the piece's first image byte, which is byte `phase` of that element's converted value; r.host and r.len count
@@ -133,8 +132,7 @@ struct CastPiece {
 };
 // Every tile's copy of the pieces' images, in one launch (none when ntiles == 0); `dst` is 16-byte aligned memory the
 // device can store to (page-locked host memory or device memory).
-int launch_stage_cast_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces, void* dst,
-                             cudaStream_t st);
+int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces, void* dst, cudaStream_t st);
 
 // Boxes of a host buffer copied into segmented device files (load_boxes_kernel, b200hash_stage.cu).  A box is `rows`
 // rows of `width` bytes, row r at byte src + r * pitch of the host buffer, packed into one destination run.  Its source

@@ -9,12 +9,15 @@
 //                        phases differ almost always (safetensors data starts at 8 + header length, a torch.save
 //                        storage where the zip puts it, and a block made of several tensors changes phase at every
 //                        tensor edge), so a copy at the widest access on which both sides agree, as
-//                        gather_segments_kernel does between HBM buffers, would degrade to byte stores here.
+//                        gather_segments_kernel does between HBM buffers, would degrade to byte stores here.  The
+//                        kernel is at the end of the file: its pieces may also convert elements, with the conversion
+//                        helpers of load_cast_boxes_kernel.
 //
 // A range is cut by the host into pieces (range intersected with one segment, never empty), listed in destination
 // order; a tile names the slice of the piece list it draws from.
-//   * a destination word that lies inside one piece is built from the two aligned 16-byte source words around it and a
-//     byte shift by (source address & 15): one load when the phases agree, two otherwise;
+//   * a tile that lies in one piece that converts nothing is copied with no lookups (stage_one_piece);
+//   * a destination word that lies inside one such piece is built from the two aligned 16-byte source words around it
+//     and a byte shift by (source address & 15): one load when the phases agree, two otherwise;
 //   * a word that crosses pieces is assembled byte by byte and still stored as one word;
 //   * only the bytes behind a range's last whole word are stored singly (the destination beyond the range is not the
 //     kernel's to write).
@@ -55,16 +58,12 @@ __device__ __forceinline__ uint4 load_word(const uint8_t* src) {
     return sh ? shift_bytes(lo, __ldg(a + 1), sh) : lo;
 }
 
-__device__ __forceinline__ const RangePiece& range_of(const RangePiece& p) { return p; }
-__device__ __forceinline__ const RangePiece& range_of(const CastPiece& p) { return p.r; }
-
 // the piece of pc[lo .. n) that holds destination offset d (the pieces of a range tile its destination without gaps)
-template <class Piece>
-__device__ __forceinline__ uint32_t find_piece(const Piece* __restrict__ pc, uint32_t lo, uint32_t n, uint64_t d) {
+__device__ __forceinline__ uint32_t find_piece(const CastPiece* __restrict__ pc, uint32_t lo, uint32_t n, uint64_t d) {
     uint32_t hi = n - 1;
     while (lo < hi) {
         const uint32_t mid = (lo + hi + 1) >> 1;
-        if (range_of(pc[mid]).host <= d) lo = mid;
+        if (pc[mid].r.host <= d) lo = mid;
         else hi = mid - 1;
     }
     return lo;
@@ -99,51 +98,6 @@ __device__ __forceinline__ void stage_one_piece(const uint8_t* src, uint8_t* out
         for (; w < words; w += kStageThreads) o[w] = shift_bytes(__ldg(a + w), __ldg(a + w + 1), sh);
     }
     if (threadIdx.x < tail) out[(uint64_t)words * 16 + threadIdx.x] = src[(uint64_t)words * 16 + threadIdx.x];
-}
-
-__global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
-    stage_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
-                        uint8_t* __restrict__ dst) {
-    for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const RangeTile tile = tiles[t];
-        const RangePiece* __restrict__ pc = pieces + tile.first_piece;
-        uint8_t* out = dst + tile.host;
-        const uint32_t words = tile.len >> 4, tail = tile.len & 15u;
-        if (tile.npieces == 1) {
-            // the whole tile comes from one segment
-            stage_one_piece(reinterpret_cast<const uint8_t*>(pc->dev) + (tile.host - pc->host), out, words, tail);
-            continue;
-        }
-        uint32_t cur = 0;
-        for (uint32_t w = threadIdx.x; w < words; w += kStageThreads) {
-            const uint64_t d = tile.host + (uint64_t)w * 16;
-            if (d >= pc[cur].host + pc[cur].len) cur = find_piece(pc, cur + 1, tile.npieces, d);
-            const uint64_t in = d - pc[cur].host, left = pc[cur].len - in;
-            uint4 v;
-            if (left >= 16) {
-                v = load_word(reinterpret_cast<const uint8_t*>(pc[cur].dev) + in);
-            } else {
-                uint32_t r[4] = {0, 0, 0, 0};
-                uint32_t i = cur;
-                uint64_t end = pc[i].host + pc[i].len;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    while (d + j >= end) {
-                        ++i;
-                        end = pc[i].host + pc[i].len;
-                    }
-                    r[j >> 2] |= (uint32_t)reinterpret_cast<const uint8_t*>(pc[i].dev)[d + j - pc[i].host] << (8 * (j & 3));
-                }
-                v = make_uint4(r[0], r[1], r[2], r[3]);
-            }
-            *reinterpret_cast<uint4*>(dst + d) = v;
-        }
-        if (threadIdx.x < tail) {
-            const uint64_t d = tile.host + (uint64_t)words * 16 + threadIdx.x;
-            const uint32_t i = find_piece(pc, 0, tile.npieces, d);
-            dst[d] = reinterpret_cast<const uint8_t*>(pc[i].dev)[d - pc[i].host];
-        }
-    }
 }
 
 // ---- the inverse direction: page-locked host memory -> segmented device files
@@ -503,21 +457,16 @@ __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
     }
 }
 
-// ---- ranges of files whose segments may change type on the way out (b200h_copy_cast_ranges, and the gather of
-//      b200h_hash_cast_segment_parts_device)
+// ---- stage_ranges_kernel, whose pieces may change type on the way out (b200h_copy_cast_ranges, and the wave-slot
+//      gather of b200h_hash_cast_segment_parts_device)
 //
-//   stage_cast_ranges_kernel   stage_ranges_kernel's tiles and destination words over CastPieces.  A converting
-//                        piece's image is its source elements converted, element k at image byte k * ds; a range may
-//                        start at any image byte, so a piece records the element that holds its first byte and that
-//                        byte's place in it (`phase`).
-//   * a tile that lies in one piece that converts nothing is stage_ranges_kernel's (stage_one_piece);
+// A converting piece's image is its source elements converted, element k at image byte k * ds; a range may start at
+// any image byte, so a piece records the element that holds its first byte and that byte's place in it (`phase`).
 //   * a destination word inside one converting piece whose first byte starts an element takes its 16 / ds * ss source
 //     bytes with aligned 16-byte loads inside the piece's 16-byte hull (two or three narrowing F32, one or two between
 //     F16 and BF16, one widening unless the 8 bytes cross a word), joined with shift_bytes and converted by cast_word;
-//   * a word inside one piece that converts nothing is stage_ranges_kernel's (load_word);
-//   * any other word (across pieces, or holding part of an element) is assembled element by element, one byte at a
-//     time, and still stored as one word;
-//   * only the bytes behind a range's last whole word are stored singly.
+//   * any other word that is not inside one piece that converts nothing (across pieces, or holding part of an element)
+//     is assembled element by element, one byte at a time, and still stored as one word.
 // A single element converts through the paired intrinsics too (the other half of the pair unused), so every path gives
 // the same bits.
 
@@ -575,8 +524,8 @@ __device__ __forceinline__ uint4 cast_load_word(const uint8_t* s, uint32_t st, u
 }
 
 __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
-    stage_cast_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles, const CastPiece* __restrict__ pieces,
-                             uint8_t* __restrict__ dst) {
+    stage_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles, const CastPiece* __restrict__ pieces,
+                        uint8_t* __restrict__ dst) {
     for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
         const RangeTile tile = tiles[t];
         const CastPiece* __restrict__ pc = pieces + tile.first_piece;
@@ -639,20 +588,11 @@ int launch_load_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece
     return 1;
 }
 
-int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const RangePiece* pieces, void* dst, cudaStream_t st) {
+int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces, void* dst, cudaStream_t st) {
     if (!ntiles) return 0;
     const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
     stage_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
                                                                                       static_cast<uint8_t*>(dst));
-    return 1;
-}
-
-int launch_stage_cast_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces, void* dst,
-                             cudaStream_t st) {
-    if (!ntiles) return 0;
-    const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
-    stage_cast_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
-        tiles, ntiles, pieces, static_cast<uint8_t*>(dst));
     return 1;
 }
 

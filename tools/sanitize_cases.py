@@ -6,14 +6,16 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
   trim kernels probe + wide scan (atomicMax across CTAs, work counter), blank and half-blank blocks
   dedupe       hash-table insert/resolve with CAS
   streams      absorb/digest on a private CUDA stream
-  stage        ranges of segmented device files into page-locked host memory: every source phase, segments that start
-               at the first and end at the last byte of their allocation (the aligned-hull loads), ranges across tiny
-               and empty segments, partial last words
+  stage        stage_ranges_kernel: ranges of segmented device files into page-locked host memory: every source
+               phase, segments that start at the first and end at the last byte of their allocation (the aligned-hull
+               loads), ranges across tiny and empty segments, partial last words
   cast boxes   load_cast_boxes_kernel: every conversion between F32, F16 and BF16, boxes that end at the last byte of
                their exact-size destination allocation and of the page-locked source, every element phase, rows that
                cross destination words, 1-element rows
-  cast ranges  stage_cast_ranges_kernel: every conversion, segments that are exact-size allocations, ranges at odd image
-               offsets into page-locked host memory and into device memory
+  cast ranges  stage_ranges_kernel with converting pieces: every conversion, segments that are exact-size allocations,
+               ranges at odd image offsets into page-locked host memory and into device memory
+  gather       gather_segments_kernel (b200h_hash_segment_parts_device): segments that are exact-size allocations,
+               parts that straddle them at every relative phase, and parts hashed in place
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -141,8 +143,9 @@ for (f, _, w, rows, a, pitch, st, dt), t in zip(boxes, outs):
 ctx.host_free(src)
 print("cast boxes ok", flush=True)
 
-# 8. stage_cast_ranges_kernel: every conversion, each segment an exact-size allocation (its first and last bytes are
-#    those of the allocation), plain bytes between them, ranges at odd image offsets into host and device memory
+# 8. stage_ranges_kernel with converting pieces: every conversion, each segment an exact-size allocation (its first
+#    and last bytes are those of the allocation), plain bytes between them, ranges at odd image offsets into host and
+#    device memory
 segs, casts, at = [], [], 0
 for st, dt in [(a, b) for a in names for b in names if a != b] + [(0, 0)]:
     ss, ds = (names[st].itemsize, names[dt].itemsize) if st else (1, 1)
@@ -173,5 +176,28 @@ for dst in (host, dev):
         assert np.array_equal(got[o : o + n], image[off : off + n]), (off, n)
 ctx.host_free(host)
 print("cast ranges ok", flush=True)
+
+# 9. gather_segments_kernel (b200h_hash_segment_parts_device): each segment an exact-size allocation, parts that
+#    straddle segments at every relative phase of source and wave slot, and parts hashed in place in the long segments
+sizes = [1, 15, 16, 17, 0, 33, 255, 4097, 70_001, 3, 5000, 64, 9] + [1 + i * 37 % 97 for i in range(48)]
+files = [[torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda") for n in f] for f in (sizes, sizes[::-1])]
+segs = [t for f in files for t in f]
+images = [b"".join(t.cpu().numpy().tobytes() for t in f) for f in files]
+for part_len in (64, 1000, 4096):
+    nrows = sum(-(-len(img) // part_len) for img in images)
+    sha = torch.empty((nrows, 32), dtype=torch.uint8, device="cuda")
+    md5 = torch.empty((nrows, 16), dtype=torch.uint8, device="cuda")
+    assert ctx.hash_segment_parts_device([t.data_ptr() if t.numel() else 0 for t in segs], [t.numel() for t in segs],
+                                         [0, len(sizes), len(segs)], part_len, BOTH, sha.data_ptr(),
+                                         md5.data_ptr()) == nrows
+    torch.cuda.synchronize()
+    sha, md5, row = sha.cpu().numpy(), md5.cpu().numpy(), 0
+    for img in images:
+        for o in range(0, len(img), part_len):
+            m = img[o : o + part_len]
+            assert sha[row].tobytes() == hashlib.sha256(m).digest(), (part_len, row)
+            assert md5[row].tobytes() == hashlib.md5(m).digest(), (part_len, row)
+            row += 1
+print("segment parts gather ok", flush=True)
 ctx.close()
 print("ALL OK")
