@@ -284,10 +284,11 @@ typedef struct b200h_cast_box {
  * address that is a multiple of the destination element size.  (Every file written by safetensors.torch.save meets the
  * alignment rules: the header is padded to a multiple of 8 and tensors are laid out by decreasing element size, so
  * every tensor starts at a multiple of its element size.)
- * ONE kernel launch (load_cast_boxes_kernel) per call, none when every box is empty, with tables that grow as those of
- * b200h_copy_boxes_from_host.  Every source word that holds a selected byte crosses PCIe once, in an aligned 16-byte
- * load inside its row's hull; device stores are full aligned 16-byte words except at the ends of a box's run and at
- * one word per 64 KiB tile of source words.  Device bytes outside every box are not written.
+ * ONE kernel launch (load_boxes_kernel, the kernel of b200h_copy_boxes_from_host) per call, none when every box is
+ * empty, with tables that grow as those of b200h_copy_boxes_from_host.  Every source word that holds a selected byte
+ * crosses PCIe once, in an aligned 16-byte load inside its row's hull; device stores are full aligned 16-byte words
+ * except at the ends of a box's run and at one word per 64 KiB tile of source words.  Device bytes outside every box
+ * are not written.
  * The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream), as the range entries do.
  * Replaces: _read_file_into_fileobj (py/modal/volume.py:923-1000) followed by safetensors.torch.load and a per-tensor
  * .to(dtype), which holds the stored image and its converted copy at once, to load a checkpoint in a compute dtype. */

@@ -540,13 +540,7 @@ class Context:
         src_pitch:]`` (any alignment), to bytes ``[offset, offset + rows * width)`` of its file; no device byte may
         belong to two boxes.  One kernel launch, only enqueued on ``stream``: ``src`` must stay unchanged until that
         stream's work has completed."""
-        segs = _segments(seg_ptrs, seg_lens)
-        ffs, nfiles = _segment_args(file_first_seg)
-        bx = np.ascontiguousarray(boxes, dtype=np.uint64).reshape(-1, 6)
-        rc = self._L.b200h_copy_boxes_from_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
-                                                nfiles, _np_ptr(bx) if len(bx) else None, len(bx),
-                                                ctypes.c_void_p(src.ctypes.data), src.size, stream or None)
-        self._check(rc, "b200h_copy_boxes_from_host")
+        self._copy_boxes("b200h_copy_boxes_from_host", 6, seg_ptrs, seg_lens, file_first_seg, boxes, src, stream)
 
     def copy_cast_boxes_from_host(self, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
                                   stream: int = 0) -> None:
@@ -555,13 +549,17 @@ class Context:
         (source element size)`` elements, ``width`` and ``src_pitch`` counted in source bytes, and writes them packed
         from byte ``offset`` of its file.  Rows start at a multiple of the source element size; a box's destination lies
         in one buffer, at a multiple of the destination element size.  One kernel launch, only enqueued on ``stream``."""
+        self._copy_boxes("b200h_copy_cast_boxes_from_host", 8, seg_ptrs, seg_lens, file_first_seg, boxes, src, stream)
+
+    def _copy_boxes(self, entry: str, width: int, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
+                    stream: int) -> None:
         segs = _segments(seg_ptrs, seg_lens)
         ffs, nfiles = _segment_args(file_first_seg)
-        bx = np.ascontiguousarray(boxes, dtype=np.uint64).reshape(-1, 8)
-        rc = self._L.b200h_copy_cast_boxes_from_host(self._h, _np_ptr(segs) if len(segs) else None, len(segs),
-                                                     _np_ptr(ffs), nfiles, _np_ptr(bx) if len(bx) else None, len(bx),
-                                                     ctypes.c_void_p(src.ctypes.data), src.size, stream or None)
-        self._check(rc, "b200h_copy_cast_boxes_from_host")
+        bx = np.ascontiguousarray(boxes, dtype=np.uint64).reshape(-1, width)
+        rc = getattr(self._L, entry)(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs), nfiles,
+                                     _np_ptr(bx) if len(bx) else None, len(bx), ctypes.c_void_p(src.ctypes.data),
+                                     src.size, stream or None)
+        self._check(rc, entry)
 
     def _copy_ranges(self, entry: str, offsets_name: str, seg_ptrs, seg_lens, file_first_seg, ranges, host: np.ndarray,
                      host_offsets, stream: int) -> None:

@@ -1689,31 +1689,29 @@ int b200h_copy_cast_ranges(b200h_ctx* ctx, const b200h_cast_segment* segs, uint6
                        cuda_stream, segs ? segs : &kNoSegment);
 }
 
-// b200h_copy_boxes_from_host (casts == NULL) and b200h_copy_cast_boxes_from_host (boxes == NULL; box i is
-// casts[i].box): box i of h_src to its packed destination run, its elements converted when it is a cast box.
-static int copy_boxes(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
-                      uint64_t nfiles, const b200h_box* boxes, const b200h_cast_box* casts, uint64_t nboxes,
+// Bytes of one element of a box's type code: dt_bytes, or 1 for code 0 (the bytes as they are).
+static uint64_t box_elem_bytes(uint64_t t) { return t ? dt_bytes(t) : 1; }
+
+// b200h_copy_boxes_from_host (cast == false; every box has type code 0 on both sides) and
+// b200h_copy_cast_boxes_from_host: box i of h_src to its packed destination run, its elements converted when its types
+// differ.
+static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint64_t nsegs,
+                      const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes, uint64_t nboxes,
                       const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
     std::vector<uint64_t> seg_lens;
     FileTable t;
     if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
-    if (nboxes && !boxes && !casts) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
+    if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
     if (nboxes && !h_src) return fail(ctx, B200H_E_INVALID, "h_src must not be NULL");
-    auto box = [&](uint64_t i) -> const b200h_box& { return casts ? casts[i].box : boxes[i]; };
-    // source and destination element sizes: a plain box copies bytes
-    auto sizes = [&](uint64_t i, uint64_t& ss, uint64_t& ds) {
-        ss = casts ? dt_bytes(casts[i].src_type) : 1;
-        ds = casts ? dt_bytes(casts[i].dst_type) : 1;
-    };
     bool any = false;
     for (uint64_t i = 0; i < nboxes; ++i) {
-        const b200h_box& b = box(i);
+        const b200h_box& b = boxes[i].box;
         const std::string name = "box " + std::to_string(i);
-        uint64_t ss, ds;
-        sizes(i, ss, ds);
-        if (casts) {
-            if (!ss || !ds) return fail(ctx, B200H_E_INVALID, name + ": unknown element type");
-            if (casts[i].src_type == casts[i].dst_type)
+        const uint64_t ss = box_elem_bytes(boxes[i].src_type), ds = box_elem_bytes(boxes[i].dst_type);
+        if (cast) {
+            if (!dt_bytes(boxes[i].src_type) || !dt_bytes(boxes[i].dst_type))
+                return fail(ctx, B200H_E_INVALID, name + ": unknown element type");
+            if (boxes[i].src_type == boxes[i].dst_type)
                 return fail(ctx, B200H_E_INVALID, name + ": src_type and dst_type are the same");
             if (b.width % ss || b.src_pitch % ss)
                 return fail(ctx, B200H_E_INVALID,
@@ -1736,7 +1734,7 @@ static int copy_boxes(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
                           b.width <= h_src_bytes - (b.rows - 1) * b.src_pitch &&
                           b.src_offset <= h_src_bytes - (b.rows - 1) * b.src_pitch - b.width;
         if (!fits) return fail(ctx, B200H_E_INVALID, name + ": its source reaches past h_src_bytes");
-        if (casts) {  // one segment, so that every destination word holds whole elements
+        if (cast) {  // one segment, so that every destination word holds whole elements
             uint64_t npieces = 0, dev = 0;
             file_pieces(t, b.file, b.offset, nd, [&](uint64_t s, uint64_t in, uint64_t) {
                 if (!npieces++) dev = (uint64_t)(uintptr_t)segs[s].d_ptr + in;
@@ -1767,13 +1765,11 @@ static int copy_boxes(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
     std::vector<CastTile> tiles;
     std::vector<uint64_t> box_of;  // per piece: the box it belongs to (for the overlap message)
     for (uint64_t i = 0; i < nboxes; ++i) {
-        const b200h_box& bx = box(i);
-        uint64_t ss, ds;
-        sizes(i, ss, ds);
+        const b200h_box& bx = boxes[i].box;
+        const uint64_t ss = box_elem_bytes(boxes[i].src_type), ds = box_elem_bytes(boxes[i].dst_type);
         const uint64_t n = bx.rows * bx.width;
         if (!n) continue;
-        CastTile ct{};
-        if (casts) ct.src_type = (uint32_t)casts[i].src_type, ct.dst_type = (uint32_t)casts[i].dst_type;
+        CastTile ct{{}, (uint32_t)boxes[i].src_type, (uint32_t)boxes[i].dst_type};
         BoxTile& b = ct.box;
         const bool run = bx.rows == 1 || bx.src_pitch == bx.width;  // one contiguous source run
         b.src = bx.src_offset + phase;
@@ -1816,14 +1812,8 @@ static int copy_boxes(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
                                                   std::to_string(box_of[by_dev[k]]) + " write the same device bytes");
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
     const void* d_src = (const uint8_t*)d_host - phase;
-    if (casts)
-        return launch_with_tables(ctx, st, tiles, pieces, [&](const CastTile* d_tiles, const RangePiece* d_pieces) {
-            return launch_load_cast_boxes(d_tiles, tiles.size(), d_pieces, d_src, st);
-        });
-    std::vector<BoxTile> plain(tiles.size());
-    for (size_t k = 0; k < tiles.size(); ++k) plain[k] = tiles[k].box;
-    return launch_with_tables(ctx, st, plain, pieces, [&](const BoxTile* d_tiles, const RangePiece* d_pieces) {
-        return launch_load_boxes(d_tiles, plain.size(), d_pieces, d_src, st);
+    return launch_with_tables(ctx, st, tiles, pieces, [&](const CastTile* d_tiles, const RangePiece* d_pieces) {
+        return launch_load_boxes(d_tiles, tiles.size(), d_pieces, d_src, st);
     });
 }
 
@@ -1833,7 +1823,10 @@ int b200h_copy_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64
     if (!ctx) return B200H_E_INVALID;
     B200H_RANGE("b200h_copy_boxes_from_host");
     std::lock_guard<std::mutex> lk(ctx->mu);
-    return copy_boxes(ctx, segs, nsegs, file_first_seg, nfiles, boxes, nullptr, nboxes, h_src, h_src_bytes, cuda_stream);
+    std::vector<b200h_cast_box> casts(boxes ? nboxes : 0);  // type code 0 on both sides: the bytes as they are
+    for (uint64_t i = 0; i < casts.size(); ++i) casts[i].box = boxes[i];
+    return copy_boxes(ctx, false, segs, nsegs, file_first_seg, nfiles, boxes ? casts.data() : nullptr, nboxes, h_src,
+                      h_src_bytes, cuda_stream);
 }
 
 int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
@@ -1843,7 +1836,7 @@ int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, u
     B200H_RANGE("b200h_copy_cast_boxes_from_host");
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
-    return copy_boxes(ctx, segs, nsegs, file_first_seg, nfiles, nullptr, boxes, nboxes, h_src, h_src_bytes, cuda_stream);
+    return copy_boxes(ctx, true, segs, nsegs, file_first_seg, nfiles, boxes, nboxes, h_src, h_src_bytes, cuda_stream);
 }
 
 // ---------------------------------------------------------------------------------------------- files

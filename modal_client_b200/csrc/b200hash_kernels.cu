@@ -684,7 +684,6 @@ lane_hash_kernel(const uint8_t* __restrict__ base, const uint64_t* __restrict__ 
 constexpr int kChainGroups = 4;     // messages per CTA by default (one expander, one SHA-256 and one MD5 warp per SMSP)
 constexpr int kChainGroupsMax = 8;  // B200H_CHAIN_GROUPS=8: twice that per SMSP; off by default
 constexpr int kChainGroupThreads = 96;
-constexpr int kChainThreadsMax = kChainGroupThreads * kChainGroupsMax;
 constexpr int kTileBlocks = 32;
 constexpr int kTileData = kTileBlocks * 64;
 constexpr int kTileStride = kTileData + 32;  // + the misaligned leading granule; keeps 16-byte alignment

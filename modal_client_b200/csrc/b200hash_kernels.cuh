@@ -163,20 +163,18 @@ __host__ __device__ inline uint64_t box_dest_at(const BoxTile& b, uint64_t v) {
     if (r >= b.rows) return b.rows * b.width;
     return c >= b.width ? (r + 1) * b.width : r * b.width + c;
 }
-// Every tile's copy host -> device, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device can
-// load from (the tiles' source offsets count from it).
-int launch_load_boxes(const BoxTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
-// A tile of a box whose elements change type (load_cast_boxes_kernel): `box` as above, in source bytes (dlo and dhi
-// included, which are multiples of the source element size), with the source and destination element types (the
-// B200H_DT_* codes of b200hash.h).  The box's destination is one piece (it lies in one segment), at a device address
-// that is a multiple of the destination element size; packed source byte p of the box lands at destination byte
-// p / (source size) * (destination size).
+// A tile of a box with its source and destination element types.  Equal types (0 and 0 for a plain box): the bytes as
+// they are, `box` as above.  Otherwise two different B200H_DT_* codes of b200hash.h, and the box's elements change type:
+// `box` counts source bytes (dlo and dhi included, which are multiples of the source element size), its destination is
+// one piece (it lies in one segment) at a device address that is a multiple of the destination element size, and packed
+// source byte p of the box lands at destination byte p / (source size) * (destination size).
 struct CastTile {
     BoxTile box;
     uint32_t src_type, dst_type;
 };
-int launch_load_cast_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
-                           cudaStream_t st);
+// Every tile's copy host -> device, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device can
+// load from (the tiles' source offsets count from it).
+int launch_load_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
 
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)

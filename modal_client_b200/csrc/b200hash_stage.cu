@@ -11,7 +11,7 @@
 //                        tensor edge), so a copy at the widest access on which both sides agree, as
 //                        gather_segments_kernel does between HBM buffers, would degrade to byte stores here.  The
 //                        kernel is at the end of the file: its pieces may also convert elements, with the conversion
-//                        helpers of load_cast_boxes_kernel.
+//                        helpers of load_boxes_kernel.
 //
 // A range is cut by the host into pieces (range intersected with one segment, never empty), listed in destination
 // order; a tile names the slice of the piece list it draws from.
@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
 
 // ---- boxes: rows of a page-locked host buffer, `pitch` bytes apart, packed into segmented device files
 //
-//   load_boxes_kernel    persistent CTAs whose warps take tiles of a box's virtual source words (BoxTile), tile t on
+//   load_boxes_kernel    persistent CTAs whose warps take tiles of a box's virtual source words (CastTile), tile t on
 //                        CTA t % gridDim.x so that a call with few tiles still spreads over every SM.  Lane k of a
 //                        chunk loads virtual word 128 * chunk + 32 * i + k (i < kLoadChunks) with one aligned 16-byte
 //                        load, so every source byte that lands crosses PCIe once and no load leaves its row's hull (the
@@ -314,33 +314,15 @@ __device__ __forceinline__ void box_tile_steps(const BoxTile& b, const uint4* wo
     }
 }
 
-__global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
-    load_boxes_kernel(const BoxTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
-                      const uint8_t* __restrict__ src) {
-    __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
-    const uint32_t lane = threadIdx.x & 31u;
-    uint4* ring = rings[threadIdx.x >> 5];
-    const uint4* words = reinterpret_cast<const uint4*>(src);
-    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
-    for (uint64_t t = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; t < ntiles; t += nwarps) {
-        const BoxTile b = tiles[t];
-        const RangePiece* __restrict__ pc = pieces + b.first_piece;
-        box_tile_steps(b, words, ring, lane, [&](uint64_t from, uint64_t upto) {
-            for (uint32_t q = 0; q < b.npieces; ++q) box_words_out(b, pc[q], ring, from, upto, lane);
-        });
-    }
-}
-
 // ---- boxes whose elements change type on the way (F32, F16, BF16; b200h_copy_cast_boxes_from_host)
 //
-//   load_cast_boxes_kernel   load_boxes_kernel's tiles, loads and ring, with a destination word built from elements
-//                        instead of bytes.  Every element of a box lies whole in one aligned source word (rows start at
-//                        a multiple of the element size), and the box's destination is one piece at a multiple of the
-//                        destination element size, so every destination word holds whole elements.  A word of 16 / ds
-//                        elements takes 16 / ds * ss source bytes: 32 when narrowing F32 (two or three ring words), 16
-//                        between F16 and BF16 (one or two), 8 when widening (one or two).  When they are one run of one
-//                        row they come from the ring with shift_bytes; otherwise (a word across rows, a box's ends) element
-//                        by element.  The conversion then takes pairs of elements with the paired sm_90 intrinsics.
+// The same tiles, loads and ring, with a destination word built from elements instead of bytes.  Every element of a
+// box lies whole in one aligned source word (rows start at a multiple of the element size), and the box's destination
+// is one piece at a multiple of the destination element size, so every destination word holds whole elements.  A word
+// of 16 / ds elements takes 16 / ds * ss source bytes: 32 when narrowing F32 (two or three ring words), 16 between F16
+// and BF16 (one or two), 8 when widening (one or two).  When they are one run of one row they come from the ring with
+// shift_bytes; otherwise (a word across rows, a box's ends) element by element.  The conversion then takes pairs of
+// elements with the paired sm_90 intrinsics.
 
 constexpr uint32_t kDtF32 = B200H_DT_F32, kDtF16 = B200H_DT_F16;
 
@@ -440,9 +422,12 @@ __device__ __forceinline__ void cast_words_out(const BoxTile& b, uint32_t st, ui
     }
 }
 
+// Every box, converting or not: the type pair is per tile, so the branch is warp-uniform.  A tile that converts
+// nothing (equal types; 0 and 0 for b200h_copy_boxes_from_host) stores bytes through every piece it uses, so its box
+// may span segments; a converting tile's box is one piece.
 __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
-    load_cast_boxes_kernel(const CastTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
-                           const uint8_t* __restrict__ src) {
+    load_boxes_kernel(const CastTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
+                      const uint8_t* __restrict__ src) {
     __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
     const uint32_t lane = threadIdx.x & 31u;
     uint4* ring = rings[threadIdx.x >> 5];
@@ -450,10 +435,18 @@ __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
     const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
     for (uint64_t t = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; t < ntiles; t += nwarps) {
         const CastTile ct = tiles[t];
-        const uint64_t dev = pieces[ct.box.first_piece].dev;
-        box_tile_steps(ct.box, words, ring, lane, [&](uint64_t from, uint64_t upto) {
-            cast_words_out(ct.box, ct.src_type, ct.dst_type, dev, ring, from, upto, lane);
-        });
+        const BoxTile& b = ct.box;
+        const RangePiece* __restrict__ pc = pieces + b.first_piece;
+        if (ct.src_type == ct.dst_type) {
+            box_tile_steps(b, words, ring, lane, [&](uint64_t from, uint64_t upto) {
+                for (uint32_t q = 0; q < b.npieces; ++q) box_words_out(b, pc[q], ring, from, upto, lane);
+            });
+        } else {
+            const uint64_t dev = pc->dev;
+            box_tile_steps(b, words, ring, lane, [&](uint64_t from, uint64_t upto) {
+                cast_words_out(b, ct.src_type, ct.dst_type, dev, ring, from, upto, lane);
+            });
+        }
     }
 }
 
@@ -562,20 +555,11 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
 
 }  // namespace
 
-int launch_load_boxes(const BoxTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
+int launch_load_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
     if (!ntiles) return 0;
     const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
     load_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
                                                                                    static_cast<const uint8_t*>(src));
-    return 1;
-}
-
-int launch_load_cast_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
-                           cudaStream_t st) {
-    if (!ntiles) return 0;
-    const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
-    load_cast_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
-        tiles, ntiles, pieces, static_cast<const uint8_t*>(src));
     return 1;
 }
 

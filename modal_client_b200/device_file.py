@@ -379,6 +379,12 @@ def load_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> L
     boxes = [tuple(int(x) for x in b) for b in boxes]
     if any(len(b) != 6 for b in boxes):
         raise ValueError("a box is (file, offset, width, rows, src_offset, src_pitch)")
+    return _load_boxes(ctx, "copy_boxes_from_host", sources, boxes, src)
+
+
+def _load_boxes(ctx, entry: str, sources: list[_TensorBytes], boxes, src: np.ndarray) -> Loaded:
+    """The body of ``load_boxes`` and ``load_cast_boxes``: ONE call of ``ctx``'s ``entry`` with the checked boxes, on
+    the first file's stream, ordered as ``load_ranges``."""
     if boxes and not sources:
         raise ValueError("boxes without files")
     if not sources:
@@ -387,7 +393,7 @@ def load_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> L
     lead._after_current()
     ptrs, lens, first = _file_table(sources)
     with lead._on_stream():
-        ctx.copy_boxes_from_host(ptrs, lens, first, boxes, src, lead.stream_handle)
+        getattr(ctx, entry)(ptrs, lens, first, boxes, src, lead.stream_handle)
     return Loaded(lead._publish())
 
 
@@ -464,16 +470,7 @@ def load_cast_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None)
             if dt not in codes:
                 raise ValueError(f"load_cast_boxes converts between {', '.join(map(str, codes))}, not {dt}")
     boxes = [tuple(int(x) for x in b[:6]) + (codes[b[6]], codes[b[7]]) for b in boxes]
-    if boxes and not sources:
-        raise ValueError("boxes without files")
-    if not sources:
-        return Loaded(None)
-    lead = sources[0]
-    lead._after_current()
-    ptrs, lens, first = _file_table(sources)
-    with lead._on_stream():
-        ctx.copy_cast_boxes_from_host(ptrs, lens, first, boxes, src, lead.stream_handle)
-    return Loaded(lead._publish())
+    return _load_boxes(ctx, "copy_cast_boxes_from_host", sources, boxes, src)
 
 
 # ------------------------------------------------------------------------------------------ safetensors

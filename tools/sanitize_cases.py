@@ -9,9 +9,11 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
   stage        stage_ranges_kernel: ranges of segmented device files into page-locked host memory: every source
                phase, segments that start at the first and end at the last byte of their allocation (the aligned-hull
                loads), ranges across tiny and empty segments, partial last words
-  cast boxes   load_cast_boxes_kernel: every conversion between F32, F16 and BF16, boxes that end at the last byte of
-               their exact-size destination allocation and of the page-locked source, every element phase, rows that
-               cross destination words, 1-element rows
+  boxes        load_boxes_kernel: rows at every source phase into a file of exact-size allocations, boxes across
+               segment seams, the last box ending at the last byte of the file and of the page-locked source
+  cast boxes   load_boxes_kernel converting: every conversion between F32, F16 and BF16, boxes that end at the last
+               byte of their exact-size destination allocation and of the page-locked source, every element phase, rows
+               that cross destination words, 1-element rows
   cast ranges  stage_ranges_kernel with converting pieces: every conversion, segments that are exact-size allocations,
                ranges at odd image offsets into page-locked host memory and into device memory
   gather       gather_segments_kernel (b200h_hash_segment_parts_device): segments that are exact-size allocations,
@@ -120,7 +122,31 @@ assert (dst[clean] == 0xC3).all()
 ctx.host_free(dst)
 print("stage ranges ok", flush=True)
 
-# 7. load_cast_boxes_kernel: each box fills an exact-size allocation; the last box reads the source's last bytes
+# 7. load_boxes_kernel, the bytes as they are: one file of exact-size allocations, every other box across the seam of
+#    two of them; rows at every source phase, with rows that touch, narrow gaps, wide gaps and a box of two tiles; the
+#    last box ends at the file's last byte and reads the source's last bytes
+src = ctx.host_alloc(1 << 20)
+src[:] = synth_array(8, 1 << 20)
+shapes = ((1, 9, 0), (3, 7, 1), (37, 5, 2), (9000, 2, 5), (17, 4, 0), (5, 6, 27), (40, 3, 40), (70_001, 1, 0))
+boxes, at, d = [], 0, 0
+for ph in range(16):
+    w, rows, gap = shapes[ph % len(shapes)]
+    at = -(-at // 16) * 16 + ph
+    boxes.append((0, d, w, rows, at, w + gap))
+    at += (rows - 1) * (w + gap) + w
+    d += w * rows
+f, o, w, rows, _, pitch = boxes[-1]
+boxes[-1] = (f, o, w, rows, src.size - (rows - 1) * pitch - w, pitch)
+cuts = [0] + [o + w * rows // 2 for _, o, w, rows, _, _ in boxes[1::2]] + [d]
+segs = [torch.zeros(b - a, dtype=torch.uint8, device="cuda") for a, b in zip(cuts, cuts[1:])]
+ctx.copy_boxes_from_host([t.data_ptr() for t in segs], [t.numel() for t in segs], [0, len(segs)], boxes, src, 1)
+torch.cuda.synchronize()
+want = np.concatenate([src[a + r * pitch : a + r * pitch + w] for _, _, w, rows, a, pitch in boxes for r in range(rows)])
+assert np.array_equal(torch.cat(segs).cpu().numpy(), want)
+ctx.host_free(src)
+print("boxes ok", flush=True)
+
+# 8. load_boxes_kernel converting: each box fills an exact-size allocation; the last box reads the source's last bytes
 names = {_lib.DT_F32: torch.float32, _lib.DT_F16: torch.float16, _lib.DT_BF16: torch.bfloat16}
 src = ctx.host_alloc(1 << 20)
 src[:] = synth_array(7, 1 << 20)
@@ -143,7 +169,7 @@ for (f, _, w, rows, a, pitch, st, dt), t in zip(boxes, outs):
 ctx.host_free(src)
 print("cast boxes ok", flush=True)
 
-# 8. stage_ranges_kernel with converting pieces: every conversion, each segment an exact-size allocation (its first
+# 9. stage_ranges_kernel with converting pieces: every conversion, each segment an exact-size allocation (its first
 #    and last bytes are those of the allocation), plain bytes between them, ranges at odd image offsets into host and
 #    device memory
 segs, casts, at = [], [], 0
@@ -177,8 +203,8 @@ for dst in (host, dev):
 ctx.host_free(host)
 print("cast ranges ok", flush=True)
 
-# 9. gather_segments_kernel (b200h_hash_segment_parts_device): each segment an exact-size allocation, parts that
-#    straddle segments at every relative phase of source and wave slot, and parts hashed in place in the long segments
+# 10. gather_segments_kernel (b200h_hash_segment_parts_device): each segment an exact-size allocation, parts that
+#     straddle segments at every relative phase of source and wave slot, and parts hashed in place in the long segments
 sizes = [1, 15, 16, 17, 0, 33, 255, 4097, 70_001, 3, 5000, 64, 9] + [1 + i * 37 % 97 for i in range(48)]
 files = [[torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda") for n in f] for f in (sizes, sizes[::-1])]
 segs = [t for f in files for t in f]
