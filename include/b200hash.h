@@ -296,6 +296,46 @@ int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, u
                                     const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes,
                                     uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream);
 
+/* FP8 element types (OCP 8-bit floats: E4M3 with no infinities, as torch.float8_e4m3fn; E5M2, as torch.float8_e5m2).
+ * Only b200h_copy_scaled_boxes_from_host takes them; the other entries refuse them as unknown types. */
+#define B200H_DT_F8E4M3 4u
+#define B200H_DT_F8E5M2 5u
+
+/* A box of FP8 elements dequantized on the way: `cast` as in b200h_cast_box, with src_type B200H_DT_F8E4M3 or
+ * B200H_DT_F8E5M2 (so width and src_pitch count elements as well as bytes) and dst_type B200H_DT_F32, F16 or BF16.
+ * The box is cut from the R x C row-major tensor W (rows_total = R, cols = C): element c of its row r is W's element
+ * first_elem + r * src_pitch + c, i.e. (that / C, that % C).  Its scales are scale_count elements of scale_type
+ * (B200H_DT_F32, F16 or BF16) at d_scales, device memory of the context's device, ceil(R / block_rows) x
+ * ceil(C / block_cols) of them in row-major order: element (i, j) of W uses scale (i / block_rows) *
+ * ceil(C / block_cols) + j / block_cols.  A block size of R or more (C or more) is one block over the dimension. */
+typedef struct b200h_scaled_box {
+    b200h_cast_box cast;
+    const void* d_scales;
+    uint64_t scale_type, scale_count;
+    uint64_t first_elem;
+    uint64_t rows_total, cols;
+    uint64_t block_rows, block_cols;
+} b200h_scaled_box;
+
+/* b200h_copy_cast_boxes_from_host for FP8 boxes with block scales: every element of box i is decoded exactly, multiplied
+ * in F32 by its scale (widened exactly), rounding to nearest even with subnormals kept, and the product rounded once
+ * to dst_type (no second rounding for F32): bit for bit what torch computes on CUDA as
+ * (W.float() * S.float().repeat_interleave(block_rows, 0)[:R].repeat_interleave(block_cols, 1)[:, :C]).to(dst).
+ * A NaN element or product gives a NaN (0x7FFF for a 16-bit target, 0x7FFFFFFF for F32).
+ * Every argument is checked before any work is enqueued, B200H_E_INVALID otherwise: every rule of
+ * b200h_copy_cast_boxes_from_host, with src_type an FP8 code, and further: block_rows and block_cols >= 1;
+ * ceil(R / block_rows) * ceil(C / block_cols) <= scale_count; every element a box touches lies below R * C (both computed
+ * without overflow); scale_type a known code; d_scales aligned to its element size, and its scale_count elements device
+ * memory of the context's device (cudaPointerGetAttributes).
+ * ONE kernel launch (load_scaled_boxes_kernel) per call, none when every box is empty, with tables that grow as those of
+ * b200h_copy_boxes_from_host (never with the rows).  Source words cross PCIe once, as for the cast entry; scales are
+ * read from device memory.  The call ONLY ENQUEUES on `cuda_stream` (NULL = the context's compute stream).
+ * Replaces: loading an FP8 checkpoint and its scales, then w.float() * expanded_scale per weight in torch (DeepSeek's
+ * fp8_cast_bf16.py), which holds the FP8 image, the results and F32 temporaries in HBM together. */
+int b200h_copy_scaled_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                      const uint64_t* file_first_seg, uint64_t nfiles, const b200h_scaled_box* boxes,
+                                      uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream);
+
 /* A segment of a file whose elements may change type on the way out: len SOURCE bytes at d_ptr (device memory on ctx's
  * device).  src_type == dst_type: the bytes as they are (0 or a B200H_DT_* code).  Otherwise two different B200H_DT_*
  * codes, and the segment contributes its len / (source element size) elements converted to dst_type, packed:

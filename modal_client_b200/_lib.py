@@ -24,6 +24,7 @@ TRIM_ZEROS = 4
 HEX_OUT = 32  # digest outputs as lowercase ASCII hex rows (64 / 32 chars), formatted on the device
 NO_OUTLIERS = 16  # keep every message on the lane kernel: device batches then only enqueue (include/b200hash.h)
 DT_F32, DT_F16, DT_BF16 = 1, 2, 3  # element types of copy_cast_boxes_from_host (B200H_DT_*)
+DT_F8E4M3, DT_F8E5M2 = 4, 5  # FP8 source types of copy_scaled_boxes_from_host only
 
 #: every symbol include/b200hash.h declares (tests check the .so exports all of them)
 ABI_SYMBOLS = (
@@ -37,7 +38,7 @@ ABI_SYMBOLS = (
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
     "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host", "b200h_copy_boxes_from_host",
     "b200h_copy_cast_boxes_from_host", "b200h_copy_cast_ranges", "b200h_hash_cast_segment_parts_device",
-    "b200h_cast_segment_parts_preview",
+    "b200h_cast_segment_parts_preview", "b200h_copy_scaled_boxes_from_host",
 )
 
 
@@ -121,6 +122,8 @@ def load_library() -> ctypes.CDLL:
         L.b200h_copy_boxes_from_host.restype = i32
         L.b200h_copy_cast_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
         L.b200h_copy_cast_boxes_from_host.restype = i32
+        L.b200h_copy_scaled_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
+        L.b200h_copy_scaled_boxes_from_host.restype = i32
         L.b200h_copy_cast_ranges.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
         L.b200h_copy_cast_ranges.restype = i32
         L.b200h_hash_cast_segment_parts_device.argtypes = [vp, vp, u64, vp, u64, u64, u32, vp, vp, vp,
@@ -550,6 +553,17 @@ class Context:
         from byte ``offset`` of its file.  Rows start at a multiple of the source element size; a box's destination lies
         in one buffer, at a multiple of the destination element size.  One kernel launch, only enqueued on ``stream``."""
         self._copy_boxes("b200h_copy_cast_boxes_from_host", 8, seg_ptrs, seg_lens, file_first_seg, boxes, src, stream)
+
+    def copy_scaled_boxes_from_host(self, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
+                                    stream: int = 0) -> None:
+        """``copy_cast_boxes_from_host`` for FP8 boxes with block scales: box i = ``(file, offset, width, rows,
+        src_offset, src_pitch, src_type, dst_type, scales_ptr, scale_type, scale_count, first_elem, R, C, block_rows,
+        block_cols)``, ``src_type`` ``DT_F8E4M3`` / ``DT_F8E5M2`` and ``dst_type`` / ``scale_type`` ``DT_F32`` /
+        ``DT_F16`` / ``DT_BF16``.  Element c of row r of the box is element ``first_elem + r * src_pitch + c`` of an R x C
+        tensor, multiplied by its scale (``scale_count`` elements at device address ``scales_ptr``, one per block,
+        row-major) before it is rounded to ``dst_type``.  One kernel launch, only enqueued on ``stream``."""
+        self._copy_boxes("b200h_copy_scaled_boxes_from_host", 16, seg_ptrs, seg_lens, file_first_seg, boxes, src,
+                         stream)
 
     def _copy_boxes(self, entry: str, width: int, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
                     stream: int) -> None:

@@ -1689,15 +1689,40 @@ int b200h_copy_cast_ranges(b200h_ctx* ctx, const b200h_cast_segment* segs, uint6
                        cuda_stream, segs ? segs : &kNoSegment);
 }
 
-// Bytes of one element of a box's type code: dt_bytes, or 1 for code 0 (the bytes as they are).
-static uint64_t box_elem_bytes(uint64_t t) { return t ? dt_bytes(t) : 1; }
+static bool is_fp8(uint64_t t) { return t == B200H_DT_F8E4M3 || t == B200H_DT_F8E5M2; }
 
-// b200h_copy_boxes_from_host (cast == false; every box has type code 0 on both sides) and
-// b200h_copy_cast_boxes_from_host: box i of h_src to its packed destination run, its elements converted when its types
-// differ.
+// Bytes of one element of a box's type code: dt_bytes, or 1 for code 0 (the bytes as they are) and the FP8 codes.
+static uint64_t box_elem_bytes(uint64_t t) { return t && !is_fp8(t) ? dt_bytes(t) : 1; }
+
+static uint64_t ceil_div(uint64_t a, uint64_t b) { return a / b + (a % b != 0); }
+
+// The rules of a scaled box that need no device: its types, block sizes, the scale count and the tensor bounds.
+static std::string scaled_box_fault(const b200h_scaled_box& x) {
+    const b200h_box& b = x.cast.box;
+    if (!is_fp8(x.cast.src_type)) return ": src_type is not an FP8 type";
+    if (!dt_bytes(x.cast.dst_type)) return ": dst_type is not F32, F16 or BF16";
+    if (!dt_bytes(x.scale_type)) return ": scale_type is not F32, F16 or BF16";
+    if (!x.block_rows || !x.block_cols) return ": block sizes must be >= 1";
+    const unsigned __int128 nscales =
+        (unsigned __int128)ceil_div(x.rows_total, x.block_rows) * ceil_div(x.cols, x.block_cols);
+    if (nscales > x.scale_count) return ": scale_count is less than ceil(R / block_rows) * ceil(C / block_cols)";
+    if (!x.d_scales) return ": d_scales is NULL";
+    if ((uintptr_t)x.d_scales % dt_bytes(x.scale_type)) return ": d_scales is not aligned to its element size";
+    if (b.rows && b.width) {  // first_elem + (rows - 1) * src_pitch + width <= R * C
+        const unsigned __int128 end =
+            (unsigned __int128)x.first_elem + (unsigned __int128)(b.rows - 1) * b.src_pitch + b.width;
+        if (end > (unsigned __int128)x.rows_total * x.cols) return ": it reaches past element R * C of its tensor";
+    }
+    return "";
+}
+
+// b200h_copy_boxes_from_host (cast == false; every box has type code 0 on both sides),
+// b200h_copy_cast_boxes_from_host and b200h_copy_scaled_boxes_from_host (`scaled`: box i's scales, boxes[i] ==
+// scaled[i].cast): box i of h_src to its packed destination run, its elements converted when its types differ.
 static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint64_t nsegs,
                       const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes, uint64_t nboxes,
-                      const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
+                      const void* h_src, uint64_t h_src_bytes, void* cuda_stream,
+                      const b200h_scaled_box* scaled = nullptr) {
     std::vector<uint64_t> seg_lens;
     FileTable t;
     if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
@@ -1708,9 +1733,14 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
         const b200h_box& b = boxes[i].box;
         const std::string name = "box " + std::to_string(i);
         const uint64_t ss = box_elem_bytes(boxes[i].src_type), ds = box_elem_bytes(boxes[i].dst_type);
-        if (cast) {
+        if (scaled) {
+            const std::string fault = scaled_box_fault(scaled[i]);
+            if (!fault.empty()) return fail(ctx, B200H_E_INVALID, name + fault);
+        } else if (cast) {
             if (!dt_bytes(boxes[i].src_type) || !dt_bytes(boxes[i].dst_type))
                 return fail(ctx, B200H_E_INVALID, name + ": unknown element type");
+        }
+        if (cast) {
             if (boxes[i].src_type == boxes[i].dst_type)
                 return fail(ctx, B200H_E_INVALID, name + ": src_type and dst_type are the same");
             if (b.width % ss || b.src_pitch % ss)
@@ -1748,6 +1778,20 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
     }
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
+    if (scaled) {  // every box's scales in device memory of ctx's device (boxes of one tensor share them: checked once)
+        std::vector<std::pair<uintptr_t, uint64_t>> seen;
+        for (uint64_t i = 0; i < nboxes; ++i) {
+            const b200h_scaled_box& x = scaled[i];
+            const std::pair<uintptr_t, uint64_t> at{(uintptr_t)x.d_scales, x.scale_count};
+            if (std::find(seen.end() - std::min<size_t>(seen.size(), 8), seen.end(), at) != seen.end()) continue;
+            const uint64_t es = dt_bytes(x.scale_type);
+            if (x.scale_count > ~0ull / es || at.first + x.scale_count * es < at.first ||
+                !device_range_ok(ctx, x.d_scales, x.scale_count * es))
+                return fail(ctx, B200H_E_INVALID, "box " + std::to_string(i) + ": its scale_count scales at d_scales "
+                                                  "are not device memory of cuda:" + std::to_string(ctx->device));
+            seen.push_back(at);
+        }
+    }
     if (nboxes == 0) return 0;
     void* d_host = pinned_device_pointer(ctx, h_src, h_src_bytes);
     if (!d_host)
@@ -1763,7 +1807,8 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
     // of every box's virtual source words (see BoxTile): neither grows with the rows
     std::vector<RangePiece> pieces;
     std::vector<CastTile> tiles;
-    std::vector<uint64_t> box_of;  // per piece: the box it belongs to (for the overlap message)
+    std::vector<uint64_t> box_of;   // per piece: the box it belongs to (for the overlap message)
+    std::vector<uint64_t> tile_of;  // per tile: its box (for the scaled tiles)
     for (uint64_t i = 0; i < nboxes; ++i) {
         const b200h_box& bx = boxes[i].box;
         const uint64_t ss = box_elem_bytes(boxes[i].src_type), ds = box_elem_bytes(boxes[i].dst_type);
@@ -1800,6 +1845,7 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
             b.first_piece = p;
             b.npieces = (uint32_t)(q - p + 1);
             tiles.push_back(ct);
+            tile_of.push_back(i);
         }
     }
     // no device byte may be written twice: two files, or two segments of one file, may share a tensor
@@ -1812,6 +1858,19 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
                                                   std::to_string(box_of[by_dev[k]]) + " write the same device bytes");
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
     const void* d_src = (const uint8_t*)d_host - phase;
+    if (scaled) {
+        std::vector<ScaledTile> sc(tiles.size());
+        for (size_t k = 0; k < tiles.size(); ++k) {
+            const b200h_scaled_box& x = scaled[tile_of[k]];
+            // a block over the whole dimension (or more) is the dimension, so that no block edge lies past it
+            const uint64_t bc = std::min(x.block_cols, x.cols), br = std::min(x.block_rows, x.rows_total);
+            sc[k] = {tiles[k], (uint64_t)(uintptr_t)x.d_scales, x.first_elem, x.cols, br, bc, ceil_div(x.cols, bc),
+                     (uint32_t)x.scale_type, 0};
+        }
+        return launch_with_tables(ctx, st, sc, pieces, [&](const ScaledTile* d_tiles, const RangePiece* d_pieces) {
+            return launch_load_scaled_boxes(d_tiles, sc.size(), d_pieces, d_src, st);
+        });
+    }
     return launch_with_tables(ctx, st, tiles, pieces, [&](const CastTile* d_tiles, const RangePiece* d_pieces) {
         return launch_load_boxes(d_tiles, tiles.size(), d_pieces, d_src, st);
     });
@@ -1837,6 +1896,19 @@ int b200h_copy_cast_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, u
     std::lock_guard<std::mutex> lk(ctx->mu);
     if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
     return copy_boxes(ctx, true, segs, nsegs, file_first_seg, nfiles, boxes, nboxes, h_src, h_src_bytes, cuda_stream);
+}
+
+int b200h_copy_scaled_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                      const uint64_t* file_first_seg, uint64_t nfiles, const b200h_scaled_box* boxes,
+                                      uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_scaled_boxes_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
+    std::vector<b200h_cast_box> casts(boxes ? nboxes : 0);
+    for (uint64_t i = 0; i < casts.size(); ++i) casts[i] = boxes[i].cast;
+    return copy_boxes(ctx, true, segs, nsegs, file_first_seg, nfiles, boxes ? casts.data() : nullptr, nboxes, h_src,
+                      h_src_bytes, cuda_stream, boxes);
 }
 
 // ---------------------------------------------------------------------------------------------- files

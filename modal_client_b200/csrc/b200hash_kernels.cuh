@@ -175,6 +175,20 @@ struct CastTile {
 // Every tile's copy host -> device, in one launch (none when ntiles == 0); `src` is 16-byte aligned memory the device can
 // load from (the tiles' source offsets count from it).
 int launch_load_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st);
+// A tile of a box of FP8 elements (cast.src_type B200H_DT_F8E4M3 or B200H_DT_F8E5M2) dequantized on the way: `cast` as
+// above with one-byte source elements, and element (i, j) of the R x C tensor the box is cut from multiplied by scale
+// (i / block_rows) * scale_cols + j / block_cols of `scales` (type scale_type, device memory) before it is rounded to
+// cast.dst_type.  The tensor element of packed source byte p (counted from the box's first source byte, box.src) is
+// first_elem + (row of p) * box.pitch + (column of p): the box's rows are rows of the tensor's row-major storage.
+struct ScaledTile {
+    CastTile cast;
+    uint64_t scales;
+    uint64_t first_elem, cols, block_rows, block_cols, scale_cols;
+    uint32_t scale_type, pad;
+};
+// Every tile's copy host -> device, in one launch (load_scaled_boxes_kernel; none when ntiles == 0).
+int launch_load_scaled_boxes(const ScaledTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
+                             cudaStream_t st);
 
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)

@@ -26,6 +26,7 @@
 // aligned and sized in multiples of that), which the lane kernel's misaligned-start reads rely on as well.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -450,6 +451,139 @@ __global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
     }
 }
 
+// ---- boxes of FP8 elements dequantized on the way (b200h_copy_scaled_boxes_from_host)
+//
+//   load_scaled_boxes_kernel  the tiles, loads and ring of load_boxes_kernel, with another store step.  A destination
+//                        word of 16 / ds elements takes 16 / ds source bytes (8 for a 16-bit target, 4 for F32): from
+//                        one ring word, or two and shift_bytes, when they are one run of one row; element by element
+//                        otherwise (a word across rows, a box's ends).  Every element is decoded exactly (FP8 -> F16
+//                        -> F32, both exact), multiplied by its scale (widened exactly) with one round-to-nearest
+//                        multiply that keeps subnormals, and rounded once to the target: bit for bit torch's
+//                        (W.float() * S_expanded).to(T) on CUDA.  The tensor coordinates (i, j) of a word's first
+//                        element are computed once per word (again where a box row ends inside the word), then
+//                        stepped one element at a time; a scale is loaded when (i, j) crosses a block-column edge or a
+//                        row's end.  Its own kernel, so that load_boxes_kernel's code stays as it is.
+
+constexpr uint32_t kDtF8E4M3 = B200H_DT_F8E4M3;
+
+// Where the next element of a word lies in the tensor, and its scale.
+struct ScaleCursor {
+    uint64_t i, j, jend;  // the element's coordinates; the column where its scale block (or the row) ends
+    float s;
+};
+
+// the scale of element (q.i, q.j), and the end of its block column
+__device__ __forceinline__ void scale_load(const ScaledTile& t, ScaleCursor& q) {
+    const uint64_t jb = q.j / t.block_cols, k = q.i / t.block_rows * t.scale_cols + jb;
+    q.jend = min((jb + 1) * t.block_cols, t.cols);
+    if (t.scale_type == kDtF32) {
+        q.s = __ldg(reinterpret_cast<const float*>(t.scales) + k);
+    } else {
+        const unsigned short x = __ldg(reinterpret_cast<const unsigned short*>(t.scales) + k);
+        q.s = t.scale_type == kDtF16 ? __half2float(__ushort_as_half(x)) : __bfloat162float(__ushort_as_bfloat16(x));
+    }
+}
+
+// the cursor at tensor element e (its row-major index)
+__device__ __forceinline__ void scale_seek(const ScaledTile& t, uint64_t e, ScaleCursor& q) {
+    q.i = e / t.cols;
+    q.j = e - q.i * t.cols;
+    scale_load(t, q);
+}
+
+// the scale of the cursor's element; the cursor moves on to the tensor's next element
+__device__ __forceinline__ float scale_next(const ScaledTile& t, ScaleCursor& q) {
+    if (q.j == q.jend) {
+        if (q.j == t.cols) q.j = 0, ++q.i;
+        scale_load(t, q);
+    }
+    ++q.j;
+    return q.s;
+}
+
+// the two FP8 elements of the low 16 bits of x (type t), exactly as floats
+__device__ __forceinline__ float2 fp8_pair(uint32_t x, uint32_t t) {
+    const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(x & 0xffffu),
+                                                     t == kDtF8E4M3 ? __NV_E4M3 : __NV_E5M2);
+    return __half22float2(__half2(h));
+}
+
+// Destination words of the box (one piece at device address `dev`) whose elements have packed source bytes in
+// [from, upto) (clipped to [b.dlo, b.dhi)) and whose last element's source lies before `upto`.
+__device__ __forceinline__ void scaled_words_out(const ScaledTile& t, uint64_t dev, const uint4* ring, uint64_t from,
+                                                 uint64_t upto, uint32_t lane) {
+    const BoxTile& b = t.cast.box;
+    const uint32_t st = t.cast.src_type, dt = t.cast.dst_type, ds = dt_bytes(dt);
+    const uint64_t qhi = b.dhi * ds, lo = from * ds, hi = upto * ds;
+    if (lo >= hi) return;
+    const uint64_t qa = dev + b.dlo * ds, qe = dev + qhi, ha = dev + hi;
+    // a word whose elements go on past `hi` waits for the next step
+    const uint64_t w1 = hi < qhi ? ha >> 4 : ((ha - 1) >> 4) + 1;
+    for (uint64_t w = ((dev + lo) >> 4) + lane; w < w1; w += 32) {
+        const uint64_t ws = w * 16, aa = max(ws, qa), ea = min(ws + 16, qe);
+        const uint32_t jlo = (uint32_t)(aa - ws), jhi = (uint32_t)(ea - ws);
+        const uint64_t e = (aa - dev) / ds;  // the word's first element, counted in the box's packed run
+        uint64_t r = e / b.width, c = e % b.width;
+        ScaleCursor q;
+        uint4 v;
+        if (jhi - jlo == 16 && c + 16 / ds <= b.width) {
+            const uint64_t s = b.src + r * b.pitch + c;
+            const uint32_t slot = (uint32_t)(box_virtual(b, r, s) - b.v0), sh = (uint32_t)s & 15u;
+            const uint4 w0 = ring[slot % kBoxRing];
+            const uint4 x = sh + 16 / ds > 16 ? shift_bytes(w0, ring[(slot + 1) % kBoxRing], sh) : shift_bytes(w0, w0, sh);
+            scale_seek(t, t.first_elem + r * b.pitch + c, q);
+            const float2 p0 = fp8_pair(x.x, st), p1 = fp8_pair(x.x >> 16, st);
+            const float s0 = scale_next(t, q), s1 = scale_next(t, q), s2 = scale_next(t, q), s3 = scale_next(t, q);
+            const float a0 = __fmul_rn(p0.x, s0), a1 = __fmul_rn(p0.y, s1), a2 = __fmul_rn(p1.x, s2),
+                        a3 = __fmul_rn(p1.y, s3);
+            if (ds == 4) {
+                v = make_uint4(__float_as_uint(a0), __float_as_uint(a1), __float_as_uint(a2), __float_as_uint(a3));
+            } else {
+                const float2 p2 = fp8_pair(x.y, st), p3 = fp8_pair(x.y >> 16, st);
+                const float s4 = scale_next(t, q), s5 = scale_next(t, q), s6 = scale_next(t, q), s7 = scale_next(t, q);
+                v = make_uint4(narrow_pair(a0, a1, dt), narrow_pair(a2, a3, dt),
+                               narrow_pair(__fmul_rn(p2.x, s4), __fmul_rn(p2.y, s5), dt),
+                               narrow_pair(__fmul_rn(p3.x, s6), __fmul_rn(p3.y, s7), dt));
+            }
+        } else {
+            uint64_t x[2] = {0, 0};  // the results, element k at byte k * ds
+            bool seek = true;
+#pragma unroll 1
+            for (uint32_t j = jlo; j < jhi; j += ds) {
+                const uint64_t s = b.src + r * b.pitch + c;
+                const uint8_t* word =
+                    reinterpret_cast<const uint8_t*>(ring + (uint32_t)(box_virtual(b, r, s) - b.v0) % kBoxRing);
+                if (seek) scale_seek(t, t.first_elem + r * b.pitch + c, q), seek = false;
+                const float a = __fmul_rn(fp8_pair(word[s & 15u], st).x, scale_next(t, q));
+                const uint64_t val = (ds == 4 ? (uint64_t)__float_as_uint(a) : (uint64_t)(narrow_pair(a, 0.f, dt) & 0xffffu))
+                                     << (8 * (j & 7));
+                if (j < 8) x[0] |= val;
+                else x[1] |= val;
+                if (++c == b.width) c = 0, ++r, seek = true;
+            }
+            v = make_uint4((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
+        }
+        store_bytes(reinterpret_cast<uint8_t*>(ws), v, jlo, jhi);
+    }
+}
+
+__global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
+    load_scaled_boxes_kernel(const ScaledTile* __restrict__ tiles, uint64_t ntiles,
+                             const RangePiece* __restrict__ pieces, const uint8_t* __restrict__ src) {
+    __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
+    const uint32_t lane = threadIdx.x & 31u;
+    uint4* ring = rings[threadIdx.x >> 5];
+    const uint4* words = reinterpret_cast<const uint4*>(src);
+    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
+    for (uint64_t k = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; k < ntiles; k += nwarps) {
+        const ScaledTile t = tiles[k];
+        const uint64_t dev = pieces[t.cast.box.first_piece].dev;
+        box_tile_steps(t.cast.box, words, ring, lane, [&](uint64_t from, uint64_t upto) {
+            scaled_words_out(t, dev, ring, from, upto, lane);
+        });
+    }
+}
+
 // ---- stage_ranges_kernel, whose pieces may change type on the way out (b200h_copy_cast_ranges, and the wave-slot
 //      gather of b200h_hash_cast_segment_parts_device)
 //
@@ -560,6 +694,15 @@ int launch_load_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* 
     const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
     load_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
                                                                                    static_cast<const uint8_t*>(src));
+    return 1;
+}
+
+int launch_load_scaled_boxes(const ScaledTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
+                             cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
+    load_scaled_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
+        tiles, ntiles, pieces, static_cast<const uint8_t*>(src));
     return 1;
 }
 

@@ -28,6 +28,8 @@ buffer into the files' tensors with ONE ``b200h_copy_ranges_from_host`` call (``
 packed into the files with ONE ``b200h_copy_boxes_from_host`` call (``volume.read_safetensors_slices``).
 ``load_cast_boxes(files, boxes, src)`` is ``load_boxes`` whose elements change type on the way (F32, F16, BF16), with
 ONE ``b200h_copy_cast_boxes_from_host`` call (``volume.read_safetensors(..., dtype=...)``).
+``load_scaled_boxes(files, boxes, src)`` dequantizes FP8 boxes with their block scales on the way, with ONE
+``b200h_copy_scaled_boxes_from_host`` call (``volume.read_safetensors(..., dtype=..., scales=...)``).
 
 ``safetensors_shards(state_dict, max_shard_size=...)`` is a checkpoint in the Hugging Face Hub's sharded layout: the
 files ``huggingface_hub.save_torch_state_dict`` writes, each shard a ``DeviceFile.safetensors``, plus the index.
@@ -471,6 +473,46 @@ def load_cast_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None)
                 raise ValueError(f"load_cast_boxes converts between {', '.join(map(str, codes))}, not {dt}")
     boxes = [tuple(int(x) for x in b[:6]) + (codes[b[6]], codes[b[7]]) for b in boxes]
     return _load_boxes(ctx, "copy_cast_boxes_from_host", sources, boxes, src)
+
+
+def fp8_dtypes() -> dict:
+    """The FP8 torch dtypes ``load_scaled_boxes`` dequantizes, with their ``_lib.DT_*`` codes."""
+    import torch
+
+    return {torch.float8_e4m3fn: _lib.DT_F8E4M3, torch.float8_e5m2: _lib.DT_F8E5M2}
+
+
+def load_scaled_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> Loaded:
+    """``load_cast_boxes`` for FP8 weights with block scales: box i = ``(index into files, offset, width, rows,
+    src_offset, src_pitch, src_dtype, dst_dtype, scales, first_elem, R, C, block_rows, block_cols)``.  ``src_dtype`` is
+    ``torch.float8_e4m3fn`` or ``torch.float8_e5m2`` (one byte per element, so ``width`` and ``src_pitch`` count both),
+    ``dst_dtype`` one of ``cast_dtypes()``, and ``scales`` a contiguous float32 / float16 / bfloat16 tensor on the
+    context's device holding ``ceil(R / block_rows) * ceil(C / block_cols)`` scales or more, row-major.  Element c of row
+    r of the box is element ``first_elem + r * src_pitch + c`` of an R x C weight W; it lands as
+    ``(W.float() * S_expanded).to(dst_dtype)``, bit for bit torch's result on CUDA (a block of R or more rows, C or more
+    columns, is the whole dimension).  The scales must not change until the copy has completed.  ONE
+    ``b200h_copy_scaled_boxes_from_host`` call, ordered exactly as ``load_boxes``."""
+    import torch
+
+    ctx = ctx or get_context()
+    sources = [f._src for f in files]
+    if any(len(b) != 14 for b in boxes):
+        raise ValueError("a box is (file, offset, width, rows, src_offset, src_pitch, src_dtype, dst_dtype, scales, "
+                         "first_elem, R, C, block_rows, block_cols)")
+    codes, fp8 = cast_dtypes(), fp8_dtypes()
+    out = []
+    for b in boxes:
+        if b[6] not in fp8:
+            raise ValueError(f"load_scaled_boxes dequantizes {', '.join(map(str, fp8))}, not {b[6]}")
+        if b[7] not in codes:
+            raise ValueError(f"load_scaled_boxes converts to {', '.join(map(str, codes))}, not {b[7]}")
+        s = b[8]
+        if not isinstance(s, torch.Tensor) or s.dtype not in codes or not s.is_contiguous():
+            raise ValueError("a box's scales are a contiguous float32, float16 or bfloat16 tensor on the context's "
+                             "device")
+        out.append(tuple(int(x) for x in b[:6]) + (fp8[b[6]], codes[b[7]], s.data_ptr(), codes[s.dtype], s.numel())
+                   + tuple(int(x) for x in b[9:]))
+    return _load_boxes(ctx, "copy_scaled_boxes_from_host", sources, out, src)
 
 
 # ------------------------------------------------------------------------------------------ safetensors
@@ -1222,5 +1264,5 @@ class DeviceFile(io.RawIOBase):
 safetensors_shards = DeviceFile.safetensors_shards
 
 __all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "SafetensorsShards", "Staged", "hash_parts_many", "load_boxes",
-           "load_cast_boxes", "load_ranges", "parse_size_to_int", "safetensors_layout", "safetensors_shards",
+           "load_cast_boxes", "load_scaled_boxes", "load_ranges", "parse_size_to_int", "safetensors_layout", "safetensors_shards",
            "stage_ranges"]

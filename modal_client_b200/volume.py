@@ -41,8 +41,8 @@ from . import _wire, blob_utils, device_file
 from ._logging import logger
 from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
-from .device_file import (BOUNCE_BYTES, DeviceFile, _st_dtypes, cast_targets, load_boxes, load_cast_boxes, load_ranges,
-                          stage_ranges)
+from .device_file import (BOUNCE_BYTES, DeviceFile, _st_dtypes, cast_dtypes, cast_targets, fp8_dtypes, load_boxes,
+                          load_cast_boxes, load_ranges, load_scaled_boxes, stage_ranges)
 from .exception import ExecutionError, ServiceError
 from .http_utils import ClientSessionRegistry
 
@@ -667,13 +667,14 @@ def _check_into(into: Mapping, entries, ctx, sliced: bool = False, stored: Mappi
 
 async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
     """Load ``files`` -- ``(path, runs, dst, start, end)`` each, ``runs`` ``[((F, W, P, R) as _slice_runs gives it,
-    packed offset in dst, (stored dtype, target dtype) or None)]`` -- into their ``dst``: ONE ``VolumeGetFile2`` call per
-    file that has a touched block, over its bytes [start, end), all made concurrently, then exactly the blocks that
-    hold a byte of a run, once each, into the page-locked waves of ONE ``_load_in_waves``, so a wave may hold the blocks
-    of several files.  Each complete wave makes at most one ``load_boxes`` call (the unconverted runs; one also when
-    nothing converts) and at most one ``load_cast_boxes`` call, over every file's ``dst``: every run is cut into boxes,
-    split where the staging stops being contiguous, at a wave's edge, a skipped block or the next file.  A converted
-    run's packed offsets count target bytes."""
+    packed offset in dst, (stored dtype, target dtype), (FP8 dtype, target dtype, _Dequant) or None)]`` -- into their
+    ``dst``: ONE ``VolumeGetFile2`` call per file that has a touched block, over its bytes [start, end), all made
+    concurrently, then exactly the blocks that hold a byte of a run, once each, into the page-locked waves of ONE
+    ``_load_in_waves``, so a wave may hold the blocks of several files.  Each complete wave makes at most one
+    ``load_boxes`` call (the unconverted runs; one also when nothing converts), at most one ``load_cast_boxes`` call
+    and at most one ``load_scaled_boxes`` call (the dequantized runs), all on one stream, over every file's ``dst``:
+    every run is cut into boxes, split where the staging stops being contiguous, at a wave's edge, a skipped block or
+    the next file.  A converted run's packed offsets count target bytes."""
     BS = blob_utils.BLOCK_SIZE
     touched = [_touched_blocks([r for r, _, _ in runs], BS) for _, runs, _, _, _ in files]
     live = [files[k] for k, t in enumerate(touched) if t]
@@ -687,7 +688,7 @@ async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
     dsts = [dst for _, _, dst, _, _ in live]
 
     def load(wave, at, buf, ctx):
-        plain, cast, k = [], [], 0
+        plain, cast, scaled, k = [], [], [], 0
         while k < len(wave):  # a stretch: blocks of one file, adjacent in the file and in the buffer
             e, i = k + 1, wave[k][3]
             while e < len(wave) and wave[e][3] == i and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and \
@@ -699,18 +700,25 @@ async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
                 for b in _clip_run(run, 0, s0, s1, at[k]):
                     if conv is None:
                         plain.append((i, d + b[0], *b[1:]))
-                    else:  # the box's offset in the run, in source bytes, to target bytes
+                    elif len(conv) == 2:  # the box's offset in the run, in source bytes, to target bytes
                         cast.append((i, d + b[0] // conv[0].itemsize * conv[1].itemsize, *b[1:], *conv))
+                    else:  # one-byte elements; the box's first element in the weight, from its file offset
+                        q = conv[2]
+                        scaled.append((i, d + b[0] * conv[1].itemsize, *b[1:], conv[0], conv[1], q.scales,
+                                       s0 + b[3] - at[k] - q.start, q.rows, q.cols, q.block_rows, q.block_cols))
             k = e
-        loaded = load_boxes(dsts, plain, buf, ctx=ctx) if plain or not cast else None
+        loaded = load_boxes(dsts, plain, buf, ctx=ctx) if plain or not (cast or scaled) else None
         if cast:  # on the same stream as the plain boxes: its completion implies theirs
             loaded = load_cast_boxes(dsts, cast, buf, ctx=ctx)
+        if scaled:  # the same stream again
+            loaded = load_scaled_boxes(dsts, scaled, buf, ctx=ctx)
         return loaded
 
     await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
 
 
 async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping | None = None, dtype=None,
+                           scales: Mapping | None = None, scale_block=(128, 128),
                            staging_bytes: int = 256 << 20) -> dict:
     """The safetensors file at ``path`` as ``{name: tensor}`` on the context's device, equal to what
     ``safetensors.torch.load`` gives for the file's bytes (same names, dtypes, shapes and values; keys in data order).
@@ -728,9 +736,27 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
     any data GET (a file not written by ``safetensors.torch.save`` may hold a tensor that cannot convert in place).
     With ``into=`` each tensor must have its target dtype.  When something converts, the same ``VolumeGetFile2`` call
     and block GETs as without ``dtype`` feed the waves of ``_load_runs``: HBM holds only the results, never the stored
-    image; when nothing converts, the call is the one without ``dtype``."""
+    image; when nothing converts, the call is the one without ``dtype``.
+
+    ``scales={weight: scale name}`` (``fp8_scales`` pairs them by name) dequantizes FP8 weights (F8_E4M3, F8_E5M2;
+    2-D, R x C) as they land, to their target from ``dtype`` (the single dtype, or the weight's entry of a mapping; a
+    single dtype still refuses FP8 tensors without a scale).  The scale S (F32, F16 or BF16) holds one value per
+    ``scale_block`` = (rows, columns) block, ``None`` meaning the whole dimension: shape [ceil(R / rows), ceil(C /
+    columns)] ([] or [1] for one block, [ceil(R / rows)] for one block column).  Each result equals, bit for bit, what
+    torch computes on CUDA: ``(W.float() * S.float().repeat_interleave(rows, 0)[:R].repeat_interleave(columns,
+    1)[:, :C]).to(target)``.  Scale tensors are consumed: not in the result, and not allowed in ``into``.
+    ``_scale_targets`` lists every problem in one ``ValueError`` before any data GET.  The scales load first into
+    temporary tensors (one ``_load_runs`` over their blocks), then everything else (a second one, whose waves make at
+    most one ``load_boxes``, one ``load_cast_boxes`` and one ``load_scaled_boxes`` call); HBM holds the results and the
+    scales, never the FP8 image, and the scales are freed on return."""
     ctx = blob_utils.get_context()
     size, n, _, entries = await _read_safetensors_header(client, volume_id, path)
+    if scales:
+        if staging_bytes < 2 * blob_utils.BLOCK_SIZE:
+            raise ValueError(f"staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), got "
+                             f"{staging_bytes}")
+        return await _read_shards(client, volume_id, path, [(path, n, entries)], None, into, dtype, scales,
+                                  scale_block, staging_bytes, ctx)
     targets = cast_targets(path, dtype, entries, 8 + n)
     if targets and staging_bytes < 2 * blob_utils.BLOCK_SIZE:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), got {staging_bytes}")
@@ -891,7 +917,8 @@ def _clip_run(run, dest: int, s0: int, s1: int, at: int):
 
 
 async def read_safetensors_slices(client, volume_id: str, path: str, select: Mapping, *, into: Mapping | None = None,
-                                  dtype=None, staging_bytes: int = 256 << 20) -> dict:
+                                  dtype=None, scales: Mapping | None = None, scale_block=(128, 128),
+                                  staging_bytes: int = 256 << 20) -> dict:
     """Slices of tensors of the safetensors file at ``path``: ``{name: full[index]}`` for every ``name: index`` of
     ``select``, in its order, each a new contiguous tensor on the context's device (``full`` as ``read_safetensors``
     returns it; for these index forms also what ``safe_open(...).get_slice(name)[index]`` gives).  An index is an int
@@ -910,12 +937,17 @@ async def read_safetensors_slices(client, volume_id: str, path: str, select: Map
     and not overlap, every mismatch in one ``ValueError`` before any data GET.  On return and on error, ordering and
     partial content are as for ``read_safetensors``.  ``dtype`` converts the slices as they land, as
     ``read_safetensors`` does (a mapping names selected tensors); each result equals ``full[index].to(dtype)`` bit for
-    bit, and the requests are those of the call without ``dtype``."""
+    bit, and the requests are those of the call without ``dtype``.  ``scales`` and ``scale_block`` dequantize FP8
+    weights as ``read_safetensors`` does; every weight named in ``scales`` must be selected and its scale must not be.
+    A slice takes the scale of each element's place in the full tensor, so it equals ``dequantized_full[index]``."""
     BS = blob_utils.BLOCK_SIZE
     if staging_bytes < 2 * BS:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
     ctx = blob_utils.get_context()
     _, n, _, entries = await _read_safetensors_header(client, volume_id, path)
+    if scales:
+        return await _read_shards(client, volume_id, path, [(path, n, entries)], select, into, dtype, scales,
+                                  scale_block, staging_bytes, ctx)
     by_name = {e[0]: e for e in entries}
     unknown = [name for name in select if name not in by_name]
     if unknown:
@@ -1004,52 +1036,189 @@ async def read_safetensors_index(client, volume_id: str, index_path: str):
 
 
 async def read_safetensors_sharded(client, volume_id: str, index_path: str, *, select: Mapping | None = None,
-                                   into: Mapping | None = None, dtype=None, staging_bytes: int = 256 << 20) -> dict:
+                                   into: Mapping | None = None, dtype=None, scales: Mapping | None = None,
+                                   scale_block=(128, 128), staging_bytes: int = 256 << 20) -> dict:
     """A sharded safetensors checkpoint (the index at ``index_path``, read as ``read_safetensors_index`` reads it) as
     ``{name: tensor}`` on the context's device: what merging ``read_safetensors`` over every shard returns, keys in
     shard order, then data order.  With ``select={name: index}`` it is what ``read_safetensors_slices`` returns for
-    those names instead, in ``select``'s order.  ``into=`` and ``dtype=`` mean what they mean there, with the same
-    messages, every problem in one ``ValueError`` before any data GET.
+    those names instead, in ``select``'s order.  ``into=``, ``dtype=``, ``scales=`` and ``scale_block=`` mean what
+    they mean there, with the same messages, every problem in one ``ValueError`` before any data GET; a weight and its
+    scale may live in different shards.
 
     Every shard's data comes through one wave loop: ONE ``VolumeGetFile2`` call per shard with a touched byte, all
     made concurrently, then every touched block once (untouched blocks of a selection never), the blocks of all shards
     in one sequence of page-locked waves (``staging_bytes`` as in ``read_file_into_device``), so a wave may hold blocks
     of several shards and the pipeline does not drain between shards.  Each complete wave makes at most one
-    ``load_boxes`` and one ``load_cast_boxes`` call, over a ``DeviceFile`` per shard.  Of HBM, the call allocates only
-    the results and the copies' small tables.  Ordering and partial content on return and on error are as for
+    ``load_boxes`` and one ``load_cast_boxes`` call (and with ``scales=`` one ``load_scaled_boxes`` call), over a
+    ``DeviceFile`` per shard.  Of HBM, the call allocates only the results and the copies' small tables (and with
+    ``scales=`` the scales, freed on return).  Ordering and partial content on return and on error are as for
     ``read_safetensors``."""
     BS = blob_utils.BLOCK_SIZE
     if staging_bytes < 2 * BS:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
     ctx = blob_utils.get_context()
     _, shards = await _read_index(client, volume_id, index_path)
+    return await _read_shards(client, volume_id, index_path, shards, select, into, dtype, scales, scale_block,
+                              staging_bytes, ctx)
+
+
+class _Dequant:
+    """How the boxes of one FP8 weight are dequantized: its scales on the device, the file offset of its element 0,
+    its shape and its block (a block of the whole dimension is the dimension)."""
+
+    def __init__(self, scales, start: int, rows: int, cols: int, block_rows: int, block_cols: int):
+        self.scales, self.start, self.rows, self.cols = scales, start, rows, cols
+        self.block_rows, self.block_cols = block_rows, block_cols
+
+
+def _scale_grid(shape, scale_block):
+    """(scale rows, scale columns) of a 2-D weight of ``shape`` in blocks ``scale_block`` (None: the whole dimension)."""
+    return tuple(1 if b is None else -(-d // b) for d, b in zip(shape, scale_block))
+
+
+def fp8_scales(names, suffix: str = "_scale_inv") -> dict:
+    """``{weight: scale}`` for every name ``n`` of ``names`` for which ``n + suffix`` is a name too, in the order of
+    ``names``: the ``scales=`` argument of the ``read_safetensors*`` calls.  ``names`` may be the tensors of
+    ``read_safetensors_header`` or of ``read_safetensors_index``.  DeepSeek-V3/R1 and the Qwen3 FP8 checkpoints store
+    ``<weight>_scale_inv`` (the default); compressed-tensors checkpoints store ``<weight>_scale``."""
+    names = list(names)
+    have = set(names)
+    return {n: n + suffix for n in names if n + suffix in have}
+
+
+def _scale_targets(where: str, there: str, dtype, scales: Mapping, scale_block, tensors: Mapping, select, into) -> dict:
+    """{weight: target dtype} of the FP8 weights of ``scales`` ({weight: scale name}), whose tensors ``tensors`` gives
+    as {name: (torch dtype, shape)} (``there`` names where they are).  Every problem in one ``ValueError``: ``scales``
+    without ``dtype``, a bad ``scale_block``, unknown or unselected weights, missing scales, a weight that is not FP8 or
+    not 2-D, a scale that is not F32 / F16 / BF16 or has the wrong shape for the block, a name that is both a weight
+    and a scale, a scale that is selected or in ``into``, and a missing or unsupported target."""
+    import torch
+
+    if not isinstance(scales, Mapping):
+        raise ValueError(f"{where}: scales must map weight names to scale names, got {type(scales).__name__}")
+    codes, fp8, tags = cast_dtypes(), fp8_dtypes(), _st_dtypes()
+    supported = "float32, float16 or bfloat16"
+    problems = []
+    if dtype is None:
+        problems.append("scales needs dtype= (the dtype the weights are dequantized to)")
+    good_block = isinstance(scale_block, (tuple, list)) and len(scale_block) == 2 and all(
+        b is None or (isinstance(b, int) and not isinstance(b, bool) and b >= 1) for b in scale_block)
+    if not good_block:
+        problems.append(f"scale_block {scale_block!r} is not a pair of ints >= 1 or None")
+    for name in sorted(set(scales) & set(scales.values())):
+        problems.append(f"{name!r} is both a weight and a scale")
+    if isinstance(dtype, Mapping):
+        for name in sorted(set(dtype) & set(scales.values())):
+            problems.append(f"{name!r} is a scale, which is consumed, but dtype names it")
+    out = {}
+    for w, sc in scales.items():
+        if w not in tensors:
+            problems.append(f"weight {w!r} is not {there}")
+        elif select is not None and w not in select:
+            problems.append(f"weight {w!r} is not selected")
+        elif tensors[w][0] not in fp8:
+            problems.append(f"weight {w!r} is {tags[tensors[w][0]][0]}, not F8_E4M3 or F8_E5M2")
+        elif len(tensors[w][1]) != 2:
+            problems.append(f"weight {w!r} has shape {list(tensors[w][1])}, not 2-D")
+        if not isinstance(sc, str) or sc not in tensors:
+            problems.append(f"scale {sc!r} of {w!r} is not {there}")
+            continue
+        sdt, sshape = tensors[sc]
+        if sdt not in codes:
+            problems.append(f"scale {sc!r} is {tags[sdt][0]}, not F32, F16 or BF16")
+        elif good_block and w in tensors and len(tensors[w][1]) == 2:
+            sr, scol = _scale_grid(tensors[w][1], scale_block)
+            fits = [(sr, scol)] + ([(), (1,)] if sr == scol == 1 else [(sr,)] if scol == 1 else [])
+            if tuple(sshape) not in fits:
+                problems.append(f"scale {sc!r} has shape {list(sshape)}; weight {w!r} of shape {list(tensors[w][1])} "
+                                f"in blocks {tuple(scale_block)} needs [{sr}, {scol}]")
+        if select is not None and sc in select:
+            problems.append(f"scale {sc!r} is selected, but scales are consumed")
+        if into is not None and sc in into:
+            problems.append(f"scale {sc!r} is in into, but scales are consumed")
+        target = dtype.get(w) if isinstance(dtype, Mapping) else dtype
+        if isinstance(dtype, Mapping) and target is None:
+            problems.append(f"weight {w!r} has no target in dtype")
+        elif target is not None and (not isinstance(target, torch.dtype) or target not in codes):
+            problems.append(f"weight {w!r}: {target} is not a supported target ({supported})")
+        else:
+            out[w] = target
+    if problems:
+        raise ValueError(f"{where}: scales: " + "; ".join(problems))
+    return out
+
+
+async def _read_shards(client, volume_id: str, where: str, shards, select, into, dtype, scales, scale_block,
+                       staging_bytes: int, ctx) -> dict:
+    """The body of ``read_safetensors_sharded`` over ``shards`` (``[(path, header length, entries)]``; also
+    ``read_safetensors`` and ``read_safetensors_slices`` with ``scales=``, over one shard).  With ``scales``, the scales
+    load first, unconverted, into temporary tensors (one ``_load_runs``: a scale may sit in a later wave, or another
+    shard, than its weight), then everything else (a second ``_load_runs``)."""
     by_name = {e[0]: (k, 8 + n + e[3], e) for k, (_, n, entries) in enumerate(shards) for e in entries}
+    scaled, consumed = {}, set()
+    if scales:
+        there = "in the checkpoint" if len(shards) > 1 else "in the file"
+        scaled = _scale_targets(where, there, dtype, scales, scale_block,
+                                {name: (e[1], e[2]) for name, (_, _, e) in by_name.items()}, select, into)
+        consumed = set(scales.values())
     plans = []  # (shard, name, stored dtype, result shape, runs)
     if select is None:
         for name, (k, at, (_, dt, shape, lo, hi)) in by_name.items():
-            plans.append((k, name, dt, shape, [(at, hi - lo, hi - lo, 1)] if hi > lo else []))
+            if name not in consumed:
+                plans.append((k, name, dt, shape, [(at, hi - lo, hi - lo, 1)] if hi > lo else []))
     else:
         unknown = [name for name in select if name not in by_name]
         if unknown:
-            raise ValueError(f"{index_path}: no tensors named {', '.join(repr(u) for u in unknown)}")
+            raise ValueError(f"{where}: no tensors named {', '.join(repr(u) for u in unknown)}")
         for name, index in select.items():
             k, at, (_, dt, shape, _, _) = by_name[name]
             bounds, kept = _slice_bounds(name, shape, index)
             result = [hi - b for (b, hi), keep in zip(bounds, kept) if keep]
             plans.append((k, name, dt, result, _slice_runs(shape, bounds, dt.itemsize, at)))
     sliced = select is not None
-    targets = cast_targets(index_path, dtype, [(name, dt, shape, by_name[name][1], None)
-                                               for _, name, dt, shape, _ in plans], 0, sliced=sliced)
+    rest = dtype
+    if scaled and isinstance(dtype, Mapping):
+        rest = {name: t for name, t in dtype.items() if name not in scaled}
+    targets = cast_targets(where, rest, [(name, dt, shape, by_name[name][1], None)
+                                         for _, name, dt, shape, _ in plans if name not in scaled], 0, sliced=sliced)
+    targets.update(scaled)
     if into is not None:
         _check_into(into, [(name, targets.get(name, dt), shape, 0, 0) for _, name, dt, shape, _ in plans], ctx,
                     sliced=sliced, stored={name: dt for _, name, dt, *_ in plans if name in targets})
         tensors = [into[name] for _, name, *_ in plans]
     else:
         tensors = [DeviceFile._Source._new_tensor(shape, targets.get(name, dt), ctx) for _, name, dt, shape, _ in plans]
+    dequant = {}
+    if scaled:  # the scales of the weights with a byte to load, whole and unconverted, into temporary tensors
+        needed = sorted({scales[name] for _, name, _, _, rs in plans if name in scaled and rs},
+                        key=lambda sc: (by_name[sc][0], by_name[sc][1]))
+        temps = {sc: DeviceFile._Source._new_tensor(by_name[sc][2][2], by_name[sc][2][1], ctx) for sc in needed}
+        per = {}  # shard -> [its scale tensors, runs, packed bytes so far]
+        for sc in needed:
+            k, at, (_, _, _, lo, hi) = by_name[sc]
+            ts, runs, base = per.setdefault(k, [[], [], 0])
+            if hi > lo:
+                runs.append(((at, hi - lo, hi - lo, 1), base, None))
+            ts.append(temps[sc])
+            per[k][2] = base + hi - lo
+        files = []
+        for k in sorted(per):
+            ts, runs, _ = per[k]
+            if runs:
+                start = min(F for (F, _, _, _), _, _ in runs)
+                end = max(F + W for (F, W, _, _), _, _ in runs)
+                files.append((shards[k][0], runs, DeviceFile._over(DeviceFile._Source(ts, BOUNCE_BYTES)), start, end))
+        await _load_runs(client, volume_id, files, staging_bytes)
+        for w in scaled:
+            if scales[w] in temps:
+                (R, C), (br, bc) = by_name[w][2][2], scale_block
+                dequant[w] = _Dequant(temps[scales[w]], by_name[w][1], R, C, max(1, R if br is None else br),
+                                      max(1, C if bc is None else bc))
     per = {}  # shard -> [its result tensors, runs, packed bytes so far]
     for (k, name, dt, _, rs), t in zip(plans, tensors):
         ts, runs, base = per.setdefault(k, [[], [], 0])
-        dest, conv = base, (dt, t.dtype) if name in targets else None
+        dest = base
+        conv = (dt, t.dtype, dequant[name]) if name in dequant else (dt, t.dtype) if name in targets else None
         for run in rs:
             runs.append((run, dest, conv))
             dest += run[1] * run[3] // dt.itemsize * t.element_size()

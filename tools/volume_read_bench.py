@@ -44,7 +44,18 @@
     host clock, peak HBM growth (torch.cuda.max_memory_allocated) and a bitwise comparison.  The same for rank
     VRB_RANK's TP slices: read_safetensors_slices(dtype=torch.bfloat16) against the slices followed by .to().
 
-VRB_ARMS (default "abcd") picks the arms; "e" is run only when named.
+(f) loading FP8 weights dequantized with 128 x 128 block scales (F8_E4M3 with F32 ``_scale_inv``, to BF16).
+    kernel: one 128 MiB wave (16 blocks of 8 MiB, the data region at 8 mod 16) of a [R, 7168] E4M3 weight as 1-row
+    boxes of one block each: (1) ONE load_scaled_boxes call against (2) ONE load_boxes call of the same FP8 bytes.
+    CUDA events, VRB_REPS runs each, alternating, best and median; the cost of dequantizing over a plain copy.  The
+    result is compared bitwise with torch's CUDA dequantization.
+    end to end over loopback: a seeded, Qwen3/DeepSeek-shaped FP8 stack of VRB_FP8_GIB (2.5) GB exported with
+    safetensors_shards in 1 GB shards and uploaded once; read_safetensors_sharded(dtype=torch.bfloat16,
+    scales=fp8_scales(...)) against read_safetensors_sharded followed by per-weight torch dequantization (what
+    DeepSeek's fp8_cast_bf16.py does), alternating, VRB_FP8_REPS (3) runs each: host clock, peak HBM growth
+    (torch.cuda.max_memory_allocated) and a bitwise comparison.
+
+VRB_ARMS (default "abcd") picks the arms; "e" and "f" are run only when named.
 
 The card name and power limit are read in the same run.  Needs a GPU: nothing here falls back.
 One JSON line per arm; also written to $VRB_OUT/volume_read_bench.json when set."""
@@ -628,6 +639,131 @@ async def cast_e2e_arm(info, out):
         print(json.dumps(out[-1]), flush=True)
 
 
+def _dequant_bf16(w, s):
+    """torch's CUDA dequantization of an E4M3 weight with 128 x 128 block scales, to bfloat16."""
+    R, C = w.shape
+    full = s.repeat_interleave(128, 0)[:R].repeat_interleave(128, 1)[:, :C]
+    return (w.float() * full).to(torch.bfloat16)
+
+
+def fp8_kernel_arm(ctx, info, out):
+    from modal_client_b200 import load_boxes, load_scaled_boxes
+
+    BS, C, phase = blob_utils.BLOCK_SIZE, 7168, 8
+    n = 16 * BS
+    R = (n - phase) // C
+    g = torch.Generator(device="cuda").manual_seed(9)
+    w = (torch.randn(R, C, generator=g, device="cuda") * 50).to(torch.float8_e4m3fn)
+    s = torch.rand(-(-R // 128), C // 128, generator=g, device="cuda") * 1e-3
+    src = ctx.host_alloc(n + 16)
+    try:
+        src[phase : phase + R * C] = w.view(torch.uint8).reshape(-1).cpu().numpy()
+        nbytes = R * C
+        blocks = [(max(phase, o), min(o + BS, phase + nbytes) - max(phase, o)) for o in range(0, n, BS)]
+        blocks = [(a, m) for a, m in blocks if m > 0]
+        plain = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+        res = torch.empty(R, C, dtype=torch.bfloat16, device="cuda")
+        fp, fr = DeviceFile(plain), DeviceFile(res)
+        plain_boxes = [(0, a - phase, m, 1, a, m) for a, m in blocks]
+        scaled_boxes = [(0, (a - phase) * 2, m, 1, a, m, torch.float8_e4m3fn, torch.bfloat16, s, a - phase, R, C, 128, 128)
+                        for a, m in blocks]
+        cands = {"load_scaled_boxes": lambda: load_scaled_boxes([fr], scaled_boxes, src, ctx=ctx),
+                 "load_boxes": lambda: load_boxes([fp], plain_boxes, src, ctx=ctx)}
+        for fn in cands.values():
+            fn()
+        times = {k: [] for k in cands}
+        for _ in range(int(os.environ.get("VRB_REPS", "5"))):
+            for k, fn in cands.items():
+                times[k].append(events_ms(fn))
+        torch.cuda.synchronize()
+        equal = torch.equal(res.view(torch.int16), _dequant_bf16(w, s).view(torch.int16)) and \
+            torch.equal(plain, w.view(torch.uint8).reshape(-1))
+        best = {k: min(v) for k, v in times.items()}
+        for k, v in times.items():
+            out.append({"arm": f"fp8_kernel.e4m3_to_bf16.{k}", "source_bytes": nbytes, "boxes": len(blocks),
+                        "best_ms": round(best[k], 3), "median_ms": round(statistics.median(v), 3),
+                        "GB_s": round(nbytes / best[k] / 1e6, 2),
+                        "share_of_load_boxes": round(best["load_boxes"] / best[k], 3), "bitwise_equal": equal, **info})
+            print(json.dumps(out[-1]), flush=True)
+        del fp, fr, plain, res
+    finally:
+        torch.cuda.synchronize()
+        ctx.host_free(src)
+
+
+def fp8_stack(total: int, h: int = 4096, m: int = 12288) -> dict:
+    """Qwen3/DeepSeek-shaped E4M3 layers (q, kv_a with 576 rows, o, gate, up, down) with F32 128 x 128
+    ``weight_scale_inv`` tensors and BF16 norms, about ``total`` bytes."""
+    shapes = {"self_attn.q_proj": (h, h), "self_attn.kv_a_proj": (576, h), "self_attn.o_proj": (h, h),
+              "mlp.gate_proj": (m, h), "mlp.up_proj": (m, h), "mlp.down_proj": (h, m)}
+    per = sum(r * c for r, c in shapes.values())
+    g = torch.Generator(device="cuda").manual_seed(10)
+    sd = {}
+    for i in range(max(1, total // per)):
+        p = f"model.layers.{i}."
+        for k, (r, c) in shapes.items():
+            sd[p + k + ".weight"] = (torch.randn(r, c, generator=g, device="cuda") * 50).to(torch.float8_e4m3fn)
+            sd[p + k + ".weight_scale_inv"] = torch.rand(-(-r // 128), -(-c // 128), generator=g, device="cuda") * 1e-3
+        sd[p + "input_layernorm.weight"] = torch.randn(h, generator=g, device="cuda").to(torch.bfloat16)
+    return sd
+
+
+async def fp8_e2e_arm(info, out):
+    from modal_client_b200 import device_file
+
+    BS = blob_utils.BLOCK_SIZE
+    sd = fp8_stack(int(float(os.environ.get("VRB_FP8_GIB", "2.5")) * 1e9))
+    size = sum(t.numel() * t.element_size() for t in sd.values())
+    index = "/fp8/model.safetensors.index.json"
+    rows = {}
+    async with running_volume_server(BS) as (stub, _):
+        client = types.SimpleNamespace(stub=stub)
+        shards = device_file.safetensors_shards(sd, max_shard_size="1GB")
+        nshards = len(shards.files)
+        async with volume.VolumeUploadContextManager2("vo-f", client) as batch:
+            shards.put(batch, "/fp8")
+        del shards, sd
+        _, where = await volume.read_safetensors_index(client, "vo-f", index)
+        scales = volume.fp8_scales(where)
+
+        async def read(fused: bool):
+            if fused:
+                return await volume.read_safetensors_sharded(client, "vo-f", index, dtype=torch.bfloat16,
+                                                             scales=scales)
+            res = await volume.read_safetensors_sharded(client, "vo-f", index)
+            for w, sc in scales.items():
+                res[w] = _dequant_bf16(res[w], res.pop(sc))
+            return res
+
+        for rep in range(int(os.environ.get("VRB_FP8_REPS", "3"))):
+            results = {}
+            order = (True, False) if rep % 2 == 0 else (False, True)
+            for fused in order:
+                route = "dtype_bf16_scales" if fused else "read_then_torch_dequant"
+                torch.cuda.synchronize()
+                hbm = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                t0 = time.perf_counter()
+                res = await read(fused)
+                torch.cuda.synchronize()
+                rows.setdefault(route, []).append([time.perf_counter() - t0,
+                                                   torch.cuda.max_memory_allocated() - hbm])
+                results[fused] = res
+            equal = sorted(results[True]) == sorted(results[False]) and all(
+                torch.equal(results[True][k].view(torch.int16), results[False][k].view(torch.int16))
+                for k in results[True])
+            for route in rows:
+                rows[route][-1].append(equal)
+            del results
+    for route, v in rows.items():
+        ts = [x[0] for x in v]
+        out.append({"arm": f"fp8_loopback.{route}", "file_bytes": size, "shards": nshards,
+                    "median_s": round(statistics.median(ts), 3), "range_s": [round(min(ts), 3), round(max(ts), 3)],
+                    "peak_hbm_growth_GB": round(max(x[1] for x in v) / 1e9, 3),
+                    "bitwise_equal": all(x[2] for x in v), **info})
+        print(json.dumps(out[-1]), flush=True)
+
+
 def main():
     if not torch.cuda.is_available():
         raise SystemExit("volume_read_bench needs a GPU")
@@ -647,6 +783,9 @@ def main():
     if "e" in arms:
         cast_kernel_arm(ctx, info, out)
         asyncio.run(cast_e2e_arm(info, out))
+    if "f" in arms:
+        fp8_kernel_arm(ctx, info, out)
+        asyncio.run(fp8_e2e_arm(info, out))
     if os.environ.get("VRB_OUT"):
         os.makedirs(os.environ["VRB_OUT"], exist_ok=True)
         with open(os.path.join(os.environ["VRB_OUT"], "volume_read_bench.json"), "w") as fh:
