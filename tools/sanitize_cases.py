@@ -18,6 +18,9 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
                ranges at odd image offsets into page-locked host memory and into device memory
   gather       gather_segments_kernel (b200h_hash_segment_parts_device): segments that are exact-size allocations,
                parts that straddle them at every relative phase, and parts hashed in place
+  scaled boxes load_scaled_boxes_kernel: FP8 boxes of every format, target and scale type, each scale tensor an
+               exact-size allocation with partial last blocks; the last box reads the last element, source byte and
+               scale, checked against the integer-exact reference of tests/test_fp8_reference_cpu.py
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -225,5 +228,54 @@ for part_len in (64, 1000, 4096):
             assert md5[row].tobytes() == hashlib.md5(m).digest(), (part_len, row)
             row += 1
 print("segment parts gather ok", flush=True)
+
+# 11. load_scaled_boxes_kernel: FP8 boxes dequantized with block scales, for every format x target x scale type; each
+#     scale tensor an exact-size allocation of ceil(R / br) * ceil(C / bc) elements whose last block is partial in both
+#     dimensions, each destination an exact-size allocation; the boxes take the fast path, the element loop and rows
+#     across tensor-row edges; the last box reads its tensor's last element, the source's last byte and the last scale
+from tests.test_cast_reference_cpu import is_nan_bits
+from tests.test_fp8_reference_cpu import NAN, reference_dequant
+
+names[_lib.DT_F8E4M3], names[_lib.DT_F8E5M2] = torch.float8_e4m3fn, torch.float8_e5m2
+src = ctx.host_alloc(1 << 20)
+src[:] = synth_array(11, 1 << 20)
+g = torch.Generator().manual_seed(11)
+combos = [(fc, tc, sc) for fc in (_lib.DT_F8E4M3, _lib.DT_F8E5M2) for tc in (_lib.DT_BF16, _lib.DT_F16, _lib.DT_F32)
+          for sc in (_lib.DT_F32, _lib.DT_F16, _lib.DT_BF16)]
+boxes, outs, meta, at = [], [], [], 0
+for k, (fc, tc, sc) in enumerate(combos):
+    br, bc = 8, 5 + k % 4
+    R, C = 37 + 2 * k, bc * (9 + k) + 1 + k % 3  # partial last blocks: R % br and C % bc are not 0
+    assert R % br and C % bc
+    nscales = -(-R // br) * -(-C // bc)
+    scales = ((torch.rand(nscales, generator=g) * 4 - 2) * 2.0 ** torch.randint(-10, 10, (nscales,), generator=g)).to(
+        names[sc]).cuda()
+    first, rows, width, pitch = [(0, 1, R * C, R * C), (C + 1, R - 2, C - 3, C), (5, R - 1, 3, C + 1),
+                                 (C - 7, 4, 20, 2 * C)][k % 4]
+    if k == len(combos) - 1:  # the last box ends at the tensor's last element, which is the source's last byte
+        first, rows, width, pitch = R * C - 1 - 2 * (C + 2) - 30 + 1, 3, 30, C + 2
+        at = src.size - R * C
+    at = -(-at // 16) * 16 + k % 16 if k < len(combos) - 1 else at
+    outs.append(torch.empty(rows * width * names[tc].itemsize, dtype=torch.uint8, device="cuda"))
+    boxes.append((len(outs) - 1, 0, width, rows, at + first, pitch, fc, tc, scales.data_ptr(), sc, nscales, first, R,
+                  C, br, bc))
+    meta.append((at, scales, R, C, br, bc))
+    at += R * C
+assert boxes[-1][4] + (boxes[-1][3] - 1) * boxes[-1][5] + boxes[-1][2] == src.size
+ctx.copy_scaled_boxes_from_host([t.data_ptr() for t in outs], [t.numel() for t in outs], list(range(len(outs) + 1)),
+                                boxes, src)
+torch.cuda.synchronize()
+for (_, _, width, rows, s_at, pitch, fc, tc, _, sc, _, first, R, C, br, bc), (at, scales, *_), t in zip(boxes, meta,
+                                                                                                      outs):
+    e = first + (torch.arange(rows)[:, None] * pitch + torch.arange(width)[None, :]).reshape(-1)
+    w_bits = torch.from_numpy(src[at : at + R * C].copy()).to(torch.int64)[e]
+    s_bits = scales.cpu().view(torch.int32 if sc == _lib.DT_F32 else torch.int16).to(torch.int64)
+    ref = reference_dequant(w_bits, names[fc], s_bits[e // C // br * -(-C // bc) + e % C // bc], names[sc], names[tc])
+    got = t.cpu().view(torch.int32 if tc == _lib.DT_F32 else torch.int16).to(torch.int64) & \
+        ((1 << (8 * names[tc].itemsize)) - 1)
+    nan = ref == NAN
+    assert torch.equal(got[~nan], ref[~nan]) and bool(is_nan_bits(got[nan], names[tc]).all()), (fc, tc, sc, R, C)
+ctx.host_free(src)
+print("scaled boxes ok", flush=True)
 ctx.close()
 print("ALL OK")
