@@ -375,6 +375,75 @@ int b200h_hash_cast_segment_parts_device(b200h_ctx* ctx, const b200h_cast_segmen
                                          uint32_t flags, void* d_sha256, void* d_md5, uint64_t* d_trimmed_len,
                                          uint64_t* nparts_out, void* cuda_stream);
 
+/* ---- FP8 export: block scales and quantizing copies ---------------------------------------------------------------
+ *
+ * A 2-D weight W (R x C, row-major, F32 / F16 / BF16) is quantized to B200H_DT_F8E4M3 per block of block_rows x
+ * block_cols elements (edge blocks are smaller; a block size of R or more, C or more, is the whole dimension), as the
+ * widely copied per_block_cast_to_fp8 does it on CUDA in torch:
+ *   a = NaN if the block holds a NaN, else max(amax |x|, 1e-4f)     (the clamped amax; torch's clamp propagates NaN)
+ *   s = a * RN(1 / 448)                                               (the F32 scale stored next to the weight)
+ *   m = RN(RN(1 / a) * 448)                                           (the multiplier: from a, never from s)
+ *   q = E4M3(RN(float(x) * m))                                        (round to nearest even, subnormals kept)
+ * A block holding an infinity has s = inf and m = 0: its finite elements give +-0, its infinities (inf * 0) NaN. */
+
+/* One weight of b200h_fp8_block_scales.  s and a hold ceil(R / block_rows) x ceil(C / block_cols) F32 values each,
+ * row-major: d_scales receives s (the weight's scale tensor), d_amax receives a (kept for the quantizing copies). */
+typedef struct b200h_fp8_scale_job {
+    const void* d_src;
+    uint64_t src_type; /* B200H_DT_F32, F16 or BF16 */
+    uint64_t rows, cols;
+    uint64_t block_rows, block_cols;
+    float* d_scales;
+    float* d_amax;
+} b200h_fp8_scale_job;
+
+/* s and a of every job (see above), computed on the device.  The amax is an integer max over the bits of |x| widened
+ * to F32 (monotone for non-negative floats, and a NaN wins), reduced per warp and CTA, with one atomicMax per CTA per
+ * block, so a per-channel or per-tensor block is spread over many CTAs.  Any R, C and block sizes; d_src need only be
+ * aligned to its element size.
+ * Every argument is checked before anything is enqueued, B200H_E_INVALID otherwise: a known src_type, R and C >= 1, block
+ * sizes >= 1, d_src aligned to its element size and its R * C elements device memory of ctx's device, d_scales and d_amax
+ * 4-byte aligned device memory of ctx's device, and no two jobs' d_amax arrays overlapping.
+ * Enqueues on `cuda_stream` (NULL = the context's compute stream), whatever njobs is: one cudaMemsetAsync per
+ * contiguous run of the jobs' d_amax arrays (one when they lie back to back), then two kernel launches (the amax
+ * reduction, then the finalisation of a and s); it never synchronises.
+ * Replaces: per_block_cast_to_fp8's padding, abs, amax and division in torch per weight, which allocates F32
+ * temporaries of 4x the weight. */
+int b200h_fp8_block_scales(b200h_ctx* ctx, const b200h_fp8_scale_job* jobs, uint64_t njobs, void* cuda_stream);
+
+/* A segment of a file that may quantize: `cast` as in b200h_cast_segment, or, with cast.dst_type B200H_DT_F8E4M3, the
+ * R x C weight at cast.d_ptr (cast.src_type F32, F16 or BF16, cast.len == R * C * its element size) quantized with the
+ * clamped amax values a at d_amax (scale_count F32 values, ceil(R / block_rows) x ceil(C / block_cols) of them used,
+ * row-major; what b200h_fp8_block_scales left there): the segment's image is the R * C one-byte elements q. */
+typedef struct b200h_scaled_segment {
+    b200h_cast_segment cast;
+    const float* d_amax;
+    uint64_t scale_count;
+    uint64_t rows, cols;
+    uint64_t block_rows, block_cols;
+} b200h_scaled_segment;
+
+/* b200h_copy_cast_ranges over files made of scaled segments: quantizing segments give q (see above), the others what
+ * they give there.  Every rule of b200h_copy_cast_ranges applies to the cast segments, and for a quantizing segment:
+ * src_type F32, F16 or BF16; len == R * C * its element size; block sizes >= 1; scale_count >= ceil(R / block_rows) *
+ * ceil(C / block_cols); d_amax 4-byte aligned device memory of ctx's device.  Everything is checked before anything is
+ * enqueued (B200H_E_INVALID).  ONE kernel launch (stage_scaled_ranges_kernel) per call, none when every range is empty;
+ * only enqueues, as b200h_copy_cast_ranges.  The cast entries keep refusing the FP8 codes.
+ * Replaces: safetensors.torch.save of the quantized dict followed by the reads of _put_missing_blocks
+ * (py/modal/volume.py:1500-1574), which holds a quantized copy of every weight in memory at once. */
+int b200h_copy_scaled_ranges(b200h_ctx* ctx, const b200h_scaled_segment* segs, uint64_t nsegs,
+                             const uint64_t* file_first_seg, uint64_t nfiles, const b200h_file_range* ranges,
+                             uint64_t nranges, void* dst, uint64_t dst_bytes, const uint64_t* dst_offsets,
+                             void* cuda_stream);
+
+/* b200h_hash_cast_segment_parts_device over files made of scaled segments (the rules of b200h_copy_scaled_ranges for
+ * them): a part that touches a quantizing or converting segment is gathered into a wave slot by
+ * stage_scaled_ranges_kernel (one launch per wave), so the quantized bytes never exist in HBM outside the wave slots. */
+int b200h_hash_scaled_segment_parts_device(b200h_ctx* ctx, const b200h_scaled_segment* segs, uint64_t nsegs,
+                                           const uint64_t* file_first_seg, uint64_t nfiles, uint64_t part_len,
+                                           uint32_t flags, void* d_sha256, void* d_md5, uint64_t* d_trimmed_len,
+                                           uint64_t* nparts_out, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.
@@ -458,6 +527,11 @@ int b200h_segment_parts_preview(const uint64_t* seg_lens, uint64_t nsegs, const 
 int b200h_cast_segment_parts_preview(const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
                                      uint64_t nfiles, uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out,
                                      uint64_t* nwaves_out, uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap);
+/* The same for b200h_hash_scaled_segment_parts_device: segments as b200h_scaled_segment (their pointers unused, every
+ * other rule checked). */
+int b200h_scaled_segment_parts_preview(const b200h_scaled_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                       uint64_t nfiles, uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out,
+                                       uint64_t* nwaves_out, uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap);
 /* Kernels launched by this context so far (all kinds). */
 uint64_t b200h_launch_count(b200h_ctx* ctx);
 /* Combining queue of b200h_hash_batch_host: GPU batches issued for, and caller requests served by, the small-request

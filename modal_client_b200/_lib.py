@@ -24,7 +24,7 @@ TRIM_ZEROS = 4
 HEX_OUT = 32  # digest outputs as lowercase ASCII hex rows (64 / 32 chars), formatted on the device
 NO_OUTLIERS = 16  # keep every message on the lane kernel: device batches then only enqueue (include/b200hash.h)
 DT_F32, DT_F16, DT_BF16 = 1, 2, 3  # element types of copy_cast_boxes_from_host (B200H_DT_*)
-DT_F8E4M3, DT_F8E5M2 = 4, 5  # FP8 source types of copy_scaled_boxes_from_host only
+DT_F8E4M3, DT_F8E5M2 = 4, 5  # FP8 types: sources of copy_scaled_boxes_from_host, E4M3 the target of scaled segments
 
 #: every symbol include/b200hash.h declares (tests check the .so exports all of them)
 ABI_SYMBOLS = (
@@ -38,7 +38,8 @@ ABI_SYMBOLS = (
     "b200h_hash_fixed_parts_device", "b200h_hash_segment_parts_device", "b200h_segment_parts_preview",
     "b200h_crc32_device", "b200h_copy_ranges_to_host", "b200h_copy_ranges_from_host", "b200h_copy_boxes_from_host",
     "b200h_copy_cast_boxes_from_host", "b200h_copy_cast_ranges", "b200h_hash_cast_segment_parts_device",
-    "b200h_cast_segment_parts_preview", "b200h_copy_scaled_boxes_from_host",
+    "b200h_cast_segment_parts_preview", "b200h_copy_scaled_boxes_from_host", "b200h_fp8_block_scales",
+    "b200h_copy_scaled_ranges", "b200h_hash_scaled_segment_parts_device", "b200h_scaled_segment_parts_preview",
 )
 
 
@@ -132,6 +133,16 @@ def load_library() -> ctypes.CDLL:
         L.b200h_cast_segment_parts_preview.argtypes = [vp, u64, vp, u64, u64, u64, ctypes.POINTER(u64),
                                                        ctypes.POINTER(u64), vp, vp, u64]
         L.b200h_cast_segment_parts_preview.restype = i32
+        L.b200h_fp8_block_scales.argtypes = [vp, vp, u64, vp]
+        L.b200h_fp8_block_scales.restype = i32
+        L.b200h_copy_scaled_ranges.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
+        L.b200h_copy_scaled_ranges.restype = i32
+        L.b200h_hash_scaled_segment_parts_device.argtypes = [vp, vp, u64, vp, u64, u64, u32, vp, vp, vp,
+                                                             ctypes.POINTER(u64), vp]
+        L.b200h_hash_scaled_segment_parts_device.restype = i32
+        L.b200h_scaled_segment_parts_preview.argtypes = [vp, u64, vp, u64, u64, u64, ctypes.POINTER(u64),
+                                                         ctypes.POINTER(u64), vp, vp, u64]
+        L.b200h_scaled_segment_parts_preview.restype = i32
         L.b200h_stat_files.argtypes = [vp, vp, u64, vp, vp]
         L.b200h_stat_files.restype = i32
         L.b200h_hash_files.argtypes = [vp, vp, u64, vp, u64, u32, vp, vp, vp]
@@ -252,6 +263,16 @@ def cast_segment_parts_preview(seg_lens, src_types, dst_types, file_first_seg, p
                     part_len, wave_bytes)
 
 
+def scaled_segment_parts_preview(seg_lens, src_types, dst_types, scales, file_first_seg, part_len: int,
+                                 wave_bytes: int):
+    """``cast_segment_parts_preview`` for ``Context.hash_scaled_segment_parts_device``: ``scales`` gives every segment's
+    ``(amax_ptr, scale_count, R, C, block_rows, block_cols)`` (zeros for one that does not quantize).  The library's
+    own host code and argument rules (d_amax unchecked); no GPU."""
+    segs = _scaled_segments(np.zeros(len(seg_lens), np.uint64), seg_lens, src_types, dst_types, scales)
+    return _preview("b200h_scaled_segment_parts_preview", _np_ptr(segs) if len(segs) else None, len(segs),
+                    file_first_seg, part_len, wave_bytes)
+
+
 def _preview(entry: str, segs, nsegs: int, file_first_seg, part_len: int, wave_bytes: int):
     fn = getattr(load_library(), entry)
     ffs, nfiles = _segment_args(file_first_seg)
@@ -275,6 +296,18 @@ def _cast_segments(ptrs, lens, src_types, dst_types) -> np.ndarray:
         if t.shape != (len(segs),):
             raise ValueError("src_types and dst_types need one entry per segment")
         segs[:, col] = t
+    return segs
+
+
+def _scaled_segments(ptrs, lens, src_types, dst_types, scales) -> np.ndarray:
+    """The b200h_scaled_segment {cast segment, d_amax, scale_count, rows, cols, block_rows, block_cols} array, as
+    uint64[n, 10]."""
+    segs = np.zeros((len(lens), 10), np.uint64)
+    segs[:, :4] = _cast_segments(ptrs, lens, src_types, dst_types)
+    sc = np.ascontiguousarray(scales, dtype=np.uint64).reshape(-1, 6)
+    if len(sc) != len(segs):
+        raise ValueError("scales needs one (amax_ptr, scale_count, R, C, block_rows, block_cols) per segment")
+    segs[:, 4:] = sc
     return segs
 
 
@@ -491,6 +524,32 @@ class Context:
         self._check(rc, "b200h_hash_cast_segment_parts_device")
         return int(got.value)
 
+    def hash_scaled_segment_parts_device(self, seg_ptrs, seg_lens, src_types, dst_types, scales, file_first_seg,
+                                         part_len: int, flags: int, d_sha: int = 0, d_md5: int = 0,
+                                         d_trimmed: int = 0, stream: int = 0) -> int:
+        """``hash_cast_segment_parts_device`` whose segments may quantize: a segment with dst_types[s] ``DT_F8E4M3``
+        is the R x C weight at seg_ptrs[s] quantized with the clamped amax values of ``scales[s]`` = ``(amax_ptr,
+        scale_count, R, C, block_rows, block_cols)`` (what ``fp8_block_scales`` left there; zeros for the other
+        segments).  Returns the row count."""
+        segs = _scaled_segments(seg_ptrs, seg_lens, src_types, dst_types, scales)
+        ffs, nfiles = _segment_args(file_first_seg)
+        got = ctypes.c_uint64()
+        rc = self._L.b200h_hash_scaled_segment_parts_device(self._h, _np_ptr(segs) if len(segs) else None, len(segs),
+                                                            _np_ptr(ffs), nfiles, part_len, flags, d_sha or None,
+                                                            d_md5 or None, d_trimmed or None, ctypes.byref(got),
+                                                            stream or None)
+        self._check(rc, "b200h_hash_scaled_segment_parts_device")
+        return int(got.value)
+
+    def fp8_block_scales(self, jobs, stream: int = 0) -> None:
+        """The FP8 E4M3 block scales of 2-D weights on the device: job i = ``(src_ptr, src_type, R, C, block_rows,
+        block_cols, scales_ptr, amax_ptr)`` (``DT_F32`` / ``DT_F16`` / ``DT_BF16``) writes s = a / 448 (F32, one per
+        block, row-major) at ``scales_ptr`` and the clamped amax a at ``amax_ptr``.  One memset per contiguous run of
+        the amax arrays and two kernel launches whatever the number of jobs, only enqueued on ``stream``."""
+        jb = np.ascontiguousarray(jobs, dtype=np.uint64).reshape(-1, 8)
+        rc = self._L.b200h_fp8_block_scales(self._h, _np_ptr(jb) if len(jb) else None, len(jb), stream or None)
+        self._check(rc, "b200h_fp8_block_scales")
+
     def crc32_device(self, ptrs, lens, d_out: int, stream: int = 0) -> None:
         """zlib.crc32 of every device range (lens[i] bytes at device address ptrs[i]) into the device uint32 array at
         ``d_out``, computed on the device; the work is only enqueued on ``stream``."""
@@ -526,6 +585,22 @@ class Context:
                                             nfiles, _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(addr),
                                             nbytes, _np_ptr(offs) if len(rg) else None, stream or None)
         self._check(rc, "b200h_copy_cast_ranges")
+
+    def copy_scaled_ranges(self, seg_ptrs, seg_lens, src_types, dst_types, scales, file_first_seg, ranges, dst,
+                           dst_offsets, stream: int = 0) -> None:
+        """``copy_cast_ranges`` whose segments may quantize (segments as for ``hash_scaled_segment_parts_device``).  One
+        kernel launch, only enqueued on ``stream``."""
+        segs = _scaled_segments(seg_ptrs, seg_lens, src_types, dst_types, scales)
+        ffs, nfiles = _segment_args(file_first_seg)
+        rg = np.ascontiguousarray(ranges, dtype=np.uint64).reshape(-1, 3)
+        offs = np.ascontiguousarray(dst_offsets, dtype=np.uint64)
+        if offs.shape != (len(rg),):
+            raise ValueError("dst_offsets needs one entry per range")
+        addr, nbytes = _dst_buffer(dst)
+        rc = self._L.b200h_copy_scaled_ranges(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs),
+                                              nfiles, _np_ptr(rg) if len(rg) else None, len(rg), ctypes.c_void_p(addr),
+                                              nbytes, _np_ptr(offs) if len(rg) else None, stream or None)
+        self._check(rc, "b200h_copy_scaled_ranges")
 
     def copy_ranges_from_host(self, seg_ptrs, seg_lens, file_first_seg, ranges, src: np.ndarray, src_offsets,
                               stream: int = 0) -> None:

@@ -844,23 +844,29 @@ static uint64_t dt_bytes(uint64_t t) {
     return t == B200H_DT_F32 ? 4 : t == B200H_DT_F16 || t == B200H_DT_BF16 ? 2 : 0;
 }
 
+// Bytes of one image element of a segment's destination type: dt_bytes, or 1 for B200H_DT_F8E4M3 (scaled segments).
+static uint64_t image_bytes(uint64_t t) { return t == B200H_DT_F8E4M3 ? 1 : dt_bytes(t); }
+
 static bool converts(const b200h_cast_segment& c) { return c.src_type != c.dst_type; }
 static const b200h_cast_segment kNoSegment{};  // what the cast entries pass as their segments when nsegs == 0
+static const b200h_scaled_segment kNoScaled{};  // and the scaled entries
 
 // The file table of cast segments (file_table over their image lengths, which `seg_lens` receives) and their source
 // ranges as plain segments in `plain` (for segments_on_device).  Checks every rule of a cast segment: known type codes
 // (equal codes are 0 or a B200H_DT_* code), a converting segment's length and, with check_ptrs, its address multiples
-// of the source element size, and its image offset in its file a multiple of the destination element size.
+// of the source element size, and its image offset in its file a multiple of the destination element size.  With
+// fp8_ok (scaled segments), B200H_DT_F8E4M3 is a destination type of one byte per element.
 static int cast_file_table(const b200h_cast_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
                            uint64_t nfiles, bool check_ptrs, std::vector<uint64_t>& seg_lens,
-                           std::vector<b200h_segment>& plain, FileTable& t, std::string& err) {
+                           std::vector<b200h_segment>& plain, FileTable& t, std::string& err, bool fp8_ok = false) {
     if (nsegs && !segs) return err = "segments must not be NULL", B200H_E_INVALID;
     seg_lens.assign(nsegs, 0);
     plain.assign(nsegs, b200h_segment{nullptr, 0});
     for (uint64_t s = 0; s < nsegs; ++s) {
         const b200h_cast_segment& c = segs[s];
         const std::string name = "segment " + std::to_string(s);
-        const uint64_t ss = dt_bytes(c.src_type), ds = dt_bytes(c.dst_type);
+        const uint64_t ss = dt_bytes(c.src_type),
+                       ds = fp8_ok && c.dst_type == B200H_DT_F8E4M3 ? 1 : dt_bytes(c.dst_type);
         plain[s] = {c.d_ptr, c.len};
         seg_lens[s] = c.len;
         if (!converts(c)) {
@@ -876,10 +882,37 @@ static int cast_file_table(const b200h_cast_segment* segs, uint64_t nsegs, const
     }
     if (int rc = file_table(segs ? seg_lens.data() : nullptr, nsegs, file_first_seg, nfiles, t, err)) return rc;
     for (uint64_t s = 0; s < nsegs; ++s)
-        if (converts(segs[s]) && t.seg_start[s] % dt_bytes(segs[s].dst_type))
+        if (converts(segs[s]) && t.seg_start[s] % image_bytes(segs[s].dst_type))
             return err = "segment " + std::to_string(s) + ": its image starts at file offset " +
                          std::to_string(t.seg_start[s]) + ", not a multiple of the destination element size",
                    B200H_E_INVALID;
+    return 0;
+}
+
+// The casts of scaled segments (what cast_file_table checks, with fp8_ok), after the rules of a quantizing segment
+// (dst_type B200H_DT_F8E4M3) that need no device: its source type, len == R * C * ss, block sizes >= 1, the scale count,
+// and with check_ptrs d_amax 4-byte aligned and not NULL.
+static int scaled_casts(const b200h_scaled_segment* segs, uint64_t nsegs, bool check_ptrs,
+                        std::vector<b200h_cast_segment>& casts, std::string& err) {
+    if (nsegs && !segs) return err = "segments must not be NULL", B200H_E_INVALID;
+    casts.resize(nsegs);
+    for (uint64_t s = 0; s < nsegs; ++s) {
+        const b200h_scaled_segment& x = segs[s];
+        casts[s] = x.cast;
+        if (x.cast.dst_type != B200H_DT_F8E4M3 || !converts(x.cast)) continue;
+        const std::string name = "segment " + std::to_string(s);
+        const uint64_t ss = dt_bytes(x.cast.src_type);
+        if (!ss) return err = name + ": only F32, F16 and BF16 sources quantize", B200H_E_INVALID;
+        if (!x.block_rows || !x.block_cols) return err = name + ": block sizes must be >= 1", B200H_E_INVALID;
+        if ((unsigned __int128)x.rows * x.cols * ss != x.cast.len)
+            return err = name + ": len is not R * C * (source element size)", B200H_E_INVALID;
+        const unsigned __int128 nscales = (unsigned __int128)(x.rows / x.block_rows + (x.rows % x.block_rows != 0)) *
+                                          (x.cols / x.block_cols + (x.cols % x.block_cols != 0));
+        if (nscales > x.scale_count)
+            return err = name + ": scale_count is less than ceil(R / block_rows) * ceil(C / block_cols)", B200H_E_INVALID;
+        if (check_ptrs && (!x.d_amax || (uintptr_t)x.d_amax % 4))
+            return err = name + ": d_amax is NULL or not 4-byte aligned", B200H_E_INVALID;
+    }
     return 0;
 }
 
@@ -978,6 +1011,19 @@ int segments_on_device(b200h_ctx* ctx, const b200h_segment* segs, uint64_t n, co
     return 0;
 }
 
+// The amax arrays of the quantizing segments among segs[0 .. n), checked as segments_on_device checks segments.
+static int scales_on_device(b200h_ctx* ctx, const b200h_scaled_segment* segs, uint64_t n) {
+    for (uint64_t i = 0; i < n; ++i) {
+        const b200h_scaled_segment& x = segs[i];
+        if (x.cast.dst_type != B200H_DT_F8E4M3 || !converts(x.cast)) continue;
+        if (x.scale_count > ~0ull / 4 || (uintptr_t)x.d_amax + x.scale_count * 4 < (uintptr_t)x.d_amax ||
+            !device_range_ok(ctx, x.d_amax, x.scale_count * 4))
+            return fail(ctx, B200H_E_INVALID, "segment " + std::to_string(i) + ": its scale_count values at d_amax "
+                                              "are not device memory of cuda:" + std::to_string(ctx->device));
+    }
+    return 0;
+}
+
 // The file table of segs[0 .. nsegs) (see file_table); `seg_lens` receives their lengths and backs t.seg_lens.
 int segment_file_table(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
                        uint64_t nfiles, std::vector<uint64_t>& seg_lens, FileTable& t) {
@@ -989,22 +1035,33 @@ int segment_file_table(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs
     return 0;
 }
 
-// Uploads the tables a and b (in that order) into one stream-ordered allocation on `st`, runs launch(device a,
-// device b) and frees the allocation behind it: no synchronisation, and no scratch shared with other streams' calls.
-template <class A, class B, class Launch>
+// Uploads the tables a, b and c (in that order; c may be empty) into one stream-ordered allocation on `st`, runs
+// launch(device a, device b, device c) and frees the allocation behind it: no synchronisation, and no scratch shared
+// with other streams' calls.
+template <class A, class B, class C, class Launch>
 int launch_with_tables(b200h_ctx* ctx, cudaStream_t st, const std::vector<A>& a, const std::vector<B>& b,
-                       Launch&& launch) {
-    const size_t a_bytes = a.size() * sizeof(A), bytes = a_bytes + b.size() * sizeof(B);
+                       const std::vector<C>& c, Launch&& launch) {
+    const size_t a_bytes = a.size() * sizeof(A), b_bytes = b.size() * sizeof(B), c_bytes = c.size() * sizeof(C);
     void* d_table = nullptr;
-    CU_TRY(ctx, cudaMallocAsync(&d_table, bytes, st));
+    CU_TRY(ctx, cudaMallocAsync(&d_table, a_bytes + b_bytes + c_bytes, st));
     A* d_a = (A*)d_table;
     B* d_b = (B*)((uint8_t*)d_table + a_bytes);
+    C* d_c = (C*)((uint8_t*)d_table + a_bytes + b_bytes);
     CU_TRY(ctx, cudaMemcpyAsync(d_a, a.data(), a_bytes, cudaMemcpyHostToDevice, st));
-    CU_TRY(ctx, cudaMemcpyAsync(d_b, b.data(), bytes - a_bytes, cudaMemcpyHostToDevice, st));
-    ctx->launches += launch(d_a, d_b);
+    CU_TRY(ctx, cudaMemcpyAsync(d_b, b.data(), b_bytes, cudaMemcpyHostToDevice, st));
+    if (c_bytes) CU_TRY(ctx, cudaMemcpyAsync(d_c, c.data(), c_bytes, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch(d_a, d_b, d_c);
     CU_TRY(ctx, cudaGetLastError());
     CU_TRY(ctx, cudaFreeAsync(d_table, st));
     return 0;
+}
+
+// launch_with_tables with two tables: launch(device a, device b).
+template <class A, class B, class Launch>
+int launch_with_tables(b200h_ctx* ctx, cudaStream_t st, const std::vector<A>& a, const std::vector<B>& b,
+                       Launch&& launch) {
+    return launch_with_tables(ctx, st, a, b, std::vector<uint8_t>{},
+                              [&](const A* d_a, const B* d_b, const uint8_t*) { return launch(d_a, d_b); });
 }
 
 // The piece of segment s (bytes [in, in + n) of its image) that lands at destination offset `at`: `segs` are the
@@ -1013,19 +1070,29 @@ static CastPiece cast_piece(const b200h_segment* segs, const b200h_cast_segment*
                             uint64_t n, uint64_t at) {
     const uint64_t dev = (uint64_t)(uintptr_t)segs[s].d_ptr;
     if (!casts || !converts(casts[s])) return {{dev + in, at, n}, 0, 0, 0, 0};
-    const uint64_t ss = dt_bytes(casts[s].src_type), ds = dt_bytes(casts[s].dst_type);
+    const uint64_t ss = dt_bytes(casts[s].src_type), ds = image_bytes(casts[s].dst_type);
     return {{dev + in / ds * ss, at, n}, (uint32_t)casts[s].src_type, (uint32_t)casts[s].dst_type, (uint32_t)(in % ds), 0};
+}
+
+// The block scales of the piece of scaled segment s that starts at image byte `in` (zero unless it quantizes).
+static PieceScale piece_scale(const b200h_scaled_segment& x, uint64_t in) {
+    if (x.cast.dst_type != B200H_DT_F8E4M3 || !converts(x.cast)) return {};
+    const uint64_t br = std::min(x.block_rows, x.rows), bc = std::min(x.block_cols, x.cols);
+    return {(uint64_t)(uintptr_t)x.d_amax, in, x.cols, br, bc, x.cols / bc + (x.cols % bc != 0)};
 }
 
 // Appends the pieces of bytes [offset, offset + len) of file `file` (len > 0) landing at destination offset `at`, in
 // file order, and the tiles of their destination bytes (kStageTileBytes each, the last one shorter), which use them.
+// With `scaled` (whose casts are `casts`), every piece's block scales go to `scales` as well.
 static void range_tables(const FileTable& t, const b200h_segment* segs, const b200h_cast_segment* casts, uint64_t file,
                          uint64_t offset, uint64_t len, uint64_t at, std::vector<CastPiece>& pieces,
-                         std::vector<RangeTile>& tiles) {
+                         std::vector<RangeTile>& tiles, const b200h_scaled_segment* scaled = nullptr,
+                         std::vector<PieceScale>* scales = nullptr) {
     const size_t first = pieces.size();
     uint64_t h = at;
     file_pieces(t, file, offset, len, [&](uint64_t s, uint64_t in, uint64_t n) {
         pieces.push_back(cast_piece(segs, casts, s, in, n, h));
+        if (scaled) scales->push_back(piece_scale(scaled[s], in));
         h += n;
     });
     size_t p = first;
@@ -1041,11 +1108,12 @@ static void range_tables(const FileTable& t, const b200h_segment* segs, const b2
 // b200h_hash_segment_parts_device with ctx->mu held, on stream `st`.  d_etag_msg != NULL (b200h_hash_fixed_parts_device):
 // two more words, the ETag message {0, nparts * 16}, ride the part-table upload, even when there are no parts, and
 // *d_etag_msg points at them.  With `casts` (b200h_hash_cast_segment_parts_device; segs is then NULL), the files are
-// the cast segments' images, and the parts that are not hashed in place are gathered by stage_ranges_kernel.
+// the cast segments' images, and the parts that are not hashed in place are gathered by stage_ranges_kernel.  With
+// `scaled` (b200h_hash_scaled_segment_parts_device; `casts` are then their casts), by stage_scaled_ranges_kernel.
 int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
                               uint64_t nfiles, uint64_t part_len, uint32_t flags, void* d_sha256, void* d_md5,
                               uint64_t* d_trimmed_len, uint64_t* nparts_out, cudaStream_t st, const uint64_t** d_etag_msg,
-                              const b200h_cast_segment* casts = nullptr) {
+                              const b200h_cast_segment* casts = nullptr, const b200h_scaled_segment* scaled = nullptr) {
     if (flags & B200H_HEX_OUT) return fail(ctx, B200H_E_INVALID, "B200H_HEX_OUT is not supported for device parts");
     if (((uintptr_t)d_sha256 | (uintptr_t)d_md5) & 15u)
         return fail(ctx, B200H_E_INVALID, "digest outputs must be 16-byte aligned");
@@ -1054,7 +1122,7 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     FileTable t;
     std::string err;
     if (casts) {
-        if (int rc = cast_file_table(casts, nsegs, file_first_seg, nfiles, true, seg_lens, plain, t, err))
+        if (int rc = cast_file_table(casts, nsegs, file_first_seg, nfiles, true, seg_lens, plain, t, err, scaled))
             return fail(ctx, rc, err);
         segs = plain.data();
     } else if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) {
@@ -1063,6 +1131,8 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     // before the layout, whose part list the segments' lengths size
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
+    if (scaled)
+        if (int rc = scales_on_device(ctx, scaled, nsegs)) return rc;
     SegmentParts p;
     if (int rc = layout_segment_parts(t, part_len, std::max(ctx->dwave_cap, ctx->dwave_want), p, err, casts))
         return fail(ctx, rc, err);
@@ -1086,6 +1156,7 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
     // with casts: the tables of every wave's stage_ranges_kernel launch (destination offsets in the wave's slot)
     std::vector<std::vector<CastPiece>> cast_pieces(casts ? nwaves : 0);
     std::vector<std::vector<RangeTile>> cast_tiles(casts ? nwaves : 0);
+    std::vector<std::vector<PieceScale>> piece_scales(scaled ? nwaves : 0);
     for (size_t w = 0; w < nwaves; ++w) {
         uint8_t* slot = ctx->dwave[w & 1];
         for (uint64_t i = p.wave_first[w]; i < p.wave_first[w + 1]; ++i) {
@@ -1096,7 +1167,8 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
             }
             table[i] = (uint64_t)(uintptr_t)(slot + p.stage[i]);
             if (casts) {
-                range_tables(t, segs, casts, p.file[i], p.off[i], p.len[i], p.stage[i], cast_pieces[w], cast_tiles[w]);
+                range_tables(t, segs, casts, p.file[i], p.off[i], p.len[i], p.stage[i], cast_pieces[w], cast_tiles[w],
+                             scaled, scaled ? &piece_scales[w] : nullptr);
                 continue;
             }
             uint64_t at = table[i];
@@ -1127,7 +1199,14 @@ int hash_segment_parts_locked(b200h_ctx* ctx, const b200h_segment* segs, uint64_
         if (staged) {
             // the slot is shared with the *_host entry points and the previous waves: wait for its last reader
             CU_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_consumed[slot], 0));
-            if (casts) {
+            if (scaled) {
+                if (int rc = launch_with_tables(ctx, st, cast_tiles[w], cast_pieces[w], piece_scales[w],
+                                                [&](const RangeTile* d_ct, const CastPiece* d_cp, const PieceScale* d_ps) {
+                                                    return launch_stage_scaled_ranges(d_ct, cast_tiles[w].size(), d_cp,
+                                                                                      d_ps, ctx->dwave[slot], st);
+                                                }))
+                    return rc;
+            } else if (casts) {
                 if (int rc = launch_with_tables(ctx, st, cast_tiles[w], cast_pieces[w],
                                                 [&](const RangeTile* d_ct, const CastPiece* d_cp) {
                                                     return launch_stage_ranges(d_ct, cast_tiles[w].size(), d_cp,
@@ -1527,6 +1606,21 @@ int b200h_hash_cast_segment_parts_device(b200h_ctx* ctx, const b200h_cast_segmen
                                      nullptr, segs ? segs : &kNoSegment);
 }
 
+int b200h_hash_scaled_segment_parts_device(b200h_ctx* ctx, const b200h_scaled_segment* segs, uint64_t nsegs,
+                                           const uint64_t* file_first_seg, uint64_t nfiles, uint64_t part_len,
+                                           uint32_t flags, void* d_sha256, void* d_md5, uint64_t* d_trimmed_len,
+                                           uint64_t* nparts_out, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_hash_scaled_segment_parts_device");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    std::vector<b200h_cast_segment> casts;
+    std::string err;
+    if (int rc = scaled_casts(segs, nsegs, true, casts, err)) return fail(ctx, rc, err);
+    return hash_segment_parts_locked(ctx, nullptr, nsegs, file_first_seg, nfiles, part_len, flags, d_sha256, d_md5,
+                                     d_trimmed_len, nparts_out, cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp,
+                                     nullptr, nsegs ? casts.data() : &kNoSegment, nsegs ? segs : &kNoScaled);
+}
+
 int b200h_crc32_device(b200h_ctx* ctx, const b200h_segment* ranges, uint64_t n, uint32_t* d_crc_out, void* cuda_stream) {
     if (!ctx) return B200H_E_INVALID;
     B200H_RANGE("b200h_crc32_device");
@@ -1574,10 +1668,11 @@ static void* pinned_device_pointer(b200h_ctx* ctx, const void* h, uint64_t bytes
 // [host_offsets[i], host_offsets[i] + len) of the page-locked buffer `host` are copied one way or the other.
 // b200h_copy_cast_ranges (casts != NULL, segs NULL, to_host): the files are the cast segments' images, and `host` is
 // page-locked host memory or memory of ctx's device.
+// b200h_copy_scaled_ranges: `scaled` as well, whose casts are `casts`.
 static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, uint64_t nsegs,
                        const uint64_t* file_first_seg, uint64_t nfiles, const b200h_file_range* ranges, uint64_t nranges,
                        const void* host, uint64_t host_bytes, const uint64_t* host_offsets, void* cuda_stream,
-                       const b200h_cast_segment* casts = nullptr) {
+                       const b200h_cast_segment* casts = nullptr, const b200h_scaled_segment* scaled = nullptr) {
     const std::string buf = casts ? "dst" : to_host ? "h_dst" : "h_src", offsets = to_host ? "dst_offsets" : "src_offsets",
                       noun = to_host ? "destination" : "source";
     std::vector<uint64_t> seg_lens;
@@ -1585,7 +1680,7 @@ static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, 
     FileTable t;
     if (casts) {
         std::string err;
-        if (int rc = cast_file_table(casts, nsegs, file_first_seg, nfiles, true, seg_lens, plain, t, err))
+        if (int rc = cast_file_table(casts, nsegs, file_first_seg, nfiles, true, seg_lens, plain, t, err, scaled))
             return fail(ctx, rc, err);
         segs = plain.data();
     } else if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) {
@@ -1617,6 +1712,8 @@ static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, 
     }
     CU_TRY(ctx, cudaSetDevice(ctx->device));
     if (int rc = segments_on_device(ctx, segs, nsegs, "segment")) return rc;
+    if (scaled)
+        if (int rc = scales_on_device(ctx, scaled, nsegs)) return rc;
     if (nranges == 0) return 0;
     void* d_host = casts && device_range_ok(ctx, host, host_bytes) ? const_cast<void*>(host)
                                                                    : pinned_device_pointer(ctx, host, host_bytes);
@@ -1631,14 +1728,21 @@ static int copy_ranges(b200h_ctx* ctx, bool to_host, const b200h_segment* segs, 
     // pieces (range x segment, in file order within a range) and the tiles of host bytes that use them
     std::vector<CastPiece> pieces;
     std::vector<RangeTile> tiles;
+    std::vector<PieceScale> scales;
     std::vector<uint64_t> range_of;  // per piece: the range it belongs to (for the overlap message)
     for (uint64_t i = 0; i < nranges; ++i) {
         const b200h_file_range& r = ranges[i];
         if (!r.len) continue;
-        range_tables(t, segs, casts, r.file, r.offset, r.len, host_offsets[i], pieces, tiles);
+        range_tables(t, segs, casts, r.file, r.offset, r.len, host_offsets[i], pieces, tiles, scaled, &scales);
         range_of.resize(pieces.size(), i);
     }
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    if (scaled)
+        return launch_with_tables(ctx, st, tiles, pieces, scales,
+                                  [&](const RangeTile* d_tiles, const CastPiece* d_pieces, const PieceScale* d_scales) {
+                                      return launch_stage_scaled_ranges(d_tiles, tiles.size(), d_pieces, d_scales,
+                                                                        d_host, st);
+                                  });
     if (to_host)
         return launch_with_tables(ctx, st, tiles, pieces, [&](const RangeTile* d_tiles, const CastPiece* d_pieces) {
             return launch_stage_ranges(d_tiles, tiles.size(), d_pieces, d_host, st);
@@ -1687,6 +1791,92 @@ int b200h_copy_cast_ranges(b200h_ctx* ctx, const b200h_cast_segment* segs, uint6
     if (nsegs && !segs) return fail(ctx, B200H_E_INVALID, "segments must not be NULL");
     return copy_ranges(ctx, true, nullptr, nsegs, file_first_seg, nfiles, ranges, nranges, dst, dst_bytes, dst_offsets,
                        cuda_stream, segs ? segs : &kNoSegment);
+}
+
+int b200h_copy_scaled_ranges(b200h_ctx* ctx, const b200h_scaled_segment* segs, uint64_t nsegs,
+                             const uint64_t* file_first_seg, uint64_t nfiles, const b200h_file_range* ranges,
+                             uint64_t nranges, void* dst, uint64_t dst_bytes, const uint64_t* dst_offsets,
+                             void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_scaled_ranges");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    std::vector<b200h_cast_segment> casts;
+    std::string err;
+    if (int rc = scaled_casts(segs, nsegs, true, casts, err)) return fail(ctx, rc, err);
+    return copy_ranges(ctx, true, nullptr, nsegs, file_first_seg, nfiles, ranges, nranges, dst, dst_bytes, dst_offsets,
+                       cuda_stream, nsegs ? casts.data() : &kNoSegment, nsegs ? segs : &kNoScaled);
+}
+
+// b200h_fp8_block_scales: the jobs' tiles.  A tile is up to kScaleTileElems elements of one block: at most
+// kScaleTileCols of its columns, and as many of its rows as fill the rest.
+constexpr uint64_t kScaleTileElems = 16384, kScaleTileCols = 4096;
+
+int b200h_fp8_block_scales(b200h_ctx* ctx, const b200h_fp8_scale_job* jobs, uint64_t njobs, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_fp8_block_scales");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (njobs && !jobs) return fail(ctx, B200H_E_INVALID, "jobs must not be NULL");
+    if (njobs > 0xffffffffull) return fail(ctx, B200H_E_INVALID, "too many jobs");
+    std::vector<ScaleJob> table(njobs);
+    std::vector<std::pair<uintptr_t, uint64_t>> amax;  // (address, bytes) of every job's a
+    uint64_t ntiles = 0, nblocks = 0;
+    for (uint64_t i = 0; i < njobs; ++i) {
+        const b200h_fp8_scale_job& x = jobs[i];
+        const std::string name = "job " + std::to_string(i);
+        const uint64_t ss = dt_bytes(x.src_type);
+        if (!ss) return fail(ctx, B200H_E_INVALID, name + ": src_type is not F32, F16 or BF16");
+        if (!x.rows || !x.cols) return fail(ctx, B200H_E_INVALID, name + ": R and C must be >= 1");
+        if (!x.block_rows || !x.block_cols) return fail(ctx, B200H_E_INVALID, name + ": block sizes must be >= 1");
+        if ((unsigned __int128)x.rows * x.cols * ss > ~0ull) return fail(ctx, B200H_E_INVALID, name + ": R * C overflows");
+        if (!x.d_src || (uintptr_t)x.d_src % ss)
+            return fail(ctx, B200H_E_INVALID, name + ": d_src is NULL or not aligned to its element size");
+        if (!x.d_scales || !x.d_amax || ((uintptr_t)x.d_scales | (uintptr_t)x.d_amax) % 4)
+            return fail(ctx, B200H_E_INVALID, name + ": d_scales and d_amax must be 4-byte aligned, not NULL");
+        ScaleJob& J = table[i];
+        J.src = (uint64_t)(uintptr_t)x.d_src;
+        J.rows = x.rows;
+        J.cols = x.cols;
+        J.block_rows = std::min(x.block_rows, x.rows);
+        J.block_cols = std::min(x.block_cols, x.cols);
+        J.scale_cols = J.cols / J.block_cols + (J.cols % J.block_cols != 0);
+        J.sub_cols = std::min(J.block_cols, kScaleTileCols);
+        J.sub_rows = std::min(J.block_rows, std::max<uint64_t>(1, kScaleTileElems / J.sub_cols));
+        J.tile_cols = J.block_cols / J.sub_cols + (J.block_cols % J.sub_cols != 0);
+        J.tiles_per_block = (J.block_rows / J.sub_rows + (J.block_rows % J.sub_rows != 0)) * J.tile_cols;
+        const uint64_t count = (J.rows / J.block_rows + (J.rows % J.block_rows != 0)) * J.scale_cols;
+        J.first_tile = ntiles;
+        J.first_block = nblocks;
+        J.scales = (uint64_t)(uintptr_t)x.d_scales;
+        J.amax = (uint64_t)(uintptr_t)x.d_amax;
+        J.src_type = (uint32_t)x.src_type;
+        ntiles += count * J.tiles_per_block;
+        nblocks += count;
+        amax.push_back({J.amax, count * 4});
+    }
+    CU_TRY(ctx, cudaSetDevice(ctx->device));
+    for (uint64_t i = 0; i < njobs; ++i) {
+        const b200h_fp8_scale_job& x = jobs[i];
+        const uint64_t count = amax[i].second / 4;
+        if (!device_range_ok(ctx, x.d_src, x.rows * x.cols * dt_bytes(x.src_type)) ||
+            !device_range_ok(ctx, x.d_scales, count * 4) || !device_range_ok(ctx, x.d_amax, count * 4))
+            return fail(ctx, B200H_E_INVALID, "job " + std::to_string(i) + ": d_src, d_scales or d_amax is not device "
+                                              "memory of cuda:" + std::to_string(ctx->device));
+    }
+    // a starts as zeros: one memset per contiguous run of the jobs' a arrays
+    std::sort(amax.begin(), amax.end());
+    std::vector<std::pair<uintptr_t, uint64_t>> runs;
+    for (const auto& r : amax) {
+        if (!runs.empty() && runs.back().first + runs.back().second > r.first)
+            return fail(ctx, B200H_E_INVALID, "the d_amax arrays of two jobs overlap");
+        if (!runs.empty() && runs.back().first + runs.back().second == r.first) runs.back().second += r.second;
+        else runs.push_back(r);
+    }
+    if (njobs == 0) return 0;
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    for (const auto& r : runs) CU_TRY(ctx, cudaMemsetAsync((void*)r.first, 0, r.second, st));
+    return launch_with_tables(ctx, st, table, std::vector<uint8_t>{}, [&](const ScaleJob* d_jobs, const uint8_t*) {
+        return launch_fp8_block_scales(d_jobs, (uint32_t)njobs, ntiles, nblocks, st);
+    });
 }
 
 static bool is_fp8(uint64_t t) { return t == B200H_DT_F8E4M3 || t == B200H_DT_F8E5M2; }
@@ -2319,6 +2509,24 @@ int b200h_cast_segment_parts_preview(const b200h_cast_segment* segs, uint64_t ns
     std::string err;
     if (int rc = cast_file_table(segs, nsegs, file_first_seg, nfiles, false, seg_lens, plain, t, err)) return rc;
     if (int rc = layout_segment_parts(t, part_len, wave_bytes, p, err, segs ? segs : &kNoSegment)) return rc;
+    report_segment_parts(p, nparts_out, nwaves_out, seg_out, wave_out, out_cap);
+    return 0;
+}
+
+int b200h_scaled_segment_parts_preview(const b200h_scaled_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                                       uint64_t nfiles, uint64_t part_len, uint64_t wave_bytes, uint64_t* nparts_out,
+                                       uint64_t* nwaves_out, uint64_t* seg_out, uint32_t* wave_out, uint64_t out_cap) {
+    std::vector<b200h_cast_segment> casts;
+    std::vector<uint64_t> seg_lens;
+    std::vector<b200h_segment> plain;
+    FileTable t;
+    SegmentParts p;
+    std::string err;
+    if (int rc = scaled_casts(segs, nsegs, false, casts, err)) return rc;
+    const b200h_cast_segment* cs = nsegs ? casts.data() : &kNoSegment;
+    if (int rc = cast_file_table(nsegs ? cs : nullptr, nsegs, file_first_seg, nfiles, false, seg_lens, plain, t, err, true))
+        return rc;
+    if (int rc = layout_segment_parts(t, part_len, wave_bytes, p, err, cs)) return rc;
     report_segment_parts(p, nparts_out, nwaves_out, seg_out, wave_out, out_cap);
     return 0;
 }

@@ -190,6 +190,33 @@ struct ScaledTile {
 int launch_load_scaled_boxes(const ScaledTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
                              cudaStream_t st);
 
+// The block scales of a quantizing piece (a CastPiece with dst_type B200H_DT_F8E4M3, whose image has one byte per
+// element and phase 0): image byte k of the piece is element first_elem + k of the R x C weight, whose block
+// (i / block_rows, j / block_cols) has its clamped amax at amax[(i / block_rows) * scale_cols + j / block_cols].  Block
+// sizes are clamped to the dimensions.  Unused (zero) for the other pieces.
+struct PieceScale {
+    uint64_t amax;
+    uint64_t first_elem, cols, block_rows, block_cols, scale_cols;
+};
+// Every tile's copy of the pieces' images, quantizing pieces included (stage_scaled_ranges_kernel); scales[k] goes with
+// pieces[k].
+int launch_stage_scaled_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces,
+                               const PieceScale* scales, void* dst, cudaStream_t st);
+
+// One weight of b200h_fp8_block_scales, split into tiles: a tile is up to sub_rows x sub_cols elements of one block
+// (tiles_per_block of them per block, tile_cols across its columns); the job's tiles are numbered from first_tile and its
+// blocks from first_block (a flat numbering over every job of the call).
+struct ScaleJob {
+    uint64_t src;
+    uint64_t rows, cols, block_rows, block_cols, scale_cols;  // block sizes clamped to the dimensions
+    uint64_t sub_rows, sub_cols, tile_cols, tiles_per_block;
+    uint64_t first_tile, first_block;
+    uint64_t scales, amax;  // F32 outputs; amax starts as zeros and receives the bits of max |x| first
+    uint32_t src_type, pad;
+};
+// The amax reduction and the finalisation of a and s (two launches; amax must be zero before them).
+int launch_fp8_block_scales(const ScaleJob* jobs, uint32_t njobs, uint64_t ntiles, uint64_t nblocks, cudaStream_t st);
+
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)
 cudaError_t configure_kernels();  // one-time cudaFuncSetAttribute calls for the current device

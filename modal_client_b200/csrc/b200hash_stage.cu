@@ -687,6 +687,251 @@ __global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
     }
 }
 
+// ---- stage_scaled_ranges_kernel: stage_ranges_kernel whose pieces may also quantize to FP8 E4M3 on the way out
+//      (b200h_copy_scaled_ranges, and the wave-slot gather of b200h_hash_scaled_segment_parts_device)
+//
+// A quantizing piece's image has one byte per element, so every image byte starts an element and a destination word
+// inside the piece is 16 elements: 32 source bytes from a 16-bit source, 64 from F32, taken with aligned 16-byte loads
+// inside the piece's hull and shift_bytes.  Element e = (i, j) of the weight is multiplied by its block's
+// m = RN(RN(1 / a) * 448) with one round-to-nearest multiply that keeps subnormals and converted with the sm_90 paired
+// E4M3 conversion (round to nearest even; satfinite, which no element reaches: |x * m| rounds to at most 448, and a NaN
+// product gives 0x7F either way).  (i, j) is computed once per word, then stepped one element at a time; m is reloaded
+// only where j crosses a block-column edge or a row's end.  Words across pieces and tail bytes go element by element.
+// Its own kernel, so that stage_ranges_kernel's code stays as it is.
+
+constexpr float kE4M3Max = 448.0f;
+
+// The element of a quantizing piece that the cursor stands on, and its block's multiplier.
+struct QuantCursor {
+    uint64_t i, j, jend;  // the element's coordinates; the column where its block column (or the row) ends
+    float m;
+};
+
+__device__ __forceinline__ void quant_load(const PieceScale& q, QuantCursor& c) {
+    const uint64_t jb = c.j / q.block_cols;
+    c.jend = min((jb + 1) * q.block_cols, q.cols);
+    const float a = __ldg(reinterpret_cast<const float*>(q.amax) + c.i / q.block_rows * q.scale_cols + jb);
+    c.m = __fmul_rn(__frcp_rn(a), kE4M3Max);
+}
+
+// the cursor at element e of the weight (its row-major index)
+__device__ __forceinline__ void quant_seek(const PieceScale& q, uint64_t e, QuantCursor& c) {
+    c.i = e / q.cols;
+    c.j = e - c.i * q.cols;
+    quant_load(q, c);
+}
+
+// the multiplier of the cursor's element; the cursor moves on to the weight's next element
+__device__ __forceinline__ float quant_next(const PieceScale& q, QuantCursor& c) {
+    if (c.j == c.jend) {
+        if (c.j == q.cols) c.j = 0, ++c.i;
+        quant_load(q, c);
+    }
+    ++c.j;
+    return c.m;
+}
+
+// one element of type st (F32, F16 or BF16; in the low bits of x), exactly as a float
+__device__ __forceinline__ float widen_one(uint32_t x, uint32_t st) {
+    return st == kDtF32 ? __uint_as_float(x) : widen_pair(x & 0xffffu, st).x;
+}
+
+// two products as E4M3, the first in the low byte
+__device__ __forceinline__ uint32_t e4m3_pair(float a, float b) {
+    return (uint32_t)__nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+}
+
+// the destination word of the 16 elements at s (a multiple of ss, inside one quantizing piece), whose first is element e
+__device__ __forceinline__ uint4 quant_load_word(const uint8_t* s, uint32_t st, const PieceScale& q, uint64_t e) {
+    const uint32_t sh = (uint32_t)((uintptr_t)s & 15u);
+    const uint4* a = reinterpret_cast<const uint4*>(s - sh);
+    float x[16];
+    if (st == kDtF32) {  // 64 source bytes
+        uint4 w[5];
+        w[0] = __ldg(a);
+#pragma unroll
+        for (int k = 1; k < 4; ++k) w[k] = __ldg(a + k);
+        w[4] = sh ? __ldg(a + 4) : w[3];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint4 v = sh ? shift_bytes(w[k], w[k + 1], sh) : w[k];
+            x[4 * k] = __uint_as_float(v.x), x[4 * k + 1] = __uint_as_float(v.y);
+            x[4 * k + 2] = __uint_as_float(v.z), x[4 * k + 3] = __uint_as_float(v.w);
+        }
+    } else {  // 32
+        const uint4 w0 = __ldg(a), w1 = __ldg(a + 1), w2 = sh ? __ldg(a + 2) : w1;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint4 v = sh ? shift_bytes(k ? w1 : w0, k ? w2 : w1, sh) : (k ? w1 : w0);
+            const float2 p0 = widen_pair(v.x, st), p1 = widen_pair(v.y, st), p2 = widen_pair(v.z, st),
+                         p3 = widen_pair(v.w, st);
+            x[8 * k] = p0.x, x[8 * k + 1] = p0.y, x[8 * k + 2] = p1.x, x[8 * k + 3] = p1.y;
+            x[8 * k + 4] = p2.x, x[8 * k + 5] = p2.y, x[8 * k + 6] = p3.x, x[8 * k + 7] = p3.y;
+        }
+    }
+    QuantCursor c;
+    quant_seek(q, e, c);
+    uint32_t out[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float y0 = __fmul_rn(x[4 * k], quant_next(q, c)), y1 = __fmul_rn(x[4 * k + 1], quant_next(q, c));
+        const float y2 = __fmul_rn(x[4 * k + 2], quant_next(q, c)), y3 = __fmul_rn(x[4 * k + 3], quant_next(q, c));
+        out[k] = e4m3_pair(y0, y1) | e4m3_pair(y2, y3) << 16;
+    }
+    return make_uint4(out[0], out[1], out[2], out[3]);
+}
+
+// byte d (a destination offset inside piece p, whose scales are q) of the piece's image
+__device__ __forceinline__ uint32_t scaled_image_byte(const CastPiece& p, const PieceScale& q, uint64_t d) {
+    if (p.dst_type != kDtF8E4M3) return image_byte(p, d);
+    const uint64_t in = d - p.r.host;
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(p.r.dev);
+    const uint32_t x = p.src_type == kDtF32 ? *reinterpret_cast<const uint32_t*>(s + in * 4)
+                                            : (uint32_t)*reinterpret_cast<const uint16_t*>(s + in * 2);
+    QuantCursor c;
+    quant_seek(q, q.first_elem + in, c);
+    return e4m3_pair(__fmul_rn(widen_one(x, p.src_type), c.m), 0.f) & 0xffu;
+}
+
+// the destination word at d, byte by byte from pieces pc[i ..] (pc[i] holds d; the word lies in the range)
+__device__ __forceinline__ uint4 scaled_image_word(const CastPiece* __restrict__ pc, const PieceScale* __restrict__ ps,
+                                                   uint32_t i, uint64_t d) {
+    uint64_t x[2] = {0, 0};
+    uint64_t end = pc[i].r.host + pc[i].r.len;
+#pragma unroll 1
+    for (uint32_t j = 0; j < 16; ++j) {
+        while (d + j >= end) {
+            ++i;
+            end = pc[i].r.host + pc[i].r.len;
+        }
+        const uint64_t b = (uint64_t)scaled_image_byte(pc[i], ps[i], d + j) << (8 * (j & 7));
+        if (j < 8) x[0] |= b;
+        else x[1] |= b;
+    }
+    return make_uint4((uint32_t)x[0], (uint32_t)(x[0] >> 32), (uint32_t)x[1], (uint32_t)(x[1] >> 32));
+}
+
+__global__ void __launch_bounds__(kStageThreads, kStageCtasPerSm)
+    stage_scaled_ranges_kernel(const RangeTile* __restrict__ tiles, uint64_t ntiles,
+                               const CastPiece* __restrict__ pieces, const PieceScale* __restrict__ scales,
+                               uint8_t* __restrict__ dst) {
+    for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const RangeTile tile = tiles[t];
+        const CastPiece* __restrict__ pc = pieces + tile.first_piece;
+        const PieceScale* __restrict__ ps = scales + tile.first_piece;
+        uint8_t* out = dst + tile.host;
+        const uint32_t words = tile.len >> 4, tail = tile.len & 15u;
+        if (tile.npieces == 1 && pc->src_type == pc->dst_type) {
+            stage_one_piece(reinterpret_cast<const uint8_t*>(pc->r.dev) + (tile.host - pc->r.host), out, words, tail);
+            continue;
+        }
+        uint32_t cur = 0;
+        for (uint32_t w = threadIdx.x; w < words; w += kStageThreads) {
+            const uint64_t d = tile.host + (uint64_t)w * 16;
+            if (d >= pc[cur].r.host + pc[cur].r.len) cur = find_piece(pc, cur + 1, tile.npieces, d);
+            const CastPiece p = pc[cur];
+            const uint64_t in = d - p.r.host, left = p.r.len - in;
+            const uint8_t* s = reinterpret_cast<const uint8_t*>(p.r.dev);
+            uint4 v;
+            if (left >= 16 && p.src_type == p.dst_type) {
+                v = load_word(s + in);
+            } else if (left >= 16 && p.dst_type == kDtF8E4M3) {
+                const PieceScale q = ps[cur];
+                v = quant_load_word(s + in * dt_bytes(p.src_type), p.src_type, q, q.first_elem + in);
+            } else if (left >= 16 && ((in + p.phase) & (dt_bytes(p.dst_type) - 1)) == 0) {
+                const uint64_t e = (in + p.phase) / dt_bytes(p.dst_type);
+                v = cast_load_word(s + e * dt_bytes(p.src_type), p.src_type, p.dst_type);
+            } else {
+                v = scaled_image_word(pc, ps, cur, d);
+            }
+            *reinterpret_cast<uint4*>(dst + d) = v;
+        }
+        if (threadIdx.x < tail) {
+            const uint64_t d = tile.host + (uint64_t)words * 16 + threadIdx.x;
+            const uint32_t k = find_piece(pc, 0, tile.npieces, d);
+            dst[d] = (uint8_t)scaled_image_byte(pc[k], ps[k], d);
+        }
+    }
+}
+
+// ---- FP8 block scales (b200h_fp8_block_scales)
+//
+//   fp8_amax_kernel      persistent CTAs take tiles (up to sub_rows x sub_cols elements of one block of one job); warp
+//                        w takes the tile's rows w, w + 8, ..., its lanes the columns.  |x| is widened to F32 and its
+//                        bits max-reduced as integers (for non-negative floats the integer order is the float order,
+//                        and a NaN's bits exceed every other value's), per warp, then per CTA, then one atomicMax per
+//                        CTA into the block's amax word.
+//   fp8_finalize_kernel  a = amax is NaN ? amax : max(amax, 1e-4f) in place, s = a * RN(1 / 448): the F32 arithmetic of
+//                        torch's clamp and its CUDA division by a CPU scalar (a multiplication by its reciprocal).
+
+constexpr int kScaleThreads = 256;
+constexpr float kAmaxFloor = 1e-4f;
+constexpr float kInvE4M3Max = 1.0f / 448.0f;
+
+__device__ __forceinline__ uint32_t abs_bits(const uint8_t* src, uint64_t e, uint32_t st) {
+    if (st == kDtF32) return __ldg(reinterpret_cast<const uint32_t*>(src) + e) & 0x7fffffffu;
+    const uint32_t x = __ldg(reinterpret_cast<const unsigned short*>(src) + e);
+    return __float_as_uint(widen_one(x, st)) & 0x7fffffffu;
+}
+
+__global__ void __launch_bounds__(kScaleThreads)
+    fp8_amax_kernel(const ScaleJob* __restrict__ jobs, uint32_t njobs, uint64_t ntiles) {
+    __shared__ uint32_t red[kScaleThreads / 32];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    for (uint64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        uint32_t lo = 0, hi = njobs - 1;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if (jobs[mid].first_tile <= t) lo = mid;
+            else hi = mid - 1;
+        }
+        const ScaleJob& J = jobs[lo];
+        const uint64_t u = t - J.first_tile, blk = u / J.tiles_per_block, in = u % J.tiles_per_block;
+        const uint64_t bi = blk / J.scale_cols, bj = blk % J.scale_cols;
+        const uint64_t si = in / J.tile_cols, sj = in % J.tile_cols;
+        const uint64_t r0 = bi * J.block_rows + si * J.sub_rows, c0 = bj * J.block_cols + sj * J.sub_cols;
+        const uint64_t r1 = min(min(r0 + J.sub_rows, (bi + 1) * J.block_rows), J.rows);
+        const uint64_t c1 = min(min(c0 + J.sub_cols, (bj + 1) * J.block_cols), J.cols);
+        if (r0 >= r1 || c0 >= c1) continue;  // a tile past an edge block's end (the whole CTA skips it)
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(J.src);
+        const uint32_t st = J.src_type, w = (uint32_t)(c1 - c0);
+        uint32_t m = 0;
+        for (uint64_t r = r0 + warp; r < r1; r += kScaleThreads / 32) {
+            const uint64_t base = r * J.cols + c0;
+#pragma unroll 4
+            for (uint32_t c = lane; c < w; c += 32) m = max(m, abs_bits(src, base + c, st));
+        }
+#pragma unroll
+        for (int k = 16; k; k >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, k));
+        if (lane == 0) red[warp] = m;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+#pragma unroll
+            for (int k = 1; k < kScaleThreads / 32; ++k) m = max(m, red[k]);
+            atomicMax(reinterpret_cast<unsigned int*>(J.amax) + (blk), m);
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(kScaleThreads)
+    fp8_finalize_kernel(const ScaleJob* __restrict__ jobs, uint32_t njobs, uint64_t nblocks) {
+    for (uint64_t k = (uint64_t)blockIdx.x * kScaleThreads + threadIdx.x; k < nblocks;
+         k += (uint64_t)gridDim.x * kScaleThreads) {
+        uint32_t lo = 0, hi = njobs - 1;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if (jobs[mid].first_block <= k) lo = mid;
+            else hi = mid - 1;
+        }
+        const uint64_t b = k - jobs[lo].first_block;
+        float* amax = reinterpret_cast<float*>(jobs[lo].amax) + b;
+        const float x = *amax, a = isnan(x) ? x : fmaxf(x, kAmaxFloor);
+        *amax = a;
+        reinterpret_cast<float*>(jobs[lo].scales)[b] = __fmul_rn(a, kInvE4M3Max);
+    }
+}
+
 }  // namespace
 
 int launch_load_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
@@ -721,6 +966,24 @@ int launch_stage_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece
     stage_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(tiles, ntiles, pieces,
                                                                                       static_cast<uint8_t*>(dst));
     return 1;
+}
+
+int launch_stage_scaled_ranges(const RangeTile* tiles, uint64_t ntiles, const CastPiece* pieces,
+                               const PieceScale* scales, void* dst, cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kStageCtasPerSm;
+    stage_scaled_ranges_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
+        tiles, ntiles, pieces, scales, static_cast<uint8_t*>(dst));
+    return 1;
+}
+
+int launch_fp8_block_scales(const ScaleJob* jobs, uint32_t njobs, uint64_t ntiles, uint64_t nblocks, cudaStream_t st) {
+    if (!njobs) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * 8;
+    fp8_amax_kernel<<<(int)(ntiles < cap ? ntiles : cap), kScaleThreads, 0, st>>>(jobs, njobs, ntiles);
+    const uint64_t ctas = (nblocks + kScaleThreads - 1) / kScaleThreads;
+    fp8_finalize_kernel<<<(int)(ctas < cap ? ctas : cap), kScaleThreads, 0, st>>>(jobs, njobs, nblocks);
+    return 2;
 }
 
 }  // namespace b200h

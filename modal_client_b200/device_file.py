@@ -33,6 +33,11 @@ ONE ``b200h_copy_cast_boxes_from_host`` call (``volume.read_safetensors(..., dty
 
 ``safetensors_shards(state_dict, max_shard_size=...)`` is a checkpoint in the Hugging Face Hub's sharded layout: the
 files ``huggingface_hub.save_torch_state_dict`` writes, each shard a ``DeviceFile.safetensors``, plus the index.
+
+``DeviceFile.safetensors(..., fp8=names)`` (and ``safetensors_shards``) exports weights as block-scaled FP8 E4M3 with
+their F32 scales: the scales are computed on the device by ONE ``b200h_fp8_block_scales`` call, and the weights are
+quantized as the file's bytes leave the device (``b200h_hash_scaled_segment_parts_device``,
+``b200h_copy_scaled_ranges``), never held quantized in HBM.
 """
 from __future__ import annotations
 
@@ -59,28 +64,32 @@ class _TensorBytes:
     With ``casts`` -- ``(src_type, dst_type)`` ``_lib.DT_*`` codes per segment, equal (0, 0) for one that converts
     nothing -- the file is the segments' converted images: segment s contributes its elements as ``dst_type``, and
     every offset and count (``seg_start``, ``nbytes``, ``bytes_to_host``) is in image bytes.  The converted bytes are
-    made on the way out, by the context ``ctx``, and never held in HBM."""
+    made on the way out, by the context ``ctx``, and never held in HBM.
+
+    With ``scales`` as well -- per segment ``(amax_ptr, scale_count, R, C, block_rows, block_cols)``, or None for one
+    that does not quantize -- a segment whose ``dst_type`` is ``_lib.DT_F8E4M3`` is its weight quantized with those
+    amax values (one image byte per element), and every copy and hash is a scaled call."""
 
     device_type = "cuda"
 
-    def __init__(self, tensors, bounce_bytes: int, casts=None, ctx=None):
+    def __init__(self, tensors, bounce_bytes: int, casts=None, ctx=None, scales=None):
         import torch
 
-        self._attach(tensors, bounce_bytes, casts, ctx)
+        self._attach(tensors, bounce_bytes, casts, ctx, scales)
         device = self.segments[0].device
         self.stream = torch.cuda.Stream(device)
         # everything already queued on the caller's stream (the kernels that produced the tensors) runs first
         self.stream.wait_stream(torch.cuda.current_stream(device))
         self.stream_handle = self.stream.cuda_stream
 
-    def _attach(self, tensors, bounce_bytes: int, casts=None, ctx=None):
+    def _attach(self, tensors, bounce_bytes: int, casts=None, ctx=None, scales=None):
         """``tensors``: one tensor, or a non-empty list of them in file order."""
         import torch
 
         self.tensors = list(tensors) if isinstance(tensors, (list, tuple)) else [tensors]  # keep the storages alive
         self.segments = [t.reshape(-1).view(torch.uint8) for t in self.tensors]
-        self.casts, self.ctx = casts, ctx
-        size = {_lib.DT_F32: 4, _lib.DT_F16: 2, _lib.DT_BF16: 2}
+        self.casts, self.ctx, self.scales = casts, ctx, scales
+        size = {_lib.DT_F32: 4, _lib.DT_F16: 2, _lib.DT_BF16: 2, _lib.DT_F8E4M3: 1}
         self.seg_start = [0]  # file offset of every segment, then the size
         for i, s in enumerate(self.segments):
             st, dt = casts[i] if casts else (0, 0)
@@ -193,7 +202,12 @@ class _TensorBytes:
                 k = min(n - done, self._bounce_bytes)
                 filled = 0
                 with self._on_stream():
-                    if self.casts:
+                    if self.scales:
+                        ptrs, lens, first = _file_table([self])
+                        self.ctx.copy_scaled_ranges(ptrs, lens, *_types([self]), _scales([self]), first,
+                                                    [(0, pos + done, k)], bounce, [0], self.stream_handle)
+                        filled = k
+                    elif self.casts:
                         ptrs, lens, first = _file_table([self])
                         self.ctx.copy_cast_ranges(ptrs, lens, *_types([self]), first, [(0, pos + done, k)], bounce, [0],
                                                   self.stream_handle)
@@ -239,7 +253,11 @@ def _hash_sources(sources: list[_TensorBytes], ctx, part_len: int, flags: int):
     n = sum(-(-src.nbytes // part_len) for src in sources)
     with lead._on_stream():
         d_sha, d_md5, d_trim = _outputs(n, flags, lead.segments[0].device)
-        if any(src.casts for src in sources):
+        if any(src.scales for src in sources):
+            got = ctx.hash_scaled_segment_parts_device(ptrs, lens, *_types(sources), _scales(sources), first, part_len,
+                                                       flags, _ptr(d_sha), _ptr(d_md5), _ptr(d_trim),
+                                                       lead.stream_handle)
+        elif any(src.casts for src in sources):
             got = ctx.hash_cast_segment_parts_device(ptrs, lens, *_types(sources), first, part_len, flags, _ptr(d_sha),
                                                      _ptr(d_md5), _ptr(d_trim), lead.stream_handle)
         else:
@@ -280,7 +298,8 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
     over page-locked memory from ``ctx.host_alloc``; range i lands at ``dst[dst_offsets[i]:]`` (offsets multiples of
     16, destinations disjoint; the layout is the caller's).  ONE ``b200h_copy_ranges_to_host`` call (one kernel launch)
     whatever the files are made of, enqueued on the first file's stream, which is ordered after every file's stream;
-    ONE ``b200h_copy_cast_ranges`` call instead when any of the files converts its tensors.
+    ONE ``b200h_copy_cast_ranges`` call instead when any of the files converts its tensors, and ONE
+    ``b200h_copy_scaled_ranges`` call when any of them quantizes.
     Returns at once; ``wait()`` on the result blocks until the bytes are in ``dst``.  Every file's ``bytes_to_host``
     grows by the bytes of its ranges."""
     ctx = ctx or get_context()
@@ -290,7 +309,10 @@ def stage_ranges(files: list["DeviceFile"], ranges, dst: np.ndarray, dst_offsets
     lead = sources[0]
     ptrs, lens, first = _file_table(sources)
     with lead._on_stream():
-        if any(src.casts for src in sources):
+        if any(src.scales for src in sources):
+            ctx.copy_scaled_ranges(ptrs, lens, *_types(sources), _scales(sources), first, ranges, dst, offsets,
+                                   lead.stream_handle)
+        elif any(src.casts for src in sources):
             ctx.copy_cast_ranges(ptrs, lens, *_types(sources), first, ranges, dst, offsets, lead.stream_handle)
         else:
             ctx.copy_ranges_to_host(ptrs, lens, first, ranges, dst, offsets, lead.stream_handle)
@@ -319,6 +341,12 @@ def _types(sources: list[_TensorBytes]):
     are)."""
     pairs = [pair for src in sources for pair in (src.casts or [(0, 0)] * len(src.segments))]
     return [st for st, _ in pairs], [dt for _, dt in pairs]
+
+
+def _scales(sources: list[_TensorBytes]):
+    """Every segment's ``(amax_ptr, scale_count, R, C, block_rows, block_cols)`` of ``sources``, in ``_file_table``
+    order (zeros for a segment that does not quantize)."""
+    return [q or (0,) * 6 for src in sources for q in (src.scales or [None] * len(src.segments))]
 
 
 def _range_args(files: list["DeviceFile"], ranges, offsets, offsets_name: str):
@@ -452,6 +480,74 @@ def cast_targets(path: str, dtype, entries, data_start: int, sliced: bool = Fals
         raise ValueError(f"{path}: dtype: " + "; ".join(problems))
     return out
 
+
+def _fp8_plan(tensors: Mapping, dtype, fp8, scale_block, scale_suffix, problems: list) -> dict:
+    """{weight: scale name} of the names in ``fp8``, in the order of ``tensors``, for ``DeviceFile.safetensors(...,
+    fp8=...)``; every problem is appended to ``problems``: unknown or repeated names, weights that are not 2-D, empty or
+    F32 / F16 / BF16, a bad ``scale_block`` or ``scale_suffix``, a scale name that is already a name, a name that
+    ``dtype`` maps too, and a weight that shares its storage with another name."""
+    import torch
+
+    if isinstance(fp8, str):
+        fp8 = None  # a single name is a common slip: refused, not read as its characters
+    try:
+        names = list(fp8)
+    except TypeError:
+        problems.append("fp8 must be an iterable of tensor names")
+        return {}
+    if not (isinstance(scale_block, (tuple, list)) and len(scale_block) == 2 and
+            all(b is None or (isinstance(b, int) and not isinstance(b, bool) and b >= 1) for b in scale_block)):
+        problems.append(f"scale_block {scale_block!r} must be (rows, columns), each an int >= 1 or None (the whole "
+                        f"dimension)")
+    if not isinstance(scale_suffix, str):
+        problems.append(f"scale_suffix must be a str, got {scale_suffix!r}")
+        scale_suffix = None
+    want, codes = set(), cast_dtypes()
+    for n in names:
+        if n in want:
+            problems.append(f"{n!r} is in fp8 twice")
+        elif not isinstance(n, str) or n not in tensors:
+            problems.append(f"{n!r} is in fp8 but not in the tensors")
+        else:
+            want.add(n)
+    owners: dict = {}  # storage -> names
+    for n, t in tensors.items():
+        if isinstance(t, torch.Tensor) and t.untyped_storage().nbytes():
+            owners.setdefault((t.device, t.untyped_storage().data_ptr()), []).append(n)
+    plan = {}
+    for n, t in tensors.items():
+        if n not in want:
+            continue
+        if not isinstance(t, torch.Tensor) or t.dim() != 2 or t.numel() == 0:
+            problems.append(f"{n!r} is not a non-empty 2-D tensor; fp8 quantizes 2-D weights")
+        elif t.dtype not in codes:
+            problems.append(f"{n!r} is {t.dtype}; only float32, float16 and bfloat16 weights quantize")
+        else:
+            others = [o for o in owners.get((t.device, t.untyped_storage().data_ptr()), []) if o != n]
+            if others:
+                problems.append(f"{n!r} shares its storage with {', '.join(map(repr, others))}; a quantized weight "
+                                f"must have a storage of its own")
+        if isinstance(dtype, Mapping) and n in dtype:
+            problems.append(f"{n!r} is in both fp8 and dtype")
+        if scale_suffix is not None:
+            if n + scale_suffix in tensors:
+                problems.append(f"the scale of {n!r}, {n + scale_suffix!r}, is already a tensor name")
+            plan[n] = n + scale_suffix
+    return plan
+
+
+def _fp8_targets(label: str, tensors: Mapping, dtype, plan: dict, problems: list) -> dict:
+    """``cast_targets`` of the tensors that do not quantize (a ``dtype`` mapping without the quantized names); its
+    problems go to ``problems``."""
+    if dtype is None:
+        return {}
+    rest = {k: v for k, v in dtype.items() if k not in plan} if isinstance(dtype, Mapping) else dtype
+    try:
+        return cast_targets(label, rest, [(n, t.dtype, t.shape, 0, None) for n, t in tensors.items() if n not in plan],
+                            0)
+    except ValueError as exc:
+        problems.append(str(exc))
+        return {}
 
 
 def load_cast_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> Loaded:
@@ -950,7 +1046,8 @@ class DeviceFile(io.RawIOBase):
         self._pos = 0
 
     @classmethod
-    def safetensors(cls, tensors: Mapping, metadata: Mapping | None = None, *, dtype=None, ctx=None,
+    def safetensors(cls, tensors: Mapping, metadata: Mapping | None = None, *, dtype=None, fp8=None,
+                    scale_block=(128, 128), scale_suffix: str = "_scale_inv", ctx=None,
                     bounce_bytes: int = BOUNCE_BYTES) -> "DeviceFile":
         """A file whose bytes are the safetensors image of ``tensors`` (``safetensors.torch.save(tensors, metadata)``),
         made of the tensors where they are: the header is built on the host and copied to the device once, every tensor
@@ -966,7 +1063,38 @@ class DeviceFile(io.RawIOBase):
         ``b200h_copy_cast_ranges``), so HBM holds only the tensors, the header and the digest tables.  A tensor
         already in its target dtype is taken as it is.  Every problem (another floating dtype under a single
         ``dtype``, names not in ``tensors``, unsupported sources or targets) is reported in one ``ValueError`` before
-        anything is copied to the device."""
+        anything is copied to the device.
+
+        ``fp8`` (an iterable of names of 2-D float32 / float16 / bfloat16 weights) exports those weights as FP8 E4M3
+        with block scales, the layout DeepSeek-V3 and the Qwen3 FP8 checkpoints use and ``volume.read_safetensors(...,
+        scales=volume.fp8_scales(names, scale_suffix))`` loads: every weight ``w`` is stored as ``F8_E4M3`` and gets an
+        F32 tensor ``w + scale_suffix`` of shape ``[ceil(R / rows), ceil(C / columns)]`` for ``scale_block = (rows,
+        columns)``, ``None`` meaning the whole dimension (``(1, None)``: per channel; ``(None, None)``: per tensor).
+        Element x of block b becomes ``E4M3(x * (448 / a_b))`` and the scale ``a_b / 448``, with ``a_b`` the block's
+        amax clamped to at least 1e-4: bit for bit what the widely copied ``per_block_cast_to_fp8`` computes in torch on
+        CUDA.  The file is exactly ``safetensors.torch.save(ref, metadata)``, where ``ref`` is ``tensors`` with every
+        quantized weight replaced and its scale inserted right after it, and the other tensors converted by ``dtype``
+        as above.  The scales are computed on the device at construction (ONE ``b200h_fp8_block_scales`` call on the
+        current stream, which does not wait for the GPU) into scale tensors that are segments of the file, plus one F32
+        value per block kept for the quantization; no quantized copy of a weight is made: the weights are quantized as
+        the file's blocks are hashed, staged or read (``b200h_hash_scaled_segment_parts_device``,
+        ``b200h_copy_scaled_ranges``).  The weights must not change while the file is read.  Every problem (see
+        ``_fp8_plan``) comes in one ``ValueError`` before anything is copied to the device."""
+        if fp8 is not None:
+            safetensors_layout(tensors, metadata)  # the names, metadata and dtypes, checked before the rest
+            problems = []
+            plan = _fp8_plan(tensors, dtype, fp8, scale_block, scale_suffix, problems)
+            targets = _fp8_targets("DeviceFile.safetensors", tensors, dtype, plan, problems)
+            if problems:
+                raise ValueError("DeviceFile.safetensors: " + "; ".join(problems))
+            if plan:
+                for name, t in tensors.items():
+                    ctx = cls._Source._check_tensor(t, ctx, f"DeviceFile.safetensors[{name!r}]")
+                ctx = ctx or get_context()
+                quant, amax = cls._fp8_scales(tensors, plan, scale_block, ctx)
+                plain = {plan[n] if n in plan else n: quant[n][0] if n in plan else t for n, t in tensors.items()}
+                return cls._safetensors_scaled(plain, {w: (tensors[w], quant[w][1]) for w in plan}, metadata, targets,
+                                               amax, ctx, bounce_bytes)
         if dtype is not None:
             safetensors_layout(tensors, metadata)  # the names, metadata and dtypes, checked before the targets
             targets = cast_targets("DeviceFile.safetensors", dtype,
@@ -1000,8 +1128,60 @@ class DeviceFile(io.RawIOBase):
         return cls._over(cls._Source(segments, bounce_bytes, casts, ctx))
 
     @classmethod
+    def _fp8_scales(cls, tensors: Mapping, plan: dict, scale_block, ctx):
+        """({weight: (scale tensor, (amax_ptr, scale_count, R, C, block_rows, block_cols))}, the amax buffer) of the
+        weights of ``plan``: ONE ``fp8_block_scales`` call on the current stream.  Every scale tensor has a storage of
+        its own; the amax values of every weight lie back to back in one buffer, so the call makes one memset."""
+        import torch
+
+        codes, jobs, out, at = cast_dtypes(), [], {}, 0
+        grids = {w: tuple(1 if b is None else -(-d // b) for d, b in zip(tensors[w].shape, scale_block)) for w in plan}
+        amax = cls._Source._new_tensor((sum(g[0] * g[1] for g in grids.values()),), torch.float32, ctx)
+        for w in plan:
+            t, (g0, g1) = tensors[w], grids[w]
+            (R, C), n = t.shape, g0 * g1
+            br, bc = (R if scale_block[0] is None else scale_block[0]), (C if scale_block[1] is None else scale_block[1])
+            s, a = cls._Source._new_tensor((g0, g1), torch.float32, ctx), amax[at : at + n]
+            jobs.append((t.data_ptr(), codes[t.dtype], R, C, br, bc, s.data_ptr(), a.data_ptr()))
+            out[w] = (s, (a.data_ptr(), n, R, C, br, bc))
+            at += n
+        ctx.fp8_block_scales(jobs, cls._Source._current_stream(ctx))
+        return out, amax
+
+    @classmethod
+    def _safetensors_scaled(cls, plain: Mapping, quant: Mapping, metadata, targets: dict, amax, ctx,
+                            bounce_bytes: int = BOUNCE_BYTES) -> "DeviceFile":
+        """The file of ``plain`` (tensors stored as they are, or converted to ``targets``; scale tensors among them)
+        and ``quant`` ({weight: (tensor, its scales as ``_TensorBytes`` takes them)}, stored as F8_E4M3): the layout is
+        that of ``meta`` stand-ins, and each quantized weight is a segment of the file that quantizes."""
+        import torch
+
+        stand_ins = {name: torch.empty(t.shape, dtype=targets[name], device="meta") if name in targets else t
+                     for name, t in plain.items()}
+        stand_ins.update({w: torch.empty(t.shape, dtype=torch.float8_e4m3fn, device="meta") for w, (t, _) in
+                          quant.items()})
+        header, ordered = safetensors_layout(stand_ins, metadata)
+        codes = cast_dtypes()
+        segments, casts, scales = [cls._Source._to_device(header, ctx)], [(0, 0)], [None]
+        for name, _ in ordered:
+            if name in quant:
+                t, q = quant[name]
+                segments.append(t)
+                casts.append((codes[t.dtype], _lib.DT_F8E4M3))
+                scales.append(q)
+                continue
+            t = plain[name]
+            segments.append(t)
+            casts.append((codes[t.dtype], codes[targets[name]]) if name in targets else (0, 0))
+            scales.append(None)
+        src = cls._Source(segments, bounce_bytes, casts, ctx, scales)
+        src.keep = amax
+        return cls._over(src)
+
+    @classmethod
     def safetensors_shards(cls, state_dict: Mapping, *, filename_pattern: str = "model{suffix}.safetensors",
-                           max_shard_size="5GB", metadata: Mapping | None = None, dtype=None,
+                           max_shard_size="5GB", metadata: Mapping | None = None, dtype=None, fp8=None,
+                           scale_block=(128, 128), scale_suffix: str = "_scale_inv",
                            shared_tensors_to_discard=None, ctx=None) -> SafetensorsShards:
         """A checkpoint in the Hugging Face Hub's sharded layout, made of the tensors where they are: every file's
         bytes are exactly what ``huggingface_hub.save_torch_state_dict(state_dict, d, filename_pattern=...,
@@ -1022,6 +1202,11 @@ class DeviceFile(io.RawIOBase):
         storage converted once, so tensors that share one still do, as in ``model.to(dtype).state_dict()`` -- split
         on the converted sizes, and every shard converts its elements on the device as it is read, never making a
         converted copy.  Names that share a storage must convert to one dtype.
+
+        ``fp8``, ``scale_block`` and ``scale_suffix`` are ``DeviceFile.safetensors``'s: the files are then the Hub's of
+        the quantized checkpoint (every scale right after its weight in key order, split on the quantized sizes, so a
+        scale may land in another shard than its weight), with the scales of the whole state dict computed by ONE
+        ``b200h_fp8_block_scales`` call before the split.
 
         Every problem is reported in one ``ValueError`` before anything is copied to the device: a pattern without
         ``{suffix}``, a bad ``max_shard_size``, non-contiguous tensors (the Hub copies them; this call makes no copies
@@ -1051,8 +1236,11 @@ class DeviceFile(io.RawIOBase):
                 valid[name] = t
             except ValueError as exc:
                 problems.append(str(exc))
-        targets = {}
-        if dtype is not None and len(valid) == len(state_dict):
+        targets, plan = {}, {}
+        if fp8 is not None and len(valid) == len(state_dict):
+            plan = _fp8_plan(state_dict, dtype, fp8, scale_block, scale_suffix, problems)
+            targets = _fp8_targets("safetensors_shards", state_dict, dtype, plan, problems)
+        elif dtype is not None and len(valid) == len(state_dict):
             try:
                 targets = cast_targets("safetensors_shards", dtype,
                                        [(name, t.dtype, t.shape, 0, None) for name, t in state_dict.items()], 0)
@@ -1074,7 +1262,12 @@ class DeviceFile(io.RawIOBase):
                 meta.setdefault(n, keep)
         removed = {n for gone in remove.values() for n in gone}
         kept = {n: t for n, t in state_dict.items() if n not in removed}
-        sizes = {n: t.untyped_storage().nbytes() // t.element_size() * targets[n].itemsize if n in targets else
+        quant, amax = cls._fp8_scales(kept, plan, scale_block, ctx) if plan else ({}, None)
+        if plan:  # every scale right after its weight: the key order the split follows
+            kept = {k: v for n, t in kept.items() for k, v in ([(n, t), (plan[n], quant[n][0])] if n in plan else
+                                                                [(n, t)])}
+        sizes = {n: t.numel() if n in quant else
+                 t.untyped_storage().nbytes() // t.element_size() * targets[n].itemsize if n in targets else
                  t.untyped_storage().nbytes() for n, t in kept.items()}
         ids = {n: (t.device, t.untyped_storage().data_ptr(), sizes[n]) for n, t in kept.items()}
         split, total = _hub_split(sizes, ids, filename_pattern, max_size)
@@ -1082,7 +1275,12 @@ class DeviceFile(io.RawIOBase):
         files = {}
         for fname, names in split.items():
             conv = {n: targets[n] for n in names if n in targets}
-            files[fname] = cls.safetensors({n: kept[n] for n in names}, file_meta, dtype=conv or None, ctx=ctx)
+            if plan:
+                files[fname] = cls._safetensors_scaled(
+                    {n: kept[n] for n in names if n not in quant}, {n: (kept[n], quant[n][1]) for n in names if n in quant},
+                    file_meta, conv, amax, ctx)
+            else:
+                files[fname] = cls.safetensors({n: kept[n] for n in names}, file_meta, dtype=conv or None, ctx=ctx)
         index = None
         if len(split) > 1:
             body = {"metadata": {"total_size": total, **meta},

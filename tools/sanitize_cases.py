@@ -21,6 +21,10 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
   scaled boxes load_scaled_boxes_kernel: FP8 boxes of every format, target and scale type, each scale tensor an
                exact-size allocation with partial last blocks; the last box reads the last element, source byte and
                scale, checked against the integer-exact reference of tests/test_fp8_reference_cpu.py
+  fp8 export   fp8_amax_kernel / fp8_finalize_kernel (b200h_fp8_block_scales) and stage_scaled_ranges_kernel: weights
+               of every source type that are exact-size allocations at every element phase, partial last blocks, the
+               atomicMax of many CTAs into one per-tensor scale; ranges at every image offset into page-locked host
+               memory and device memory, checked against torch's per_block_cast_to_fp8 on CUDA
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -277,5 +281,46 @@ for (_, _, width, rows, s_at, pitch, fc, tc, _, sc, _, first, R, C, br, bc), (at
     assert torch.equal(got[~nan], ref[~nan]) and bool(is_nan_bits(got[nan], names[tc]).all()), (fc, tc, sc, R, C)
 ctx.host_free(src)
 print("scaled boxes ok", flush=True)
+
+# 11. FP8 export: the scale call and the quantizing copies over exact-size allocations
+from safetensors.torch import save as st_save  # noqa: E402
+
+from modal_client_b200 import DeviceFile, stage_ranges  # noqa: E402
+
+sd, fp8 = {}, []
+for k, (dt, shape) in enumerate([(torch.float32, (37, 29)), (torch.float16, (130, 141)), (torch.bfloat16, (5, 1001)),
+                                 (torch.bfloat16, (1 << 10, 1 << 9))]):
+    sd[f"w{k}"] = torch.randn(*shape, generator=g).to(dt).cuda()  # its own allocation, sized exactly
+    fp8.append(f"w{k}")
+sd["norm"] = torch.ones(29, dtype=torch.float32).cuda()
+for block in ((128, 128), (7, 5), (None, None)):
+    f = DeviceFile.safetensors(sd, fp8=fp8, scale_block=block, ctx=ctx)
+    ref = {}
+    for n, t in sd.items():
+        if n not in fp8:
+            ref[n] = t.cpu()
+            continue
+        R, C = t.shape
+        bR, bC = block[0] or R, block[1] or C
+        padded = t.new_zeros(-(-R // bR) * bR, -(-C // bC) * bC)
+        padded[:R, :C] = t
+        v = padded.view(-(-R // bR), bR, -(-C // bC), bC)
+        amax = v.abs().float().amax(dim=(1, 3), keepdim=True).clamp(1e-4)
+        q = (v * (448.0 / amax)).to(torch.float8_e4m3fn).view(padded.shape)[:R, :C].contiguous()
+        ref[n], ref[n + "_scale_inv"] = q.cpu(), (amax / 448.0).view(-(-R // bR), -(-C // bC)).cpu()
+    want = np.frombuffer(st_save(ref), np.uint8)
+    assert f.nbytes == want.size
+    ranges = [(0, 0, want.size)] + [(0, o, min(777, want.size - o)) for o in range(1, want.size, want.size // 37)]
+    offsets = [sum(-(-n // 16) * 16 for _, _, n in ranges[:i]) for i in range(len(ranges))]
+    total = offsets[-1] + -(-ranges[-1][2] // 16) * 16
+    pinned = ctx.host_alloc(total)
+    device = torch.empty(total, dtype=torch.uint8, device="cuda")
+    for dst in (pinned, device):
+        stage_ranges([f], ranges, dst, offsets, ctx=ctx).wait()
+        got = dst if isinstance(dst, np.ndarray) else dst.cpu().numpy()
+        for (_, o, n), at in zip(ranges, offsets):
+            assert np.array_equal(got[at : at + n], want[o : o + n]), (block, o, n)
+    ctx.host_free(pinned)
+print("fp8 export ok", flush=True)
 ctx.close()
 print("ALL OK")
