@@ -384,7 +384,13 @@ int b200h_hash_cast_segment_parts_device(b200h_ctx* ctx, const b200h_cast_segmen
  *   s = a * RN(1 / 448)                                               (the F32 scale stored next to the weight)
  *   m = RN(RN(1 / a) * 448)                                           (the multiplier: from a, never from s)
  *   q = E4M3(RN(float(x) * m))                                        (round to nearest even, subnormals kept)
- * A block holding an infinity has s = inf and m = 0: its finite elements give +-0, its infinities (inf * 0) NaN. */
+ * A block holding an infinity has s = inf and m = 0: its finite elements give +-0, its infinities (inf * 0) NaN.
+ * NaN bits: a NaN a is the block's largest |x| pattern widened to F32 (an F32 or BF16 payload kept, signalling ones
+ * included; every F16 NaN widens to 0x7FFFFFFF), and its s is 0x7FFFFFFF.  Every NaN product gives q = 0x7F, whatever
+ * the sign of the NaN.
+ * The conversion saturates (satfinite): with a block's own a no product reaches 448 by more than rounding, but the
+ * quantizing copies take the a they are given, and with an a below the block's max every product of magnitude 448 or
+ * more gives 0x7E / 0xFE (+-448), +-inf * m (m > 0) included; torch's conversion gives NaN from 464 on instead. */
 
 /* One weight of b200h_fp8_block_scales.  s and a hold ceil(R / block_rows) x ceil(C / block_cols) F32 values each,
  * row-major: d_scales receives s (the weight's scale tensor), d_amax receives a (kept for the quantizing copies). */

@@ -23,8 +23,9 @@ for compute-sanitizer (memcheck / racecheck / synccheck slow kernels down 10-100
                scale, checked against the integer-exact reference of tests/test_fp8_reference_cpu.py
   fp8 export   fp8_amax_kernel / fp8_finalize_kernel (b200h_fp8_block_scales) and stage_scaled_ranges_kernel: weights
                of every source type that are exact-size allocations at every element phase, partial last blocks, the
-               atomicMax of many CTAs into one per-tensor scale; ranges at every image offset into page-locked host
-               memory and device memory, checked against torch's per_block_cast_to_fp8 on CUDA
+               atomicMax of many CTAs into one per-tensor scale, blocks that span two amax tiles beside neighbour
+               blocks; ranges at every image offset into page-locked host memory and device memory, checked against
+               the integer-exact reference of tests/test_fp8_quant_reference_cpu.py
 Digests are compared with hashlib, so a sanitizer run is also a parity run.
   compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
   compute-sanitizer --tool racecheck python tools/sanitize_cases.py"""
@@ -282,18 +283,20 @@ for (_, _, width, rows, s_at, pitch, fc, tc, _, sc, _, first, R, C, br, bc), (at
 ctx.host_free(src)
 print("scaled boxes ok", flush=True)
 
-# 11. FP8 export: the scale call and the quantizing copies over exact-size allocations
+# 12. FP8 export: the scale call and the quantizing copies over exact-size allocations, one block form (3, 4097) whose
+#     blocks span two amax tiles and have neighbours in both directions; checked against the integer-exact reference
 from safetensors.torch import save as st_save  # noqa: E402
 
 from modal_client_b200 import DeviceFile, stage_ranges  # noqa: E402
+from tests.test_fp8_quant_reference_cpu import reference_block_scales, reference_multiplier, reference_quant  # noqa: E402
 
 sd, fp8 = {}, []
 for k, (dt, shape) in enumerate([(torch.float32, (37, 29)), (torch.float16, (130, 141)), (torch.bfloat16, (5, 1001)),
-                                 (torch.bfloat16, (1 << 10, 1 << 9))]):
+                                 (torch.bfloat16, (1 << 10, 1 << 9)), (torch.float32, (8, 8300))]):
     sd[f"w{k}"] = torch.randn(*shape, generator=g).to(dt).cuda()  # its own allocation, sized exactly
     fp8.append(f"w{k}")
 sd["norm"] = torch.ones(29, dtype=torch.float32).cuda()
-for block in ((128, 128), (7, 5), (None, None)):
+for block in ((128, 128), (7, 5), (None, None), (3, 4097)):
     f = DeviceFile.safetensors(sd, fp8=fp8, scale_block=block, ctx=ctx)
     ref = {}
     for n, t in sd.items():
@@ -301,13 +304,14 @@ for block in ((128, 128), (7, 5), (None, None)):
             ref[n] = t.cpu()
             continue
         R, C = t.shape
-        bR, bC = block[0] or R, block[1] or C
-        padded = t.new_zeros(-(-R // bR) * bR, -(-C // bC) * bC)
-        padded[:R, :C] = t
-        v = padded.view(-(-R // bR), bR, -(-C // bC), bC)
-        amax = v.abs().float().amax(dim=(1, 3), keepdim=True).clamp(1e-4)
-        q = (v * (448.0 / amax)).to(torch.float8_e4m3fn).view(padded.shape)[:R, :C].contiguous()
-        ref[n], ref[n + "_scale_inv"] = q.cpu(), (amax / 448.0).view(-(-R // bR), -(-C // bC)).cpu()
+        bR, bC = min(block[0] or R, R), min(block[1] or C, C)
+        bits = t.cpu().view(torch.int32 if t.dtype == torch.float32 else torch.int16).to(torch.int64).reshape(-1)
+        bits &= (1 << (8 * t.element_size())) - 1
+        a, s = reference_block_scales(bits, t.dtype, R, C, (bR, bC))
+        e = torch.arange(R * C)
+        q = reference_quant(bits, t.dtype, reference_multiplier(a.reshape(-1))[e // C // bR * a.shape[1] + e % C // bC])
+        ref[n] = q.to(torch.uint8).view(torch.float8_e4m3fn).view(R, C)
+        ref[n + "_scale_inv"] = s.to(torch.int32).view(torch.float32)
     want = np.frombuffer(st_save(ref), np.uint8)
     assert f.nbytes == want.size
     ranges = [(0, 0, want.size)] + [(0, o, min(777, want.size - o)) for o in range(1, want.size, want.size // 37)]
