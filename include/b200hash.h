@@ -450,6 +450,69 @@ int b200h_hash_scaled_segment_parts_device(b200h_ctx* ctx, const b200h_scaled_se
                                            uint32_t flags, void* d_sha256, void* d_md5, uint64_t* d_trimmed_len,
                                            uint64_t* nparts_out, void* cuda_stream);
 
+/* ---- FP8 load: weights quantized as they arrive from page-locked host memory ---------------------------------------
+ *
+ * The numerical contract is the export's (above): a, s, m and q bit for bit as b200h_fp8_block_scales and the
+ * quantizing copies give them.  A block's s depends on every element of the block, so a weight that arrives in pieces
+ * is quantized in two calls per piece of staging: b200h_fp8_amax_boxes_from_host reduces the amax of the elements that
+ * have arrived into a, and once every element of a block row (a "band") has arrived, b200h_copy_quant_boxes_from_host
+ * finalizes the band's a and s and writes its E4M3 codes. */
+
+/* A box of F32 / F16 / BF16 elements quantized to E4M3: `cast` as in b200h_cast_box with cast.src_type B200H_DT_F32,
+ * F16 or BF16 and cast.dst_type B200H_DT_F8E4M3 (one destination byte per element).  The box is cut from the R x C
+ * row-major weight W (rows_total = R, cols = C): the element at source byte c of its row r is W's element first_elem +
+ * (r * src_pitch + c) / (source element size).  d_amax holds W's a: scale_count F32 values, ceil(R / block_rows) x
+ * ceil(C / block_cols) of them used, row-major (a block size of R or more, C or more, is the whole dimension). */
+typedef struct b200h_quant_box {
+    b200h_cast_box cast;
+    float* d_amax;
+    uint64_t scale_count;
+    uint64_t first_elem;
+    uint64_t rows_total, cols;
+    uint64_t block_rows, block_cols;
+} b200h_quant_box;
+
+/* count consecutive blocks to finalize: d_amax[k] = NaN ? d_amax[k] : max(d_amax[k], 1e-4f) in place, and
+ * d_scales[k] = d_amax[k] * RN(1 / 448), for k < count (fp8_finalize_kernel's rules). */
+typedef struct b200h_fp8_band {
+    float* d_amax;
+    float* d_scales;
+    uint64_t count;
+} b200h_fp8_band;
+
+/* The amax of every element of box i of h_src, max-reduced into its block's d_amax value: an integer max over the bits
+ * of |x| widened to F32, exactly as b200h_fp8_block_scales reduces it.  The max is order-independent, so the elements
+ * of a block may arrive over any number of calls (d_amax starts as zeros; the caller clears it).  Nothing but d_amax is
+ * written; the destinations in segs are checked, not written, so that the amax and the copy take the same boxes.
+ * Every argument is checked before anything is enqueued, B200H_E_INVALID otherwise: every rule of
+ * b200h_copy_cast_boxes_from_host (destinations measured in one byte per element), and further: src_type F32, F16 or
+ * BF16 and dst_type B200H_DT_F8E4M3; block sizes >= 1; scale_count >= ceil(R / block_rows) * ceil(C / block_cols);
+ * every element a box touches below R * C (both without overflow); d_amax 4-byte aligned, and its scale_count values
+ * device memory of the context's device.
+ * ONE kernel launch (fp8_amax_boxes_kernel) per call, none when every box is empty; within the call source words cross
+ * PCIe once, in the loads of b200h_copy_boxes_from_host.  The copy of the same boxes (b200h_copy_quant_boxes_from_host)
+ * reads them again: quantizing on load takes every source byte across PCIe twice, once for the amax and once for the
+ * codes.  Only enqueues on `cuda_stream` (NULL = the context's compute stream). */
+int b200h_fp8_amax_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                   const uint64_t* file_first_seg, uint64_t nfiles, const b200h_quant_box* boxes,
+                                   uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream);
+
+/* The bands' a and s finalized (b200h_fp8_band), then every element x of box i of h_src written to its destination as
+ * q = E4M3(RN(float(x) * m)), m = RN(RN(1 / a) * 448) from its block's finalized a: what the FP8 export stores for the
+ * weight, once every element of the boxes' blocks has gone through b200h_fp8_amax_boxes_from_host and been finalized
+ * (by this call or an earlier one).
+ * Every argument is checked before anything is enqueued, B200H_E_INVALID otherwise: every rule of
+ * b200h_fp8_amax_boxes_from_host for segs and boxes, and for every band: count >= 1, d_amax and d_scales not NULL,
+ * 4-byte aligned, their count values device memory of the context's device (both without overflow).
+ * Enqueues on `cuda_stream` (NULL = the context's compute stream): one launch (fp8_finalize_kernel) when nbands > 0, then
+ * one (load_quant_boxes_kernel) when a box is not empty; it never synchronises.
+ * Replaces: loading a bfloat16 checkpoint into HBM and quantizing it per weight in torch (per_block_cast_to_fp8), which
+ * holds the whole bfloat16 image and F32 temporaries of 4x a weight in HBM besides the FP8 results. */
+int b200h_copy_quant_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                     const uint64_t* file_first_seg, uint64_t nfiles, const b200h_quant_box* boxes,
+                                     uint64_t nboxes, const b200h_fp8_band* bands, uint64_t nbands, const void* h_src,
+                                     uint64_t h_src_bytes, void* cuda_stream);
+
 /* ---- files (native reader pool; no Python I/O, no mmap) ------------------------------------------ */
 
 /* Sizes (and permission bits, may be NULL) of n regular files, stat'ed by the library's I/O threads.

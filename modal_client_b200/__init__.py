@@ -10,5 +10,6 @@ __version__ = "0.1.0"
 
 from . import _lib  # noqa: F401  (symbols only; touching the GPU happens on first use)
 from .batch import DigestTable, hash_table_buffers, hash_table_host  # noqa: F401
-from .device_file import DeviceFile, load_boxes, load_cast_boxes, load_ranges, load_scaled_boxes, stage_ranges  # noqa: F401
+from .device_file import (DeviceFile, load_boxes, load_cast_boxes, load_fp8_amax_boxes, load_quant_boxes,  # noqa: F401
+                          load_ranges, load_scaled_boxes, stage_ranges)
 from .hash_utils import UploadHashes, get_upload_hashes, get_upload_hashes_many  # noqa: F401

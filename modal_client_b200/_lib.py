@@ -40,6 +40,7 @@ ABI_SYMBOLS = (
     "b200h_copy_cast_boxes_from_host", "b200h_copy_cast_ranges", "b200h_hash_cast_segment_parts_device",
     "b200h_cast_segment_parts_preview", "b200h_copy_scaled_boxes_from_host", "b200h_fp8_block_scales",
     "b200h_copy_scaled_ranges", "b200h_hash_scaled_segment_parts_device", "b200h_scaled_segment_parts_preview",
+    "b200h_fp8_amax_boxes_from_host", "b200h_copy_quant_boxes_from_host",
 )
 
 
@@ -125,6 +126,10 @@ def load_library() -> ctypes.CDLL:
         L.b200h_copy_cast_boxes_from_host.restype = i32
         L.b200h_copy_scaled_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
         L.b200h_copy_scaled_boxes_from_host.restype = i32
+        L.b200h_fp8_amax_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp]
+        L.b200h_fp8_amax_boxes_from_host.restype = i32
+        L.b200h_copy_quant_boxes_from_host.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, u64, vp]
+        L.b200h_copy_quant_boxes_from_host.restype = i32
         L.b200h_copy_cast_ranges.argtypes = [vp, vp, u64, vp, u64, vp, u64, vp, u64, vp, vp]
         L.b200h_copy_cast_ranges.restype = i32
         L.b200h_hash_cast_segment_parts_device.argtypes = [vp, vp, u64, vp, u64, u64, u32, vp, vp, vp,
@@ -640,14 +645,34 @@ class Context:
         self._copy_boxes("b200h_copy_scaled_boxes_from_host", 16, seg_ptrs, seg_lens, file_first_seg, boxes, src,
                          stream)
 
+    def fp8_amax_boxes_from_host(self, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
+                                 stream: int = 0) -> None:
+        """The amax of boxes of F32 / F16 / BF16 weights in ``src`` into each weight's a: box i = ``(file, offset,
+        width, rows, src_offset, src_pitch, src_type, DT_F8E4M3, amax_ptr, scale_count, first_elem, R, C, block_rows,
+        block_cols)``; the element at source byte c of row r is element ``first_elem + (r * src_pitch + c) / itemsize``
+        of the R x C weight, and the bits of its |x| widened to F32 are max-reduced into its block's value of the
+        ``scale_count`` F32 values at device address ``amax_ptr``.  The destinations are checked as for the copy, not
+        written.  One kernel launch, only enqueued on ``stream``."""
+        self._copy_boxes("b200h_fp8_amax_boxes_from_host", 15, seg_ptrs, seg_lens, file_first_seg, boxes, src, stream)
+
+    def copy_quant_boxes_from_host(self, seg_ptrs, seg_lens, file_first_seg, boxes, bands, src: np.ndarray,
+                                   stream: int = 0) -> None:
+        """Band i = ``(amax_ptr, scales_ptr, count)`` finalized (a clamped in place, s = a * RN(1 / 448)), then the
+        boxes of ``fp8_amax_boxes_from_host`` quantized to E4M3 with their blocks' a and written packed, one byte per
+        element, from byte ``offset`` of their files.  A launch for the bands and one for the boxes, only enqueued on
+        ``stream``."""
+        bd = np.ascontiguousarray(bands, dtype=np.uint64).reshape(-1, 3)
+        self._copy_boxes("b200h_copy_quant_boxes_from_host", 15, seg_ptrs, seg_lens, file_first_seg, boxes, src, stream,
+                         (_np_ptr(bd) if len(bd) else None, len(bd)))
+
     def _copy_boxes(self, entry: str, width: int, seg_ptrs, seg_lens, file_first_seg, boxes, src: np.ndarray,
-                    stream: int) -> None:
+                    stream: int, extra=()) -> None:
         segs = _segments(seg_ptrs, seg_lens)
         ffs, nfiles = _segment_args(file_first_seg)
         bx = np.ascontiguousarray(boxes, dtype=np.uint64).reshape(-1, width)
         rc = getattr(self._L, entry)(self._h, _np_ptr(segs) if len(segs) else None, len(segs), _np_ptr(ffs), nfiles,
-                                     _np_ptr(bx) if len(bx) else None, len(bx), ctypes.c_void_p(src.ctypes.data),
-                                     src.size, stream or None)
+                                     _np_ptr(bx) if len(bx) else None, len(bx), *extra,
+                                     ctypes.c_void_p(src.ctypes.data), src.size, stream or None)
         self._check(rc, entry)
 
     def _copy_ranges(self, entry: str, offsets_name: str, seg_ptrs, seg_lens, file_first_seg, ranges, host: np.ndarray,

@@ -1906,13 +1906,44 @@ static std::string scaled_box_fault(const b200h_scaled_box& x) {
     return "";
 }
 
+// The rules of a quantizing box that need no device: its types, block sizes, the scale count, a's alignment and the
+// weight's bounds.
+static std::string quant_box_fault(const b200h_quant_box& x) {
+    const b200h_box& b = x.cast.box;
+    const uint64_t ss = dt_bytes(x.cast.src_type);
+    if (!ss) return ": src_type is not F32, F16 or BF16";
+    if (x.cast.dst_type != B200H_DT_F8E4M3) return ": dst_type is not B200H_DT_F8E4M3";
+    if (!x.rows_total || !x.cols) return ": R and C must be >= 1";
+    if (!x.block_rows || !x.block_cols) return ": block sizes must be >= 1";
+    const unsigned __int128 nscales =
+        (unsigned __int128)ceil_div(x.rows_total, x.block_rows) * ceil_div(x.cols, x.block_cols);
+    if (nscales > x.scale_count) return ": scale_count is less than ceil(R / block_rows) * ceil(C / block_cols)";
+    if (!x.d_amax || (uintptr_t)x.d_amax % 4) return ": d_amax is NULL or not 4-byte aligned";
+    if (b.rows && b.width) {  // first_elem + ((rows - 1) * src_pitch + width) / ss <= R * C
+        const unsigned __int128 end =
+            (unsigned __int128)x.first_elem + ((unsigned __int128)(b.rows - 1) * b.src_pitch + b.width) / ss;
+        if (end > (unsigned __int128)x.rows_total * x.cols) return ": it reaches past element R * C of its weight";
+    }
+    return "";
+}
+
+// The quantizing entries' own arguments: box i's weight and a (boxes[i] == quant.boxes[i].cast), the bands
+// b200h_copy_quant_boxes_from_host finalizes before its copy, and amax: b200h_fp8_amax_boxes_from_host.
+struct QuantArgs {
+    const b200h_quant_box* boxes;
+    const b200h_fp8_band* bands;
+    uint64_t nbands;
+    bool amax;
+};
+
 // b200h_copy_boxes_from_host (cast == false; every box has type code 0 on both sides),
 // b200h_copy_cast_boxes_from_host and b200h_copy_scaled_boxes_from_host (`scaled`: box i's scales, boxes[i] ==
 // scaled[i].cast): box i of h_src to its packed destination run, its elements converted when its types differ.
+// With `quant`, the amax of the boxes (quant->amax) or the bands' finalisation and the quantizing copy.
 static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint64_t nsegs,
                       const uint64_t* file_first_seg, uint64_t nfiles, const b200h_cast_box* boxes, uint64_t nboxes,
                       const void* h_src, uint64_t h_src_bytes, void* cuda_stream,
-                      const b200h_scaled_box* scaled = nullptr) {
+                      const b200h_scaled_box* scaled = nullptr, const QuantArgs* quant = nullptr) {
     std::vector<uint64_t> seg_lens;
     FileTable t;
     if (int rc = segment_file_table(ctx, segs, nsegs, file_first_seg, nfiles, seg_lens, t)) return rc;
@@ -1923,8 +1954,8 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
         const b200h_box& b = boxes[i].box;
         const std::string name = "box " + std::to_string(i);
         const uint64_t ss = box_elem_bytes(boxes[i].src_type), ds = box_elem_bytes(boxes[i].dst_type);
-        if (scaled) {
-            const std::string fault = scaled_box_fault(scaled[i]);
+        if (scaled || quant) {
+            const std::string fault = scaled ? scaled_box_fault(scaled[i]) : quant_box_fault(quant->boxes[i]);
             if (!fault.empty()) return fail(ctx, B200H_E_INVALID, name + fault);
         } else if (cast) {
             if (!dt_bytes(boxes[i].src_type) || !dt_bytes(boxes[i].dst_type))
@@ -1982,12 +2013,54 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
             seen.push_back(at);
         }
     }
-    if (nboxes == 0) return 0;
+    std::vector<ScaleJob> jobs;  // the bands to finalize (first_block, amax and scales)
+    uint64_t nblocks = 0;
+    if (quant) {  // every box's a, and every band's a and s, in device memory of ctx's device
+        std::vector<std::pair<uintptr_t, uint64_t>> seen;
+        for (uint64_t i = 0; i < nboxes; ++i) {
+            const b200h_quant_box& x = quant->boxes[i];
+            const std::pair<uintptr_t, uint64_t> at{(uintptr_t)x.d_amax, x.scale_count};
+            if (std::find(seen.end() - std::min<size_t>(seen.size(), 8), seen.end(), at) != seen.end()) continue;
+            if (x.scale_count > ~0ull / 4 || at.first + x.scale_count * 4 < at.first ||
+                !device_range_ok(ctx, x.d_amax, x.scale_count * 4))
+                return fail(ctx, B200H_E_INVALID, "box " + std::to_string(i) + ": its scale_count values at d_amax "
+                                                  "are not device memory of cuda:" + std::to_string(ctx->device));
+            seen.push_back(at);
+        }
+        if (quant->nbands && !quant->bands) return fail(ctx, B200H_E_INVALID, "bands must not be NULL");
+        if (quant->nbands > 0xffffffffull) return fail(ctx, B200H_E_INVALID, "too many bands");
+        for (uint64_t i = 0; i < quant->nbands; ++i) {
+            const b200h_fp8_band& x = quant->bands[i];
+            const std::string name = "band " + std::to_string(i);
+            if (!x.count) return fail(ctx, B200H_E_INVALID, name + ": count must be >= 1");
+            if (!x.d_amax || !x.d_scales || ((uintptr_t)x.d_amax | (uintptr_t)x.d_scales) % 4)
+                return fail(ctx, B200H_E_INVALID, name + ": d_amax and d_scales must be 4-byte aligned, not NULL");
+            if (x.count > ~0ull / 4 || (uintptr_t)x.d_amax + x.count * 4 < (uintptr_t)x.d_amax ||
+                (uintptr_t)x.d_scales + x.count * 4 < (uintptr_t)x.d_scales ||
+                !device_range_ok(ctx, x.d_amax, x.count * 4) || !device_range_ok(ctx, x.d_scales, x.count * 4))
+                return fail(ctx, B200H_E_INVALID, name + ": d_amax or d_scales is not device memory of cuda:" +
+                                                      std::to_string(ctx->device));
+            ScaleJob J{};
+            J.first_block = nblocks;
+            J.amax = (uint64_t)(uintptr_t)x.d_amax;
+            J.scales = (uint64_t)(uintptr_t)x.d_scales;
+            jobs.push_back(J);
+            nblocks += x.count;
+        }
+    }
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
+    auto finalize = [&]() -> int {  // the bands' a and s, before the copy that reads a
+        if (jobs.empty()) return 0;
+        return launch_with_tables(ctx, st, jobs, std::vector<uint8_t>{}, [&](const ScaleJob* d_jobs, const uint8_t*) {
+            return launch_fp8_finalize(d_jobs, (uint32_t)jobs.size(), nblocks, st);
+        });
+    };
+    if (nboxes == 0) return finalize();
     void* d_host = pinned_device_pointer(ctx, h_src, h_src_bytes);
     if (!d_host)
         return fail(ctx, B200H_E_INVALID,
                     "h_src is not page-locked host memory reachable from cuda:" + std::to_string(ctx->device));
-    if (!any) return 0;
+    if (!any) return finalize();
 
     // h_src may sit at any phase (a view into page-locked memory): the kernel reads aligned words from the aligned-down
     // base, so every source offset in the tables is taken from there.  The words it reads hold selected bytes, so they
@@ -2046,8 +2119,23 @@ static int copy_boxes(b200h_ctx* ctx, bool cast, const b200h_segment* segs, uint
         if (pieces[by_dev[k - 1]].dev + pieces[by_dev[k - 1]].len > pieces[by_dev[k]].dev)
             return fail(ctx, B200H_E_INVALID, "boxes " + std::to_string(box_of[by_dev[k - 1]]) + " and " +
                                                   std::to_string(box_of[by_dev[k]]) + " write the same device bytes");
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->s_comp;
     const void* d_src = (const uint8_t*)d_host - phase;
+    if (quant) {
+        std::vector<QuantTile> qt(tiles.size());
+        for (size_t k = 0; k < tiles.size(); ++k) {
+            const b200h_quant_box& x = quant->boxes[tile_of[k]];
+            const uint64_t bc = std::min(x.block_cols, x.cols), br = std::min(x.block_rows, x.rows_total);
+            qt[k] = {tiles[k], {(uint64_t)(uintptr_t)x.d_amax, x.first_elem, x.cols, br, bc, ceil_div(x.cols, bc)}};
+        }
+        if (quant->amax)
+            return launch_with_tables(ctx, st, qt, std::vector<uint8_t>{}, [&](const QuantTile* d_tiles, const uint8_t*) {
+                return launch_fp8_amax_boxes(d_tiles, qt.size(), d_src, st);
+            });
+        if (int rc = finalize()) return rc;
+        return launch_with_tables(ctx, st, qt, pieces, [&](const QuantTile* d_tiles, const RangePiece* d_pieces) {
+            return launch_load_quant_boxes(d_tiles, qt.size(), d_pieces, d_src, st);
+        });
+    }
     if (scaled) {
         std::vector<ScaledTile> sc(tiles.size());
         for (size_t k = 0; k < tiles.size(); ++k) {
@@ -2099,6 +2187,39 @@ int b200h_copy_scaled_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs,
     for (uint64_t i = 0; i < casts.size(); ++i) casts[i] = boxes[i].cast;
     return copy_boxes(ctx, true, segs, nsegs, file_first_seg, nfiles, boxes ? casts.data() : nullptr, nboxes, h_src,
                       h_src_bytes, cuda_stream, boxes);
+}
+
+// b200h_fp8_amax_boxes_from_host (bands == nullptr) and b200h_copy_quant_boxes_from_host.
+static int quant_boxes(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs, const uint64_t* file_first_seg,
+                       uint64_t nfiles, const b200h_quant_box* boxes, uint64_t nboxes, const b200h_fp8_band* bands,
+                       uint64_t nbands, bool amax, const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
+    if (nboxes && !boxes) return fail(ctx, B200H_E_INVALID, "boxes must not be NULL");
+    std::vector<b200h_cast_box> casts(boxes ? nboxes : 0);
+    for (uint64_t i = 0; i < casts.size(); ++i) casts[i] = boxes[i].cast;
+    const QuantArgs q{boxes, bands, nbands, amax};
+    return copy_boxes(ctx, true, segs, nsegs, file_first_seg, nfiles, boxes ? casts.data() : nullptr, nboxes, h_src,
+                      h_src_bytes, cuda_stream, nullptr, &q);
+}
+
+int b200h_fp8_amax_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                   const uint64_t* file_first_seg, uint64_t nfiles, const b200h_quant_box* boxes,
+                                   uint64_t nboxes, const void* h_src, uint64_t h_src_bytes, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_fp8_amax_boxes_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    return quant_boxes(ctx, segs, nsegs, file_first_seg, nfiles, boxes, nboxes, nullptr, 0, true, h_src, h_src_bytes,
+                       cuda_stream);
+}
+
+int b200h_copy_quant_boxes_from_host(b200h_ctx* ctx, const b200h_segment* segs, uint64_t nsegs,
+                                     const uint64_t* file_first_seg, uint64_t nfiles, const b200h_quant_box* boxes,
+                                     uint64_t nboxes, const b200h_fp8_band* bands, uint64_t nbands, const void* h_src,
+                                     uint64_t h_src_bytes, void* cuda_stream) {
+    if (!ctx) return B200H_E_INVALID;
+    B200H_RANGE("b200h_copy_quant_boxes_from_host");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    return quant_boxes(ctx, segs, nsegs, file_first_seg, nfiles, boxes, nboxes, bands, nbands, false, h_src,
+                       h_src_bytes, cuda_stream);
 }
 
 // ---------------------------------------------------------------------------------------------- files

@@ -216,6 +216,23 @@ struct ScaleJob {
 };
 // The amax reduction and the finalisation of a and s (two launches; amax must be zero before them).
 int launch_fp8_block_scales(const ScaleJob* jobs, uint32_t njobs, uint64_t ntiles, uint64_t nblocks, cudaStream_t st);
+// The finalisation alone (fp8_finalize_kernel; one launch, none when nblocks == 0): of the jobs only first_block, amax
+// and scales are read.
+int launch_fp8_finalize(const ScaleJob* jobs, uint32_t njobs, uint64_t nblocks, cudaStream_t st);
+
+// A tile of a box of F32 / F16 / BF16 elements quantized to E4M3 on the way in: `cast` as for CastTile (dst_type
+// B200H_DT_F8E4M3, one destination byte per element), and q as for a quantizing piece, with q.first_elem the weight's
+// element of the box's first source byte; the element of packed source byte p (row r, column c of the box) is
+// q.first_elem + r * box.pitch / ss + c / ss.  q.amax holds the weight's a.
+struct QuantTile {
+    CastTile cast;
+    PieceScale q;
+};
+// The amax of every tile's elements into q.amax (atomicMax over the bits of |x|; fp8_amax_boxes_kernel), and the
+// quantizing copy (load_quant_boxes_kernel) that reads the finalized a: one launch each, none when ntiles == 0.
+int launch_fp8_amax_boxes(const QuantTile* tiles, uint64_t ntiles, const void* src, cudaStream_t st);
+int launch_load_quant_boxes(const QuantTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
+                            cudaStream_t st);
 
 int chain_groups_per_cta();        // long messages one chain CTA can host (one CTA per SM)
 int device_sm_count();             // SMs of the current device (as seen by configure_kernels)

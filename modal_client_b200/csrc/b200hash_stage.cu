@@ -932,6 +932,190 @@ __global__ void __launch_bounds__(kScaleThreads)
     }
 }
 
+// ---- boxes of F32 / F16 / BF16 elements quantized to E4M3 on the way in (b200h_fp8_amax_boxes_from_host,
+//      b200h_copy_quant_boxes_from_host)
+//
+//   fp8_amax_boxes_kernel   the tiles, loads and ring of load_boxes_kernel; no device stores but the amax.  At each
+//                           step lane k takes the k-th 32nd of the elements whose source has arrived, contiguous, and
+//                           max-reduces the bits of |x| widened to F32 (as fp8_amax_kernel does) per block, following
+//                           the block with a cursor; where its elements leave a block it flushes with one atomicMax.
+//                           Its last block's value then goes through a warp reduction over the lanes that end in the
+//                           same block, and one lane per such run issues the atomicMax.
+//   load_quant_boxes_kernel the same tiles and ring with the store step of the cast boxes: a destination word is 16 E4M3
+//                           elements, 32 or 64 source bytes (three or five ring words with shift_bytes) when they are
+//                           one run of one row, element by element otherwise.  The multiplier and conversion are those
+//                           of stage_scaled_ranges_kernel (quant_seek / quant_next: m = RN(RN(1 / a) * 448), reloaded
+//                           only where j crosses a block-column edge or a row's end; FMUL without .FTZ; satfinite).
+// The a they read was finalized (fp8_finalize_kernel, launched by b200h_copy_quant_boxes_from_host before the copy).
+
+// Bits of |x| of the element of type st at byte `at` of a ring word, widened to F32.
+__device__ __forceinline__ uint32_t ring_abs_bits(const uint8_t* word, uint32_t at, uint32_t st) {
+    const uint32_t x = st == kDtF32 ? *reinterpret_cast<const uint32_t*>(word + at)
+                                    : (uint32_t)*reinterpret_cast<const uint16_t*>(word + at);
+    return __float_as_uint(widen_one(x, st)) & 0x7fffffffu;
+}
+
+// The amax of the box's elements whose packed source bytes lie in [from, upto) (clipped to [b.dlo, b.dhi)).
+__device__ __forceinline__ void amax_words_out(const BoxTile& b, uint32_t st, const PieceScale& q, const uint4* ring,
+                                               uint64_t from, uint64_t upto, uint32_t lane) {
+    const uint32_t ss = dt_bytes(st);
+    const uint64_t lo = max(from, b.dlo) / ss, hi = min(upto, b.dhi) / ss, welems = b.width / ss;
+    const uint64_t per = hi > lo ? (hi - lo + 31) / 32 : 0;
+    const uint64_t e0 = min(lo + lane * per, hi), e1 = min(e0 + per, hi);
+    float* amax = reinterpret_cast<float*>(q.amax);
+    uint64_t key = ~0ull;
+    uint32_t m = 0;
+    if (e0 < e1) {
+        uint64_t r = e0 / welems, c = e0 % welems;
+        QuantCursor cur;
+        bool seek = true;
+#pragma unroll 1
+        for (uint64_t e = e0; e < e1; ++e) {
+            bool load = seek;
+            if (seek) {  // the element's coordinates, once per lane and again where a box row ends
+                const uint64_t te = q.first_elem + r * (b.pitch / ss) + c;
+                cur.i = te / q.cols;
+                cur.j = te - cur.i * q.cols;
+                seek = false;
+            } else if (cur.j == cur.jend) {
+                if (cur.j == q.cols) cur.j = 0, ++cur.i;
+                load = true;
+            }
+            if (load) {
+                const uint64_t jb = cur.j / q.block_cols, k = cur.i / q.block_rows * q.scale_cols + jb;
+                cur.jend = min((jb + 1) * q.block_cols, q.cols);
+                if (k != key) {
+                    if (key != ~0ull) atomicMax(reinterpret_cast<unsigned int*>(amax) + key, m);
+                    key = k, m = 0;
+                }
+            }
+            const uint64_t s = b.src + r * b.pitch + c * ss;
+            const uint8_t* word =
+                reinterpret_cast<const uint8_t*>(ring + (uint32_t)(box_virtual(b, r, s) - b.v0) % kBoxRing);
+            m = max(m, ring_abs_bits(word, (uint32_t)s & 15u, st));
+            ++cur.j;
+            if (++c == welems) c = 0, ++r, seek = true;
+        }
+    }
+    // lanes that end in one block: a segmented max, every merged value from a lane of the same key
+#pragma unroll
+    for (int k = 1; k < 32; k <<= 1) {
+        const uint32_t om = __shfl_down_sync(0xffffffffu, m, k);
+        const uint64_t ok = __shfl_down_sync(0xffffffffu, key, k);
+        if (lane + k < 32 && ok == key) m = max(m, om);
+    }
+    const uint64_t before = __shfl_up_sync(0xffffffffu, key, 1);
+    if (key != ~0ull && (lane == 0 || before != key)) atomicMax(reinterpret_cast<unsigned int*>(amax) + key, m);
+}
+
+__global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
+    fp8_amax_boxes_kernel(const QuantTile* __restrict__ tiles, uint64_t ntiles, const uint8_t* __restrict__ src) {
+    __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
+    const uint32_t lane = threadIdx.x & 31u;
+    uint4* ring = rings[threadIdx.x >> 5];
+    const uint4* words = reinterpret_cast<const uint4*>(src);
+    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
+    for (uint64_t k = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; k < ntiles; k += nwarps) {
+        const QuantTile t = tiles[k];
+        box_tile_steps(t.cast.box, words, ring, lane, [&](uint64_t from, uint64_t upto) {
+            amax_words_out(t.cast.box, t.cast.src_type, t.q, ring, from, upto, lane);
+        });
+    }
+}
+
+// Destination words of the box (one piece at device address `dev`, one byte per element) whose elements have packed
+// source bytes in [from, upto) (clipped to [b.dlo, b.dhi)) and whose last element's source lies before `upto`.
+__device__ __forceinline__ void quant_words_out(const BoxTile& b, uint32_t st, const PieceScale& q, uint64_t dev,
+                                                const uint4* ring, uint64_t from, uint64_t upto, uint32_t lane) {
+    const uint32_t ss = dt_bytes(st);
+    const uint64_t qhi = b.dhi / ss, lo = from / ss, hi = upto / ss;
+    if (lo >= hi) return;
+    const uint64_t qa = dev + b.dlo / ss, qe = dev + qhi, ha = dev + hi, welems = b.width / ss;
+    // a word whose elements go on past `hi` waits for the next step
+    const uint64_t w1 = hi < qhi ? ha >> 4 : ((ha - 1) >> 4) + 1;
+    for (uint64_t w = ((dev + lo) >> 4) + lane; w < w1; w += 32) {
+        const uint64_t ws = w * 16, aa = max(ws, qa), ea = min(ws + 16, qe);
+        const uint32_t jlo = (uint32_t)(aa - ws), jhi = (uint32_t)(ea - ws);
+        const uint64_t e = aa - dev;  // the word's first element, counted in the box's packed run
+        uint64_t r = e / welems, c = e % welems;
+        QuantCursor cur;
+        uint4 v;
+        if (jhi - jlo == 16 && c + 16 <= welems) {
+            const uint64_t s = b.src + r * b.pitch + c * ss;
+            const uint32_t slot = (uint32_t)(box_virtual(b, r, s) - b.v0), sh = (uint32_t)s & 15u;
+            float x[16];
+            if (st == kDtF32) {  // 64 source bytes
+                uint4 wd[5];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wd[k] = ring[(slot + k) % kBoxRing];
+                wd[4] = sh ? ring[(slot + 4) % kBoxRing] : wd[3];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint4 u = sh ? shift_bytes(wd[k], wd[k + 1], sh) : wd[k];
+                    x[4 * k] = __uint_as_float(u.x), x[4 * k + 1] = __uint_as_float(u.y);
+                    x[4 * k + 2] = __uint_as_float(u.z), x[4 * k + 3] = __uint_as_float(u.w);
+                }
+            } else {  // 32
+                const uint4 w0 = ring[slot % kBoxRing], w1 = ring[(slot + 1) % kBoxRing];
+                const uint4 w2 = sh ? ring[(slot + 2) % kBoxRing] : w1;
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                    const uint4 u = sh ? shift_bytes(k ? w1 : w0, k ? w2 : w1, sh) : (k ? w1 : w0);
+                    const float2 p0 = widen_pair(u.x, st), p1 = widen_pair(u.y, st), p2 = widen_pair(u.z, st),
+                                 p3 = widen_pair(u.w, st);
+                    x[8 * k] = p0.x, x[8 * k + 1] = p0.y, x[8 * k + 2] = p1.x, x[8 * k + 3] = p1.y;
+                    x[8 * k + 4] = p2.x, x[8 * k + 5] = p2.y, x[8 * k + 6] = p3.x, x[8 * k + 7] = p3.y;
+                }
+            }
+            quant_seek(q, q.first_elem + r * (b.pitch / ss) + c, cur);
+            uint32_t out[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float y0 = __fmul_rn(x[4 * k], quant_next(q, cur)), y1 = __fmul_rn(x[4 * k + 1], quant_next(q, cur));
+                const float y2 = __fmul_rn(x[4 * k + 2], quant_next(q, cur)),
+                            y3 = __fmul_rn(x[4 * k + 3], quant_next(q, cur));
+                out[k] = e4m3_pair(y0, y1) | e4m3_pair(y2, y3) << 16;
+            }
+            v = make_uint4(out[0], out[1], out[2], out[3]);
+        } else {
+            uint64_t y[2] = {0, 0};  // the codes, element k at byte k
+            bool seek = true;
+#pragma unroll 1
+            for (uint32_t j = jlo; j < jhi; ++j) {
+                const uint64_t s = b.src + r * b.pitch + c * ss;
+                const uint8_t* word =
+                    reinterpret_cast<const uint8_t*>(ring + (uint32_t)(box_virtual(b, r, s) - b.v0) % kBoxRing);
+                const uint32_t x = ss == 4 ? *reinterpret_cast<const uint32_t*>(word + (s & 15u))
+                                           : (uint32_t)*reinterpret_cast<const uint16_t*>(word + (s & 15u));
+                if (seek) quant_seek(q, q.first_elem + r * (b.pitch / ss) + c, cur), seek = false;
+                const uint64_t code = e4m3_pair(__fmul_rn(widen_one(x, st), quant_next(q, cur)), 0.f) & 0xffu;
+                if (j < 8) y[0] |= code << (8 * j);
+                else y[1] |= code << (8 * (j - 8));
+                if (++c == welems) c = 0, ++r, seek = true;
+            }
+            v = make_uint4((uint32_t)y[0], (uint32_t)(y[0] >> 32), (uint32_t)y[1], (uint32_t)(y[1] >> 32));
+        }
+        store_bytes(reinterpret_cast<uint8_t*>(ws), v, jlo, jhi);
+    }
+}
+
+__global__ void __launch_bounds__(kStageThreads, kBoxCtasPerSm)
+    load_quant_boxes_kernel(const QuantTile* __restrict__ tiles, uint64_t ntiles, const RangePiece* __restrict__ pieces,
+                            const uint8_t* __restrict__ src) {
+    __shared__ uint4 rings[kStageThreads / 32][kBoxRing];
+    const uint32_t lane = threadIdx.x & 31u;
+    uint4* ring = rings[threadIdx.x >> 5];
+    const uint4* words = reinterpret_cast<const uint4*>(src);
+    const uint64_t nwarps = (uint64_t)gridDim.x * (kStageThreads / 32);
+    for (uint64_t k = (uint64_t)(threadIdx.x >> 5) * gridDim.x + blockIdx.x; k < ntiles; k += nwarps) {
+        const QuantTile t = tiles[k];
+        const uint64_t dev = pieces[t.cast.box.first_piece].dev;
+        box_tile_steps(t.cast.box, words, ring, lane, [&](uint64_t from, uint64_t upto) {
+            quant_words_out(t.cast.box, t.cast.src_type, t.q, dev, ring, from, upto, lane);
+        });
+    }
+}
+
 }  // namespace
 
 int launch_load_boxes(const CastTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src, cudaStream_t st) {
@@ -984,6 +1168,30 @@ int launch_fp8_block_scales(const ScaleJob* jobs, uint32_t njobs, uint64_t ntile
     const uint64_t ctas = (nblocks + kScaleThreads - 1) / kScaleThreads;
     fp8_finalize_kernel<<<(int)(ctas < cap ? ctas : cap), kScaleThreads, 0, st>>>(jobs, njobs, nblocks);
     return 2;
+}
+
+int launch_fp8_finalize(const ScaleJob* jobs, uint32_t njobs, uint64_t nblocks, cudaStream_t st) {
+    if (!nblocks) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * 8, ctas = (nblocks + kScaleThreads - 1) / kScaleThreads;
+    fp8_finalize_kernel<<<(int)(ctas < cap ? ctas : cap), kScaleThreads, 0, st>>>(jobs, njobs, nblocks);
+    return 1;
+}
+
+int launch_fp8_amax_boxes(const QuantTile* tiles, uint64_t ntiles, const void* src, cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
+    fp8_amax_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
+        tiles, ntiles, static_cast<const uint8_t*>(src));
+    return 1;
+}
+
+int launch_load_quant_boxes(const QuantTile* tiles, uint64_t ntiles, const RangePiece* pieces, const void* src,
+                            cudaStream_t st) {
+    if (!ntiles) return 0;
+    const uint64_t cap = (uint64_t)device_sm_count() * kBoxCtasPerSm;
+    load_quant_boxes_kernel<<<(int)(ntiles < cap ? ntiles : cap), kStageThreads, 0, st>>>(
+        tiles, ntiles, pieces, static_cast<const uint8_t*>(src));
+    return 1;
 }
 
 }  // namespace b200h

@@ -412,9 +412,9 @@ def load_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> L
     return _load_boxes(ctx, "copy_boxes_from_host", sources, boxes, src)
 
 
-def _load_boxes(ctx, entry: str, sources: list[_TensorBytes], boxes, src: np.ndarray) -> Loaded:
-    """The body of ``load_boxes`` and ``load_cast_boxes``: ONE call of ``ctx``'s ``entry`` with the checked boxes, on
-    the first file's stream, ordered as ``load_ranges``."""
+def _load_boxes(ctx, entry: str, sources: list[_TensorBytes], boxes, src: np.ndarray, *extra) -> Loaded:
+    """The body of ``load_boxes`` and ``load_cast_boxes``: ONE call of ``ctx``'s ``entry`` with the checked boxes (and
+    ``extra`` after them), on the first file's stream, ordered as ``load_ranges``."""
     if boxes and not sources:
         raise ValueError("boxes without files")
     if not sources:
@@ -423,7 +423,7 @@ def _load_boxes(ctx, entry: str, sources: list[_TensorBytes], boxes, src: np.nda
     lead._after_current()
     ptrs, lens, first = _file_table(sources)
     with lead._on_stream():
-        getattr(ctx, entry)(ptrs, lens, first, boxes, src, lead.stream_handle)
+        getattr(ctx, entry)(ptrs, lens, first, boxes, *extra, src, lead.stream_handle)
     return Loaded(lead._publish())
 
 
@@ -609,6 +609,63 @@ def load_scaled_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=Non
         out.append(tuple(int(x) for x in b[:6]) + (fp8[b[6]], codes[b[7]], s.data_ptr(), codes[s.dtype], s.numel())
                    + tuple(int(x) for x in b[9:]))
     return _load_boxes(ctx, "copy_scaled_boxes_from_host", sources, out, src)
+
+
+def _f32_device(t, what: str):
+    import torch
+
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_contiguous():
+        raise ValueError(f"{what} is a contiguous float32 tensor on the context's device")
+    return t.data_ptr()
+
+
+def _quant_boxes(boxes) -> list:
+    """The ``_lib`` form of ``load_fp8_amax_boxes`` / ``load_quant_boxes`` boxes, checked."""
+    codes = cast_dtypes()
+    if any(len(b) != 13 for b in boxes):
+        raise ValueError("a box is (file, offset, width, rows, src_offset, src_pitch, src_dtype, amax, first_elem, R, "
+                         "C, block_rows, block_cols)")
+    out = []
+    for b in boxes:
+        if b[6] not in codes:
+            raise ValueError(f"quantizing boxes take {', '.join(map(str, codes))}, not {b[6]}")
+        ptr = _f32_device(b[7], "a box's amax")
+        out.append(tuple(int(x) for x in b[:6]) + (codes[b[6]], _lib.DT_F8E4M3, ptr, b[7].numel())
+                   + tuple(int(x) for x in b[8:]))
+    return out
+
+
+def load_fp8_amax_boxes(files: list["DeviceFile"], boxes, src: np.ndarray, ctx=None) -> Loaded:
+    """The first half of quantizing F32 / F16 / BF16 weights to FP8 E4M3 as they arrive in ``src`` (a uint8 array over
+    page-locked memory from ``ctx.host_alloc``): box i = ``(index into files, offset, width, rows, src_offset,
+    src_pitch, src_dtype, amax, first_elem, R, C, block_rows, block_cols)``, ``src_dtype`` one of ``cast_dtypes()``
+    (``width`` and ``src_pitch`` count source bytes).  The element at source byte c of row r of the box is element
+    ``first_elem + (r * src_pitch + c) / itemsize`` of an R x C weight; the bits of its |x| widened to F32 are
+    max-reduced into its block's value of ``amax`` (a contiguous float32 tensor on the context's device of
+    ``ceil(R / block_rows) * ceil(C / block_cols)`` values or more, row-major, zeros before a weight's first box).  The
+    box's destination in its file (one byte per element) is checked as ``load_quant_boxes`` checks it, and not written.
+    ONE ``b200h_fp8_amax_boxes_from_host`` call, ordered exactly as ``load_boxes``."""
+    ctx = ctx or get_context()
+    return _load_boxes(ctx, "fp8_amax_boxes_from_host", [f._src for f in files], _quant_boxes(boxes), src)
+
+
+def load_quant_boxes(files: list["DeviceFile"], boxes, bands, src: np.ndarray, ctx=None) -> Loaded:
+    """The second half: band i = ``(amax, scales, first, count)`` finalizes blocks ``[first, first + count)`` of a
+    weight (``amax`` and ``scales`` contiguous float32 tensors on the context's device: a clamped in place, s = a *
+    RN(1 / 448)), then every element of the boxes (as for ``load_fp8_amax_boxes``, whose every block is finalized by now)
+    is quantized as the FP8 export quantizes it, q = E4M3(RN(x * RN(RN(1 / a) * 448))), and written packed, one byte
+    per element, from byte ``offset`` of its file, into one tensor at any address.  ONE
+    ``b200h_copy_quant_boxes_from_host`` call, ordered exactly as ``load_boxes``."""
+    ctx = ctx or get_context()
+    out = []
+    for b in bands:
+        if len(b) != 4:
+            raise ValueError("a band is (amax, scales, first, count)")
+        a, s = _f32_device(b[0], "a band's amax"), _f32_device(b[1], "a band's scales")
+        if not 0 <= int(b[2]) <= int(b[2]) + int(b[3]) <= min(b[0].numel(), b[1].numel()):
+            raise ValueError(f"band ({int(b[2])}, {int(b[3])}) reaches past its amax or scales")
+        out.append((a + 4 * int(b[2]), s + 4 * int(b[2]), int(b[3])))
+    return _load_boxes(ctx, "copy_quant_boxes_from_host", [f._src for f in files], _quant_boxes(boxes), src, out)
 
 
 # ------------------------------------------------------------------------------------------ safetensors
@@ -1462,5 +1519,5 @@ class DeviceFile(io.RawIOBase):
 safetensors_shards = DeviceFile.safetensors_shards
 
 __all__ = ["DeviceFile", "BOUNCE_BYTES", "Loaded", "SafetensorsShards", "Staged", "hash_parts_many", "load_boxes",
-           "load_cast_boxes", "load_scaled_boxes", "load_ranges", "parse_size_to_int", "safetensors_layout", "safetensors_shards",
+           "load_cast_boxes", "load_fp8_amax_boxes", "load_quant_boxes", "load_scaled_boxes", "load_ranges", "parse_size_to_int", "safetensors_layout", "safetensors_shards",
            "stage_ranges"]

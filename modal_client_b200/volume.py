@@ -42,7 +42,8 @@ from ._logging import logger
 from .async_utils import bounded_map, bounded_map_ordered, gather_cancel_on_error, retry
 from .blob_utils import FileUploadSpec, FileUploadSpec2, _ByteBudget
 from .device_file import (BOUNCE_BYTES, DeviceFile, _st_dtypes, cast_dtypes, cast_targets, fp8_dtypes, load_boxes,
-                          load_cast_boxes, load_ranges, load_scaled_boxes, stage_ranges)
+                          load_cast_boxes, load_fp8_amax_boxes, load_quant_boxes, load_ranges, load_scaled_boxes,
+                          stage_ranges)
 from .exception import ExecutionError, ServiceError
 from .http_utils import ClientSessionRegistry
 
@@ -550,9 +551,10 @@ async def _load_in_waves(slices, load, staging_bytes: int, concurrency: int | No
     every block goes to its own ``BLOCK_SIZE`` slot of a page-locked buffer (``ctx.host_alloc``) of two halves, a wave
     per half; when a wave is complete,
     ``load(wave, at, buf, ctx)`` -- the wave's slices, their offsets in the buffer, the buffer and the context -- makes
-    its one copy (``load_ranges`` or ``load_boxes``) and returns the ``Loaded``.  A half is refilled only after its
-    previous copy has read it, so ``load`` may still read the previous wave's slots; every copy has read the buffer
-    before it is freed, however the call ends."""
+    its one copy (``load_ranges`` or ``load_boxes``) and returns the ``Loaded``, or ``(Loaded, True)`` when its copies
+    also read the previous wave's slots (a quantized band carried over from there).  A half is refilled only after
+    every copy that reads it has read it, so ``load`` may still read the previous wave's slots; every copy has read the
+    buffer before it is freed, however the call ends."""
     BS = blob_utils.BLOCK_SIZE
     per_half = staging_bytes // 2 // BS  # block slots per half (every slot starts at a multiple of BLOCK_SIZE)
     semaphore = asyncio.Semaphore(concurrency or os.cpu_count() or 1)
@@ -572,7 +574,10 @@ async def _load_in_waves(slices, load, staging_bytes: int, concurrency: int | No
                 progress_cb(advance=m)
 
             await gather_cancel_on_error(*[fetch(url, m, a) for (url, _, m, *_), a in zip(wave, at)])
-            loaded[half] = load(wave, at, buf, ctx)
+            got = load(wave, at, buf, ctx)
+            loaded[half], carried = got if isinstance(got, tuple) else (got, False)
+            if carried:  # the copy also read the previous wave's slots: that half is refilled only after it too
+                loaded[1 - half] = loaded[half]
     finally:
         for pending in loaded:  # the copies must have read the buffer before it is freed
             if pending is not None:
@@ -671,8 +676,11 @@ async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
     ``dst``: ONE ``VolumeGetFile2`` call per file that has a touched block, over its bytes [start, end), all made
     concurrently, then exactly the blocks that hold a byte of a run, once each, into the page-locked waves of ONE
     ``_load_in_waves``, so a wave may hold the blocks of several files.  Each complete wave makes at most one
-    ``load_boxes`` call (the unconverted runs; one also when nothing converts), at most one ``load_cast_boxes`` call
-    and at most one ``load_scaled_boxes`` call (the dequantized runs), all on one stream, over every file's ``dst``:
+    ``load_boxes`` call (the unconverted runs; one also when nothing converts), at most one ``load_cast_boxes`` call,
+    at most one ``load_scaled_boxes`` call (the dequantized runs), and for the runs of weights quantized to FP8 (a
+    ``_Quant``) at most one ``load_fp8_amax_boxes`` call (every box of the wave) and one ``load_quant_boxes`` call (the
+    bands the wave completes, with the boxes of their first part that landed in the previous wave, whose half is then
+    not refilled before this copy has read it), all on one stream, over every file's ``dst``:
     every run is cut into boxes, split where the staging stops being contiguous, at a wave's edge, a skipped block or
     the next file.  A converted run's packed offsets count target bytes."""
     BS = blob_utils.BLOCK_SIZE
@@ -689,6 +697,7 @@ async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
 
     def load(wave, at, buf, ctx):
         plain, cast, scaled, k = [], [], [], 0
+        landed = {}  # _Quant -> [(file offset, end, staging offset, file, weight's packed offset)] of this wave
         while k < len(wave):  # a stretch: blocks of one file, adjacent in the file and in the buffer
             e, i = k + 1, wave[k][3]
             while e < len(wave) and wave[e][3] == i and wave[e][1] == wave[e - 1][1] + wave[e - 1][2] and \
@@ -702,24 +711,43 @@ async def _load_runs(client, volume_id: str, files, staging_bytes: int) -> None:
                         plain.append((i, d + b[0], *b[1:]))
                     elif len(conv) == 2:  # the box's offset in the run, in source bytes, to target bytes
                         cast.append((i, d + b[0] // conv[0].itemsize * conv[1].itemsize, *b[1:], *conv))
+                    elif isinstance(conv[2], _Quant):  # a whole weight's run: one row per box
+                        lo = s0 + b[3] - at[k]
+                        landed.setdefault(conv[2], []).append((lo, lo + b[1], b[3], i, d))
                     else:  # one-byte elements; the box's first element in the weight, from its file offset
                         q = conv[2]
                         scaled.append((i, d + b[0] * conv[1].itemsize, *b[1:], conv[0], conv[1], q.scales,
                                        s0 + b[3] - at[k] - q.start, q.rows, q.cols, q.block_rows, q.block_cols))
             k = e
-        loaded = load_boxes(dsts, plain, buf, ctx=ctx) if plain or not (cast or scaled) else None
+        amax, quant, bands, carried = [], [], [], False
+        for q, now in landed.items():  # every box's amax; then the bands this wave completes, their carried part too
+            amax += [q.box(*x) for x in now]
+            top = max(hi for _, hi, *_ in now)
+            done = q.nbands if top == q.end else (top - q.start) // q.band
+            edge = min(q.start + done * q.band, q.end)
+            if done > q.done:
+                quant += [q.box(*x) for x in _clip_landed(q.pending + now, q.start + q.done * q.band, edge)]
+                bands.append((q.amax, q.scales, q.done * q.grid_cols, (done - q.done) * q.grid_cols))
+                carried = carried or bool(q.pending)
+                q.done = done
+            q.pending = _clip_landed(q.pending + now, edge, q.end)
+        loaded = load_boxes(dsts, plain, buf, ctx=ctx) if plain or not (cast or scaled or amax) else None
         if cast:  # on the same stream as the plain boxes: its completion implies theirs
             loaded = load_cast_boxes(dsts, cast, buf, ctx=ctx)
         if scaled:  # the same stream again
             loaded = load_scaled_boxes(dsts, scaled, buf, ctx=ctx)
-        return loaded
+        if amax:  # the same stream: the amax of a wave is in before its bands are finalized
+            loaded = load_fp8_amax_boxes(dsts, amax, buf, ctx=ctx)
+        if bands:
+            loaded = load_quant_boxes(dsts, quant, bands, buf, ctx=ctx)
+        return (loaded, True) if carried else loaded
 
     await _load_in_waves(slices, load, staging_bytes, None, lambda **_: None)
 
 
 async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping | None = None, dtype=None,
-                           scales: Mapping | None = None, scale_block=(128, 128),
-                           staging_bytes: int = 256 << 20) -> dict:
+                           scales: Mapping | None = None, scale_block=(128, 128), fp8=None,
+                           scale_suffix: str = "_scale_inv", staging_bytes: int = 256 << 20) -> dict:
     """The safetensors file at ``path`` as ``{name: tensor}`` on the context's device, equal to what
     ``safetensors.torch.load`` gives for the file's bytes (same names, dtypes, shapes and values; keys in data order).
 
@@ -748,15 +776,28 @@ async def read_safetensors(client, volume_id: str, path: str, *, into: Mapping |
     ``_scale_targets`` lists every problem in one ``ValueError`` before any data GET.  The scales load first into
     temporary tensors (one ``_load_runs`` over their blocks), then everything else (a second one, whose waves make at
     most one ``load_boxes``, one ``load_cast_boxes`` and one ``load_scaled_boxes`` call); HBM holds the results and the
-    scales, never the FP8 image, and the scales are freed on return."""
+    scales, never the FP8 image, and the scales are freed on return.
+
+    ``fp8=names`` quantizes the named weights (non-empty 2-D F32 / F16 / BF16 tensors) to ``torch.float8_e4m3fn`` as
+    they land, in ``scale_block`` blocks as above, and returns each one's F32 scale tensor ([ceil(R / rows),
+    ceil(C / columns)]) as ``name + scale_suffix``, right after the weight: both bit for bit what
+    ``DeviceFile.safetensors({...}, fp8=names, scale_block=..., scale_suffix=...)`` stores for it (DESIGN §5.20).
+    Every other tensor is read as without ``fp8``, converted by ``dtype`` if given.  With ``into=`` a weight needs a
+    contiguous float8_e4m3fn tensor of its shape and its scale name an F32 tensor of the grid's shape.  The blocks,
+    the requests and the waves are those of a read with ``dtype``; each wave reduces the amax of the weights' boxes
+    into one temporary F32 array (one value per block), then finalizes and quantizes every band (the block_rows rows of
+    one block row) whose last byte has landed, so HBM holds only the results, their scales and that array.  A band must
+    touch at most ``staging_bytes // 2 // BLOCK_SIZE + 1`` blocks.  ``fp8`` with ``scales``, a name that is not such a
+    weight or is given twice, a name a ``dtype`` mapping names, a scale name that is already a tensor and a band too
+    large for ``staging_bytes`` are refused, every problem in one ``ValueError`` before any data GET."""
     ctx = blob_utils.get_context()
     size, n, _, entries = await _read_safetensors_header(client, volume_id, path)
-    if scales:
+    if scales or fp8 is not None:
         if staging_bytes < 2 * blob_utils.BLOCK_SIZE:
             raise ValueError(f"staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), got "
                              f"{staging_bytes}")
         return await _read_shards(client, volume_id, path, [(path, n, entries)], None, into, dtype, scales,
-                                  scale_block, staging_bytes, ctx)
+                                  scale_block, staging_bytes, ctx, fp8, scale_suffix)
     targets = cast_targets(path, dtype, entries, 8 + n)
     if targets and staging_bytes < 2 * blob_utils.BLOCK_SIZE:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * blob_utils.BLOCK_SIZE} bytes), got {staging_bytes}")
@@ -1037,7 +1078,8 @@ async def read_safetensors_index(client, volume_id: str, index_path: str):
 
 async def read_safetensors_sharded(client, volume_id: str, index_path: str, *, select: Mapping | None = None,
                                    into: Mapping | None = None, dtype=None, scales: Mapping | None = None,
-                                   scale_block=(128, 128), staging_bytes: int = 256 << 20) -> dict:
+                                   scale_block=(128, 128), fp8=None, scale_suffix: str = "_scale_inv",
+                                   staging_bytes: int = 256 << 20) -> dict:
     """A sharded safetensors checkpoint (the index at ``index_path``, read as ``read_safetensors_index`` reads it) as
     ``{name: tensor}`` on the context's device: what merging ``read_safetensors`` over every shard returns, keys in
     shard order, then data order.  With ``select={name: index}`` it is what ``read_safetensors_slices`` returns for
@@ -1052,14 +1094,16 @@ async def read_safetensors_sharded(client, volume_id: str, index_path: str, *, s
     ``load_boxes`` and one ``load_cast_boxes`` call (and with ``scales=`` one ``load_scaled_boxes`` call), over a
     ``DeviceFile`` per shard.  Of HBM, the call allocates only the results and the copies' small tables (and with
     ``scales=`` the scales, freed on return).  Ordering and partial content on return and on error are as for
-    ``read_safetensors``."""
+    ``read_safetensors``.  ``fp8=`` and ``scale_suffix=`` quantize weights as ``read_safetensors`` does, each scale
+    right after its weight; a band never spans shards, and each wave adds at most one ``load_fp8_amax_boxes`` and one
+    ``load_quant_boxes`` call."""
     BS = blob_utils.BLOCK_SIZE
     if staging_bytes < 2 * BS:
         raise ValueError(f"staging_bytes must hold two blocks ({2 * BS} bytes), got {staging_bytes}")
     ctx = blob_utils.get_context()
     _, shards = await _read_index(client, volume_id, index_path)
     return await _read_shards(client, volume_id, index_path, shards, select, into, dtype, scales, scale_block,
-                              staging_bytes, ctx)
+                              staging_bytes, ctx, fp8, scale_suffix)
 
 
 class _Dequant:
@@ -1069,6 +1113,105 @@ class _Dequant:
     def __init__(self, scales, start: int, rows: int, cols: int, block_rows: int, block_cols: int):
         self.scales, self.start, self.rows, self.cols = scales, start, rows, cols
         self.block_rows, self.block_cols = block_rows, block_cols
+
+
+class _Quant:
+    """How the boxes of one weight are quantized to FP8 E4M3 as they land: its a (``amax``, a view of the read's one
+    amax array) and its result ``scales``, the file offset of its element 0, its shape, its block (a block of the whole
+    dimension is the dimension) and its source element size.  A band -- the block_rows rows of one block row, one
+    contiguous byte range of the file -- is quantized once all of it has landed: ``done`` bands are so far, and
+    ``pending`` holds the landed boxes of the next one (``(file offset, end, staging offset, file, weight's packed
+    offset)``), which all lie in the previous wave's half."""
+
+    def __init__(self, amax, scales, start: int, rows: int, cols: int, block_rows: int, block_cols: int,
+                 src_dtype):
+        self.amax, self.scales, self.start, self.rows, self.cols = amax, scales, start, rows, cols
+        self.block_rows, self.block_cols, self.src_dtype = block_rows, block_cols, src_dtype
+        self.itemsize = src_dtype.itemsize
+        self.end, self.band = start + rows * cols * self.itemsize, block_rows * cols * self.itemsize
+        self.nbands, self.grid_cols = -(-rows // block_rows), -(-cols // block_cols)
+        self.done, self.pending = 0, []
+
+    def box(self, lo: int, hi: int, at: int, i: int, d: int):
+        """The ``load_fp8_amax_boxes`` / ``load_quant_boxes`` box of file bytes [lo, hi) staged at ``at``."""
+        e = (lo - self.start) // self.itemsize
+        return (i, d + e, hi - lo, 1, at, hi - lo, self.src_dtype, self.amax, e, self.rows, self.cols,
+                self.block_rows, self.block_cols)
+
+
+def _clip_landed(boxes, lo: int, hi: int) -> list:
+    """The parts of ``_Quant`` landed boxes that lie in file bytes [lo, hi)."""
+    return [(max(a, lo), min(b, hi), at + max(a, lo) - a, i, d) for a, b, at, i, d in boxes if max(a, lo) < min(b, hi)]
+
+
+def _band_blocks(start: int, rows: int, cols: int, block_rows: int, itemsize: int, BS: int) -> int:
+    """The most staging blocks one band of a weight (file offset ``start``) touches."""
+    band, end = block_rows * cols * itemsize, start + rows * cols * itemsize
+    lo = start + band * np.arange(-(-rows // block_rows), dtype=np.int64)
+    hi = np.minimum(lo + band, end)
+    return int(((hi - 1) // BS - lo // BS + 1).max())
+
+
+def _fp8_load_plan(there: str, tensors: Mapping, starts: Mapping, fp8, scale_block, scale_suffix, dtype, scales,
+                   select, staging_bytes: int, problems: list) -> dict:
+    """{weight: scale name}, in the order of ``tensors`` ({name: (torch dtype, shape)}, ``there`` names where they are;
+    ``starts``: their file offsets),
+    of the weights ``fp8`` quantizes on load; every problem is appended to ``problems``: ``scales`` or ``select`` given
+    too, a bad ``scale_block`` or ``scale_suffix``, unknown or repeated names, weights that are not non-empty 2-D
+    F32 / F16 / BF16 tensors, a name that a ``dtype`` mapping names too, a scale name that is already a tensor, and a
+    weight whose band touches more staging blocks than a wave can carry into the next (``per_half + 1``)."""
+    if scales:
+        problems.append("fp8 cannot be combined with scales (the FP8 weights of a file are dequantized, not quantized)")
+    if select is not None:
+        problems.append("fp8 does not take select= (slices are not quantized on load)")
+    if isinstance(fp8, str):
+        fp8 = None  # a single name is a common slip: refused, not read as its characters
+    try:
+        names = list(fp8)
+    except TypeError:
+        problems.append("fp8 must be an iterable of tensor names")
+        return {}
+    good_block = isinstance(scale_block, (tuple, list)) and len(scale_block) == 2 and all(
+        b is None or (isinstance(b, int) and not isinstance(b, bool) and b >= 1) for b in scale_block)
+    if not good_block:
+        problems.append(f"scale_block {scale_block!r} must be (rows, columns), each an int >= 1 or None (the whole "
+                        f"dimension)")
+    if not isinstance(scale_suffix, str):
+        problems.append(f"scale_suffix must be a str, got {scale_suffix!r}")
+        scale_suffix = None
+    want, codes = set(), cast_dtypes()
+    for n in names:
+        if n in want:
+            problems.append(f"{n!r} is in fp8 twice")
+        elif not isinstance(n, str) or n not in tensors:
+            problems.append(f"{n!r} is in fp8 but not {there}")
+        else:
+            want.add(n)
+    BS = blob_utils.BLOCK_SIZE
+    per_half = staging_bytes // 2 // BS
+    plan = {}
+    for n, (dt, shape) in tensors.items():
+        if n not in want:
+            continue
+        if len(shape) != 2 or 0 in shape:
+            problems.append(f"{n!r} has shape {list(shape)}; fp8 quantizes non-empty 2-D weights")
+        elif dt not in codes:
+            problems.append(f"{n!r} is {_st_dtypes()[dt][0]}; only F32, F16 and BF16 weights quantize")
+        elif good_block:
+            R, C = shape
+            br = min(R, scale_block[0] or R)
+            need = _band_blocks(starts[n], R, C, br, dt.itemsize, BS)
+            if need > per_half + 1:
+                problems.append(f"{n!r}: one band of {br} rows ({br * C * dt.itemsize} bytes) touches {need} staging "
+                                f"blocks, and staging_bytes={staging_bytes} carries {per_half + 1}; "
+                                f"staging_bytes={2 * max(1, need - 1) * BS} would hold it")
+        if isinstance(dtype, Mapping) and n in dtype:
+            problems.append(f"{n!r} is in both fp8 and dtype")
+        if scale_suffix is not None:
+            if n + scale_suffix in tensors:
+                problems.append(f"the scale of {n!r}, {n + scale_suffix!r}, is already a tensor of the checkpoint")
+            plan[n] = n + scale_suffix
+    return plan
 
 
 def _scale_grid(shape, scale_block):
@@ -1149,13 +1292,46 @@ def _scale_targets(where: str, there: str, dtype, scales: Mapping, scale_block, 
 
 
 async def _read_shards(client, volume_id: str, where: str, shards, select, into, dtype, scales, scale_block,
-                       staging_bytes: int, ctx) -> dict:
+                       staging_bytes: int, ctx, fp8=None, scale_suffix: str = "_scale_inv") -> dict:
     """The body of ``read_safetensors_sharded`` over ``shards`` (``[(path, header length, entries)]``; also
-    ``read_safetensors`` and ``read_safetensors_slices`` with ``scales=``, over one shard).  With ``scales``, the scales
-    load first, unconverted, into temporary tensors (one ``_load_runs``: a scale may sit in a later wave, or another
-    shard, than its weight), then everything else (a second ``_load_runs``)."""
+    ``read_safetensors`` and ``read_safetensors_slices`` with ``scales=``, and ``read_safetensors`` with ``fp8=``, over
+    one shard).  With ``scales``, the scales load first, unconverted, into temporary tensors (one ``_load_runs``: a
+    scale may sit in a later wave, or another shard, than its weight), then everything else (a second ``_load_runs``).
+    With ``fp8``, the weights it names are quantized in the one ``_load_runs`` (``_Quant``), their a in one temporary
+    array, zeroed once and freed on return."""
+    import torch
+
     by_name = {e[0]: (k, 8 + n + e[3], e) for k, (_, n, entries) in enumerate(shards) for e in entries}
-    scaled, consumed = {}, set()
+    scaled, consumed, quant = {}, set(), {}
+    if fp8 is not None:
+        problems = []
+        there = "in the checkpoint" if len(shards) > 1 else "in the file"
+        quant = _fp8_load_plan(there, {name: (e[1], e[2]) for name, (_, _, e) in by_name.items()},
+                               {name: at for name, (_, at, _) in by_name.items()}, fp8, scale_block, scale_suffix,
+                               dtype, scales, select, staging_bytes, problems)
+        rest = {name: t for name, t in dtype.items() if name not in quant} if isinstance(dtype, Mapping) else dtype
+        targets = {}
+        try:
+            targets = cast_targets(where, rest, [(name, e[1], e[2], at, None) for name, (_, at, e) in by_name.items()
+                                                 if name not in quant], 0)
+        except ValueError as exc:
+            problems.append(str(exc))
+        if into is not None:  # its mismatches go in the same error (the weights as E4M3, their scales as F32 grids)
+            grids = {}
+            for w, sc in quant.items():
+                try:
+                    grids[sc] = list(_scale_grid(by_name[w][2][2], scale_block))
+                except (TypeError, ValueError, ZeroDivisionError):  # a bad scale_block, already reported
+                    pass
+            want = [(name, torch.float8_e4m3fn if name in quant else targets.get(name, e[1]), e[2], 0, 0)
+                    for name, (_, _, e) in by_name.items()] + [(sc, torch.float32, g, 0, 0) for sc, g in grids.items()]
+            try:
+                _check_into(into, want, ctx, stored={name: e[1] for name, (_, _, e) in by_name.items()
+                                                     if name in quant or name in targets})
+            except ValueError as exc:
+                problems.append(str(exc))
+        if problems:
+            raise ValueError(f"{where}: fp8: " + "; ".join(problems))
     if scales:
         there = "in the checkpoint" if len(shards) > 1 else "in the file"
         scaled = _scale_targets(where, there, dtype, scales, scale_block,
@@ -1179,15 +1355,30 @@ async def _read_shards(client, volume_id: str, where: str, shards, select, into,
     rest = dtype
     if scaled and isinstance(dtype, Mapping):
         rest = {name: t for name, t in dtype.items() if name not in scaled}
-    targets = cast_targets(where, rest, [(name, dt, shape, by_name[name][1], None)
-                                         for _, name, dt, shape, _ in plans if name not in scaled], 0, sliced=sliced)
+    if fp8 is None:
+        targets = cast_targets(where, rest, [(name, dt, shape, by_name[name][1], None)
+                                             for _, name, dt, shape, _ in plans if name not in scaled], 0, sliced=sliced)
     targets.update(scaled)
+    targets.update({name: torch.float8_e4m3fn for name in quant})
+    grids = {sc: list(_scale_grid(by_name[w][2][2], scale_block)) for w, sc in quant.items()}
     if into is not None:
-        _check_into(into, [(name, targets.get(name, dt), shape, 0, 0) for _, name, dt, shape, _ in plans], ctx,
-                    sliced=sliced, stored={name: dt for _, name, dt, *_ in plans if name in targets})
+        if fp8 is None:  # with fp8, checked above
+            _check_into(into, [(name, targets.get(name, dt), shape, 0, 0) for _, name, dt, shape, _ in plans], ctx,
+                        sliced=sliced, stored={name: dt for _, name, dt, *_ in plans if name in targets})
         tensors = [into[name] for _, name, *_ in plans]
+        qscales = {sc: into[sc] for sc in quant.values()}
     else:
         tensors = [DeviceFile._Source._new_tensor(shape, targets.get(name, dt), ctx) for _, name, dt, shape, _ in plans]
+        qscales = {sc: DeviceFile._Source._new_tensor(grids[sc], torch.float32, ctx) for sc in quant.values()}
+    qs = {}
+    if quant:  # every weight's a, in one array zeroed with one memset
+        amax = DeviceFile._Source._new_tensor([sum(g[0] * g[1] for g in grids.values())], torch.float32, ctx).zero_()
+        at = 0
+        for w, sc in quant.items():
+            (R, C), (br, bc), n = by_name[w][2][2], scale_block, grids[sc][0] * grids[sc][1]
+            qs[w] = _Quant(amax[at : at + n], qscales[sc].view(-1), by_name[w][1], R, C, min(R, br or R),
+                           min(C, bc or C), by_name[w][2][1])
+            at += n
     dequant = {}
     if scaled:  # the scales of the weights with a byte to load, whole and unconverted, into temporary tensors
         needed = sorted({scales[name] for _, name, _, _, rs in plans if name in scaled and rs},
@@ -1218,7 +1409,8 @@ async def _read_shards(client, volume_id: str, where: str, shards, select, into,
     for (k, name, dt, _, rs), t in zip(plans, tensors):
         ts, runs, base = per.setdefault(k, [[], [], 0])
         dest = base
-        conv = (dt, t.dtype, dequant[name]) if name in dequant else (dt, t.dtype) if name in targets else None
+        conv = (dt, t.dtype, dequant[name]) if name in dequant else (dt, t.dtype, qs[name]) if name in qs else \
+            (dt, t.dtype) if name in targets else None
         for run in rs:
             runs.append((run, dest, conv))
             dest += run[1] * run[3] // dt.itemsize * t.element_size()
@@ -1232,7 +1424,12 @@ async def _read_shards(client, volume_id: str, where: str, shards, select, into,
             end = max(F + (R - 1) * P + W for (F, W, P, R), _, _ in runs)
             files.append((shards[k][0], runs, DeviceFile._over(DeviceFile._Source(ts, BOUNCE_BYTES)), start, end))
     await _load_runs(client, volume_id, files, staging_bytes)
-    return {name: t for (_, name, *_), t in zip(plans, tensors)}
+    out = {}
+    for (_, name, *_), t in zip(plans, tensors):
+        out[name] = t
+        if name in quant:
+            out[quant[name]] = qscales[quant[name]]
+    return out
 
 
 _ZIP_TAIL = 1 << 16  # the end of a torch.save file read first: its end records and, usually, its central directory
